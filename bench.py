@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — carved-attention hot path at the BASELINE.json workload.
+"""bench.py — carved-attention hot path at the HunyuanVideo 720p workload.
 
 One "step" = one call of the AttenCarve operator (block pooling of q and k, block
 scoring/selection, block-sparse attention incl. the dense text rows) on one DiT layer's
@@ -8,6 +8,7 @@ q,k,v at the HunyuanVideo 720x1280x125f shape: q,k,v [1, 115456, 24, 128] bf16
 p_remain 0.3, text_amp 0, 26-neighbour adjacency of the 32x45x80 gilbert curve).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--drop 0.7]
+                    [--dump-outputs DIR]
 
 N>1 (torchrun): Ulysses — image tokens sharded over ranks outside the operator, all-to-all to
 (all tokens x H/N heads) inside (jenga_b200.ulysses), strong scaling of the same layer.
@@ -22,6 +23,11 @@ roofline         attention kernel alone (CUDA events on its stream), vs the meas
 cpu_baseline     the oracle port (oracle/attention_oracle.py) on the host cores, bounded sample.
 --impl reference the reference's CPU-runnable path for this operator (torch SDPA with the
                  expanded block mask, hyvideo/modules/attenion.py:102-107) on a bounded sample.
+--dump-outputs   after the timed steps, DIR/out.npy = float32 rows of the last timed step's result
+                 (a fixed, seeded sample of token rows, all heads; DIR/out_rows.npy their indices), so
+                 that two builds can be compared output for output on identical seeded inputs.  With
+                 N>1 every rank writes the rows of its own shard, DIR/out.rank<r>.npy and
+                 DIR/out_rows.rank<r>.npy, within an equal share of the size budget.
 """
 from __future__ import annotations
 
@@ -57,17 +63,17 @@ def workload(name: str, drop: float):
                     grid=(21, 30, 52), sliced=1, heads=12, text_tokens=0, text_valid=0,
                     text_blocks=0, p_remain=0.9, drop=0.5, variant="wan", text_amp=0.0,
                     first_frame=(21 * 30 * 52 + 127) // 128 // 21, layers=30, computed_steps=60)
-    if name == "hy_turbo_s0":  # BASELINE configs[2], stage 0 of Jenga-Turbo: 0.75x latent grid, text_amp on
+    if name == "hy_turbo_s0":  # stage 0 of Jenga-Turbo: 0.75x latent grid, text_amp on
         return dict(name="HunyuanVideo Jenga-Turbo stage 0 layer (grid 32x33x60, q,k,v [1,63616,24,128])",
                     grid=(32, 33, 60), sliced=0, heads=24, text_tokens=256, text_valid=180,
                     text_blocks=2, p_remain=0.3, drop=0.75, variant="hyvideo", text_amp=0.431,
                     first_frame=0, layers=60, computed_steps=12)
-    if name == "hy_i2v":  # BASELINE configs[4] shape: 400 text tokens -> 4 text blocks, ragged S
+    if name == "hy_i2v":  # 400 text tokens -> 4 text blocks, ragged S
         return dict(name="HunyuanVideo-I2V 720x1280x125f layer (q,k,v [1,115600,24,128])",
                     grid=(32, 45, 80), sliced=0, heads=24, text_tokens=400, text_valid=300,
                     text_blocks=4, p_remain=0.3, drop=0.75, variant="hyvideo_i2v", text_amp=0.0,
                     first_frame=0, layers=60, computed_steps=24)
-    if name == "wan14b":  # BASELINE configs[3]
+    if name == "wan14b":
         return dict(name="Wan2.1-14B 1280x720x81f layer (q,k,v [1,75600,40,128])",
                     grid=(21, 45, 80), sliced=1, heads=40, text_tokens=0, text_valid=0,
                     text_blocks=0, p_remain=0.8, drop=0.7, variant="wan", text_amp=0.0,
@@ -137,7 +143,7 @@ def run_operator(wl, inp, q=None, k=None, v=None, return_bits=False):
 
 
 def algorithmic_flops(wl, inp, bits):
-    """4*128*128*128 per live (q-block, k-block) tile + dense text rows (BASELINE.md FLOP rule)."""
+    """4*128*128*128 per live (q-block, k-block) tile + dense text rows."""
     words = bits.to(torch.int64) & 0xFFFFFFFF
     pop = 0
     x = words
@@ -204,9 +210,10 @@ def peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return dict(bf16_burst=d.get("bf16_tflops", 1590.0), bf16_sustained=d.get("bf16_tflops_sustained", 1400.0),
-                    hbm=d.get("hbm_gbs", 6650.0), source="measured (MEASURED_PEAKS.json)")
-    return dict(bf16_burst=1590.0, bf16_sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+        return dict(bf16_burst=d.get("bf16_tflops", 989.0), bf16_sustained=d.get("bf16_tflops_sustained", 989.0),
+                    hbm=d.get("hbm_gbs", 3350.0), source="measured (MEASURED_PEAKS.json)")
+    return dict(bf16_burst=989.0, bf16_sustained=989.0, hbm=3350.0,
+                source="NVIDIA H100 SXM data sheet (dense bf16, 700 W card)")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -286,7 +293,7 @@ def cpu_sample(wl, kind: str, nq: int, min_seconds: float):
 
 # ------------------------------------------------------------------------------------------------
 # GPU reference leg: the UNMODIFIED reference operator (Triton JIT + FlashAttention-2) on the same
-# tensors on the same B200 (SURVEY §8d "Reference timed beside it (1)").  Checker/baseline only.
+# tensors on the same GPU (SURVEY §8d "Reference timed beside it (1)").  Checker/baseline only.
 # ------------------------------------------------------------------------------------------------
 def gpu_reference_leg(wl, inp, iters=3):
     sys.path.insert(0, str(ROOT / "tests"))
@@ -347,7 +354,7 @@ def gpu_reference_leg(wl, inp, iters=3):
             for cache in getattr(kern, "device_caches", {}).values():
                 for ck in cache[0].values():
                     ptx = ck.asm.get("ptx", "")
-                    isa = {"tcgen05.mma": ptx.count("tcgen05.mma"), "mma.sync": ptx.count("mma.sync"),
+                    isa = {"mma.sync": ptx.count("mma.sync"),
                            "wgmma": ptx.count("wgmma"), "cp.async.bulk": ptx.count("cp.async.bulk")}
         except Exception:  # noqa: BLE001
             pass
@@ -489,6 +496,27 @@ def dit_forward_leg(wl, inp, n_double, n_single, hidden=3072, heads=24, fp8_too=
 
 
 # ------------------------------------------------------------------------------------------------
+DUMP_BYTES = 48 << 20   # what --dump-outputs writes at most (float32)
+
+
+def dump_outputs(out_dir: Path, result: torch.Tensor, rank: int = 0, world: int = 1):
+    """The result of one operator call ([1, S, H*D] on this rank) as float32 .npy files: every row
+    when it fits this rank's share of DUMP_BYTES, otherwise a fixed seeded sample of rows (ascending),
+    plus the row indices."""
+    import numpy as np
+    x = result.reshape(result.shape[1], -1)
+    n_rows, width = x.shape
+    keep = max(1, min(n_rows, DUMP_BYTES // world // (4 * width)))
+    if keep < n_rows:
+        rows = torch.randperm(n_rows, generator=torch.Generator().manual_seed(20240611))[:keep].sort().values
+    else:
+        rows = torch.arange(n_rows)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    tag = "" if world == 1 else f".rank{rank}"
+    np.save(out_dir / f"out{tag}.npy", x[rows.to(x.device)].float().cpu().numpy())
+    np.save(out_dir / f"out_rows{tag}.npy", rows.double().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -510,7 +538,11 @@ def main():
                     help="ALSO time the opt-in FP8 P.V variant (reported under 'fp8_pv_variant'; never the headline)")
     ap.add_argument("--no-gpu-reference", action="store_true",
                     help="skip timing the unmodified reference operator (Triton + FA2) on this GPU")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's result to DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        raise SystemExit("--steps must be >= 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     wl = workload(args.workload, args.drop)
     rank = int(os.environ.get("RANK", "0"))
@@ -581,10 +613,13 @@ def main():
     with ClockSampler(local_rank) as clk:
         ev0.record()
         for _ in range(args.steps):
-            step()
+            last = step()
         ev1.record()
         barrier()
     ms = ev0.elapsed_time(ev1) / args.steps
+    if args.dump_outputs:
+        dump_outputs(Path(args.dump_outputs), last, rank, world)
+    del last
     if dist is not None:
         t = torch.tensor([ms], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -635,15 +670,8 @@ def main():
         torch.cuda.synchronize()
         ams = a0.elapsed_time(a1) / n_it
         ach = r_flops / (ams * 1e-3) / 1e12
-        traffic = None
-        tp = ROOT / "profiles" / "attn_traffic.json"
-        if tp.exists() and args.workload == "hy720p":
-            try:
-                traffic = json.loads(tp.read_text()).get("dram_bytes_per_launch")
-            except Exception:
-                traffic = None
         roof = {"bound": "tensor", "kernel": "carved_attn_fwd_kernel", "achieved": ach, "peak": pk["bf16_burst"],
-                "unit": "TFLOP/s", "frac": ach / pk["bf16_burst"], "traffic": traffic, "ms_per_launch": ams,
+                "unit": "TFLOP/s", "frac": ach / pk["bf16_burst"], "ms_per_launch": ams,
                 "frac_of_sustained_peak": ach / pk["bf16_sustained"], "sustained_peak": pk["bf16_sustained"],
                 "peak_source": pk["source"] + ", bf16 burst (kernel timed alone)",
                 "algorithmic_flops_per_launch": r_flops, "live_tiles": r_pop, "mask_source": mask_source}
@@ -659,7 +687,7 @@ def main():
         hq, hk, hv = (x.to(torch.bfloat16).cpu().pin_memory() for x in (inp["q"], inp["k"], inp["v"]))
         hout = torch.empty_like(hq).pin_memory()
         groups = int(os.environ.get("JENGA_E2E_GROUPS", "0")) or (
-            12 if inp["heads"] % 12 == 0 else (4 if inp["heads"] % 4 == 0 else 1))  # measured: 12 groups best at H=24
+            12 if inp["heads"] % 12 == 0 else (4 if inp["heads"] % 4 == 0 else 1))  # 12 head groups at H=24
         pipe = HostPipelinedAttention(1, inp["S"], inp["heads"], 128, torch.bfloat16, dev, groups=groups,
                                       variant=wl["variant"])
         kw = dict(cu_seqlens_q=inp["cu"], cu_seqlens_kv=inp["cu"], text_blocks=wl["text_blocks"],

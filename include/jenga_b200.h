@@ -1,9 +1,9 @@
 /*
- * jenga_b200 — C ABI of the B200-native AttenCarve hot path.
+ * jenga_b200 — C ABI of the H100-native AttenCarve hot path.
  *
- * Drop-in boundary for the one path of dvlab-research/Jenga that BASELINE.json names:
+ * Drop-in boundary for the AttenCarve path of dvlab-research/Jenga:
  * gilbert token reordering, block scoring/selection and the 128x128 block-sparse
- * self-attention (RMSNorm + RoPE prologue), as hand-written sm_100a CUDA.
+ * self-attention (RMSNorm + RoPE prologue), as hand-written sm_90a CUDA.
  *
  * Conventions (every entry point):
  *   - plain pointers and sizes only; device pointers unless the name says "host";

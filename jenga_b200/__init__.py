@@ -1,4 +1,4 @@
-"""jenga_b200 — B200-native (sm_100a) AttenCarve hot path of dvlab-research/Jenga.
+"""jenga_b200 — H100-native (sm_90a) AttenCarve hot path of dvlab-research/Jenga.
 
 Public surface mirrors the reference's operator for this path:
   jenga_b200.attention.block_sparse_attention(...)   (hyvideo / hyvideo_i2v / wan variants)

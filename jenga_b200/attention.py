@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's AttenCarve operator for the B200 path.
+"""Host-side mirror of the reference's AttenCarve operator for the H100 path.
 
 `block_sparse_attention` keeps the reference signature
 (hyvideo/modules/attention_block_triton_diffres.py:399-424, hyvideo_i2v twin :398-423,
@@ -62,7 +62,7 @@ def carved_attention_fwd(
     kv_limit_dense: int | None = None, out: torch.Tensor | None = None,
     err_flag: torch.Tensor | None = None,
 ) -> torch.Tensor:
-    """One launch of the sm_100a carved-attention kernel (C-ABI jenga_carved_attn_fwd).
+    """One launch of the sm_90a carved-attention kernel (C-ABI jenga_carved_attn_fwd).
     Sparse q-blocks [0, nq_sparse) follow the reference Triton kernel (:38-136); dense
     q-blocks [nq_sparse, nq_sparse+nq_dense) follow its flash_attn_func text rows (:371-380).
     Returns `out` [B, Sq, H, D]."""

@@ -1,4 +1,4 @@
-"""Builds libjenga_b200.so (sm_100a only) in-tree with nvcc.
+"""Builds libjenga_b200.so (sm_90a, H100, only) in-tree with nvcc.
 
 The shared library is the product: a C-ABI (include/jenga_b200.h) with no torch types in its
 signatures.  It is built next to the sources (jenga_b200/_C/) so that it travels with the
@@ -20,11 +20,12 @@ OUT_DIR = PKG / "_C"
 LIB = OUT_DIR / "libjenga_b200.so"
 STAMP = OUT_DIR / "build.stamp"
 
-CU_SOURCES = ["api.cu", "carved_attn.cu", "carved_attn_v6.cu", "carved_attn_v7.cu", "prologue.cu", "prologue_bulk.cu", "select.cu", "stepcache.cu", "dense_fused.cu", "gilbert_device.cu", "fp8.cu"]
+CU_SOURCES = ["api.cu", "carved_attn.cu", "prologue.cu", "prologue_bulk.cu", "select.cu", "stepcache.cu", "dense_fused.cu", "gilbert_device.cu", "fp8.cu"]
 CXX_SOURCES = ["gilbert.cpp"]
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function",
     "-Xptxas", "-v",
@@ -78,8 +79,7 @@ def build(force: bool = False, verbose: bool = False, defines: tuple[str, ...] =
             sys.stderr.write(logs[-1])
             raise RuntimeError(f"nvcc failed on {src.name}")
         objs.append(obj)
-    cmd = [nvcc, "-shared", "-o", str(LIB), *map(str, objs), "-gencode",
-           "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-lcudart_static", "-ldl", "-lrt",
+    cmd = [nvcc, "-shared", "-o", str(LIB), *map(str, objs), *GENCODE, "-Xcompiler", "-fPIC", "-lcudart_static", "-ldl", "-lrt",
            "-lpthread"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     logs.append(f"$ {' '.join(cmd)}\n{r.stdout}{r.stderr}")
@@ -110,7 +110,7 @@ def _build_variant(defines, variant, verbose):
             print(r.stderr)
         objs.append(obj)
     out = OUT_DIR / f"libjenga_b200.{variant}.so"
-    cmd = [nvcc, "-shared", "-o", str(out), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-shared", "-o", str(out), *map(str, objs), *GENCODE,
            "-Xcompiler", "-fPIC", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

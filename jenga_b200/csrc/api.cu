@@ -169,7 +169,7 @@ extern "C" int jenga_gather_rows(const void* src, void* dst, const int64_t* inde
   const int vec = static_cast<int>(row_bytes / 16);
   const long long total = n_index * vec;
   long long blocks = (total + 255) / 256;
-  const long long cap = 148ll * 8 * 4;  // a few waves of 8 CTAs/SM; grid-stride beyond that
+  const long long cap = static_cast<long long>(kNumSMs) * 8 * 4;  // a few waves of 8 CTAs/SM; grid-stride beyond that
   if (blocks > cap) blocks = cap;
   dim3 grid(static_cast<unsigned>(blocks), static_cast<unsigned>(batch));
   gather_rows_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -248,7 +248,7 @@ extern "C" int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* a, void* str
   for (int r = 0; r < a->world; ++r) p.peer[r] = a->peer_qkv_host[r];
   const long long total = (a->n_loc * a->world + a->n_text) * p.hg * p.vec_per_head;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148ll * 16) blocks = 148ll * 16;
+  if (blocks > static_cast<long long>(kNumSMs) * 16) blocks = static_cast<long long>(kNumSMs) * 16;
   dim3 grid(static_cast<unsigned>(blocks), 3);
   ulysses_scatter_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   cudaError_t ce = cudaGetLastError();

@@ -1,53 +1,23 @@
-// Carved (block-sparse) flash-attention forward for sm_100a.
+// Carved (block-sparse) flash-attention forward for sm_90a.
 //
 // Replaces the reference's Triton one-hot kernel
 //   hyvideo/modules/attention_block_triton_diffres.py:38-136 (+ launcher :139-196)
 // and its text-row flash_attn_func call (:371-380) with ONE launch.
 //
-// Work decomposition: one CTA per (batch*head, 128-row query block); 192 threads:
-//   warp 0      TMA producer      Q once, then one K tile and one V tile per live key block
-//   warp 1      tcgen05 issuer    S = Q~ K^T (SS), O += P V (TS, P read from TMEM); owns TMEM
-//   warps 2..5  softmax           one query row per thread: tcgen05.ld S -> online softmax in
-//                                 base 2 -> P as packed 16-bit back into TMEM; lazy O rescale;
-//                                 final O / l -> global
-// Key blocks are processed as two 64-key halves with S double-buffered in TMEM, so the tensor
-// pipe always runs one half ahead of the softmax warps (see the pipeline comment on the
-// kernel).  Two CTAs are co-resident per SM (256 TMEM columns and ~100 KB shared memory each).
+// Work decomposition: one CTA per (batch*head, 128-row query block); 288 threads:
+//   warps 0..7  two consumer warpgroups of 64 query rows each: S = Q~ K^T by wgmma (Q and K from
+//               shared memory, S in registers), online softmax in base 2 on the registers, then
+//               O += P V by wgmma with P as the register A operand; final O / l -> global
+//   warp 8      TMA producer: Q once, then one K tile and one V tile per live key block into a
+//               two-stage ring (K and V slots are released separately, so the next K tile lands
+//               while the P.V product of the current one runs)
+// S and O are fp32 register accumulators (64 + 64 registers per thread); one CTA per SM with
+// ~164 KB of shared memory, two warpgroups whose softmax and MMA phases interleave on the SM.
 //
 // HBM/L2 layout: q,k,v stay in the caller's [B,S,H,D] layout; TMA boxes are {64 d, 128 rows}
-// (Q: 128 rows) or {64 d, 64 rows} (K, V) with 128-byte swizzle.  K boxes are K-major UMMA
-// operands, V boxes are MN-major UMMA operands (no transpose anywhere).
-// CTAs are numbered head-major so that all CTAs in flight read the same head's K/V (59 MB at
-// 115K tokens) out of L2.
-#include <cstdlib>
-#include <cstring>
-
+// with 128-byte swizzle.  K boxes are K-major wgmma operands, V boxes MN-major (no transpose).
+// CTAs are numbered head-major so that all CTAs in flight read the same head's K/V out of L2.
 #include "carved_attn_common.cuh"
-
-#ifndef JENGA_POLY_EVERY
-#define JENGA_POLY_EVERY 3
-#endif
-#ifndef JENGA_RELAXED_PRODUCER
-#define JENGA_RELAXED_PRODUCER 0
-#endif
-#if JENGA_RELAXED_PRODUCER
-#define JENGA_PRODUCER_WAIT mbar_wait_relaxed
-#else
-#define JENGA_PRODUCER_WAIT mbar_wait
-#endif
-#ifndef JENGA_PRODUCER_CONSUMPTION_ORDER
-#define JENGA_PRODUCER_CONSUMPTION_ORDER 1
-#endif
-#ifndef JENGA_QK_FULL
-#define JENGA_QK_FULL 0
-#endif
-
-// L2 residency hints (experiment, profiles/README.md): 1 = Q loads evict_first, K/V loads evict_last,
-// O stores streaming.  K+V of a head (59 MB at HY-720p) are re-read by every q block of the head; Q and O
-// are touched once.
-#ifndef JENGA_ATTN_L2HINT
-#define JENGA_ATTN_L2HINT 0
-#endif
 
 namespace jenga {
 
@@ -57,53 +27,43 @@ using attn::BlockWalker;
 using attn::KernelParams;
 
 constexpr int kBlock = 128;           // rows per q block == keys per kv block
-constexpr int kHalf = 64;             // keys per half tile (the softmax / MMA pipelining unit)
 constexpr int kHeadDim = 128;
-constexpr int kThreads = 192;
-constexpr int kQHalfBytes = kBlock * 64 * 2;     // 16 KB: 128 q rows x 64 d
-constexpr int kQTileBytes = 2 * kQHalfBytes;     // 32 KB
-constexpr int kKVBoxBytes = kHalf * 64 * 2;      // 8 KB: 64 keys x 64 d  (one TMA box)
-constexpr int kKVSlotBytes = 2 * kKVBoxBytes;    // 16 KB: 64 keys x 128 d (two d-halves)
+constexpr int kConsumerThreads = 256;
+constexpr int kThreads = kConsumerThreads + 32;
+constexpr int kStages = 2;                       // K/V ring depth
+constexpr int kBoxBytes = kBlock * 64 * 2;       // 16 KB: 128 rows x 64 d (one TMA box)
+constexpr int kTileBytes = 2 * kBoxBytes;        // 32 KB: 128 rows x 128 d (two d halves)
 constexpr int kMaxMaskWords = 256;               // up to 8192 key blocks (1M tokens)
-constexpr uint32_t kTmemCols = 256;              // S_a [0,64)  S_b [64,128)  O [128,256)
-constexpr bool kQKFull = JENGA_QK_FULL != 0;      // 1: one N=128 QK issue per tile (A read once per k-step)
-constexpr int kPolyEvery = JENGA_POLY_EVERY;     // every n-th exp2 pair uses the FMA-pipe polynomial (0 = never)
 
 // shared-memory carve-up (offsets from the 1024-aligned base)
 constexpr int kOffQ = 0;
-constexpr int kOffK = kOffQ + kQTileBytes;        // K_a, K_b
-constexpr int kOffV = kOffK + 2 * kKVSlotBytes;   // V_a, V_b
-constexpr int kOffBars = kOffV + 2 * kKVSlotBytes;
+constexpr int kOffK = kOffQ + kTileBytes;
+constexpr int kOffV = kOffK + kStages * kTileBytes;
+constexpr int kOffBars = kOffV + kStages * kTileBytes;
 constexpr int kOffMask = kOffBars + 128;
 constexpr int kSmemBytes = 1024 /*align slack*/ + kOffMask + kMaxMaskWords * 4;
 
-// mbarriers.  [h] = key half (a = keys 0..63, b = keys 64..127 of the current key block).
 enum BarId {
-  Q_FULL = 0, Q_READY,
-  K_FULL0, K_FULL1, K_EMPTY0, K_EMPTY1,
-  V_FULL0, V_FULL1, V_EMPTY0, V_EMPTY1,   // V_EMPTY[h] == "PV of half h retired"
-  S_FULL0, S_FULL1, P_FULL0, P_FULL1,
-  NUM_BARS
+  Q_FULL = 0,
+  K_FULL = 1, V_FULL = K_FULL + kStages,
+  K_EMPTY = V_FULL + kStages, V_EMPTY = K_EMPTY + kStages,   // one arrival per consumer warp
+  NUM_BARS = V_EMPTY + kStages
 };
-static_assert(NUM_BARS * 8 + 4 <= 128, "barrier block overflow");
+static_assert(NUM_BARS * 8 <= 128, "barrier block overflow");
 
-// Pipeline of one CTA (one 128-row q block), per live key block j and key half h:
-//
-//   TMA      K_h(j) -> smem   V_h(j) -> smem                      (4 single-buffered 16 KB slots)
-//   tensor   S_h = Q~ K_h^T (N=64)  ...  O += P_h V_h (K=64)        (in-order tcgen05 pipe)
-//   softmax  ld S_h -> max -> exp2 -> P_h (16-bit, over S_h) -> arrive
-//
-// S is double-buffered across the two halves, so while the softmax warps work on S_a(j) the
-// tensor pipe runs S_b(j) and the PV of the previous half; S_h(j+1) is issued right behind
-// PV_h(j) — the tcgen05 pipe executes MMAs in issue order, so it overwrites S_h only after
-// PV_h(j) has consumed P_h(j).  The softmax warps therefore never wait for the tensor pipe in
-// steady state, and two co-resident CTAs per SM keep both the MUFU and the tensor pipe fed.
-// kPvFp8 (SURVEY §8 f-3, opt-in): P and V enter the P.V product as FP8 e4m3 — V quantised per head by
+// byte offset of (row, col) inside a 128-byte-swizzled tile of 128-byte rows (1024-B aligned)
+__device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t col) {
+  return row * 128u + ((((col >> 4) ^ row) & 7u) << 4) + (col & 15u);
+}
+
+// kPvFp8 (opt-in): P and V enter the P.V product as FP8 e4m3 — V quantised per head by
 // jenga_quantize_v_fp8 (scale = absmax/448), P converted with cvt.rn.satfinite.e4m3x2 (p <= 2^8 by
-// the lazy-rescale bound, e4m3 max 448) — through tcgen05.mma kind::f8f6f4 (K = 32 per MMA: half the
-// P.V tensor cycles and half the V shared-memory traffic).  Q.K^T, the softmax and l stay as they are.
+// the lazy-rescale bound, e4m3 max 448) — through wgmma m64n128k32 e4m3 (half the P.V tensor cycles).
+// 8-bit wgmma operands must be K-major, so the consumers transpose each V tile in shared memory
+// into V^T with the keys of every 32-key group permuted to match the order in which the S
+// accumulator fragment already holds P: no shuffles of P.  Q.K^T, the softmax and l are unchanged.
 template <bool kBF16, bool kPvFp8 = false>
-__global__ void __launch_bounds__(kThreads, 2)
+__global__ void __launch_bounds__(kThreads, 1)
 carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
                        const __grid_constant__ CUtensorMap tm_k,
                        const __grid_constant__ CUtensorMap tm_v, const KernelParams p) {
@@ -111,10 +71,9 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
   uint8_t* sQ = smem + kOffQ;
-  uint8_t* sK = smem + kOffK;  // + h * kKVSlotBytes
+  uint8_t* sK = smem + kOffK;  // + stage * kTileBytes
   uint8_t* sV = smem + kOffV;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NUM_BARS);
   uint32_t* s_mask = reinterpret_cast<uint32_t*>(smem + kOffMask);
 
   const int warp = threadIdx.x >> 5;
@@ -154,349 +113,247 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     s_mask[w] = bits;
   }
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_q);
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
 #pragma unroll
-    for (int i = 0; i < NUM_BARS; ++i)
-      mbar_init(&bars[i], (i == Q_READY || i == P_FULL0 || i == P_FULL1) ? 128u : 1u);
+    for (int i = 0; i < NUM_BARS; ++i) mbar_init(&bars[i], i >= K_EMPTY ? 8u : 1u);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_O = tmem_base + 128;  // fp32 O accumulator; S_h at tmem_base + 64*h
 
   int n_tiles = 0;
   for (int w = 0; w < nwords; ++w) n_tiles += __popc(s_mask[w]);
 
-  if (warp == 0) {
+  if (warp == kConsumerThreads / 32) {
     // =============================== TMA producer ===============================
-    if (n_tiles > 0 && elect_one()) {
-      mbar_arrive_expect_tx(&bars[Q_FULL], kQTileBytes);
-#if JENGA_ATTN_L2HINT
-      const uint64_t pol_q = l2_policy_evict_first(), pol_kv = l2_policy_evict_last();
-      tma_load_4d_hint(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b, pol_q);
-      tma_load_4d_hint(sQ + kQHalfBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b, pol_q);
-#define JENGA_KV_LOAD(dst, map, bar, c0, c1, c2, c3) tma_load_4d_hint(dst, map, bar, c0, c1, c2, c3, pol_kv)
-#else
+    if (n_tiles > 0 && lane == 0) {
+      mbar_arrive_expect_tx(&bars[Q_FULL], kTileBytes);
       tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
-      tma_load_4d(sQ + kQHalfBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b);
-#define JENGA_KV_LOAD(dst, map, bar, c0, c1, c2, c3) tma_load_4d(dst, map, bar, c0, c1, c2, c3)
-#endif
-      // Loads are issued in the order the tensor pipe consumes them,
-      //   K_a(0) K_b(0) | V_a(0) K_a(1) | V_b(0) K_b(1) | V_a(1) K_a(2) | ...
-      // so a wait for a V slot never holds up the K half the next QK needs first (A/B on one
-      // box: 1.2 % faster than tile order K_a K_b V_a V_b = JENGA_PRODUCER_CONSUMPTION_ORDER 0).
-      // K boxes are laid out [d half][key half] (4 x 8 KB) so the 128 keys
-      // of one d half are contiguous: serves two N=64 operands or one N=128 operand.
-      auto load_k = [&](int blk, int hh, uint32_t par) {
-        const int row0 = blk * kBlock + hh * kHalf;
-        uint8_t* dst = sK + hh * kKVBoxBytes;
-        JENGA_PRODUCER_WAIT(&bars[K_EMPTY0 + hh], par, p.err_flag);
-        mbar_arrive_expect_tx(&bars[K_FULL0 + hh], kKVSlotBytes);
-        JENGA_KV_LOAD(dst, &tm_k, &bars[K_FULL0 + hh], 0, row0, h, b);
-        JENGA_KV_LOAD(dst + 2 * kKVBoxBytes, &tm_k, &bars[K_FULL0 + hh], 64, row0, h, b);
-      };
-      auto load_v = [&](int blk, int hh, uint32_t par) {
-        const int row0 = blk * kBlock + hh * kHalf;
-        uint8_t* dst = sV + hh * kKVSlotBytes;
-        JENGA_PRODUCER_WAIT(&bars[V_EMPTY0 + hh], par, p.err_flag);
-        if constexpr (kPvFp8) {   // 64 keys x 128 one-byte channels = one 8 KB box
-          mbar_arrive_expect_tx(&bars[V_FULL0 + hh], kKVBoxBytes);
-          JENGA_KV_LOAD(dst, &tm_v, &bars[V_FULL0 + hh], 0, row0, h, b);
-        } else {
-          mbar_arrive_expect_tx(&bars[V_FULL0 + hh], kKVSlotBytes);
-          JENGA_KV_LOAD(dst, &tm_v, &bars[V_FULL0 + hh], 0, row0, h, b);
-          JENGA_KV_LOAD(dst + kKVBoxBytes, &tm_v, &bars[V_FULL0 + hh], 64, row0, h, b);
-        }
-      };
+      tma_load_4d(sQ + kBoxBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b);
       BlockWalker it(s_mask, nwords);
-#if JENGA_PRODUCER_CONSUMPTION_ORDER
-      int blk = it.next();
-      load_k(blk, 0, 1);
-      load_k(blk, 1, 1);
-      for (int j = 0; blk >= 0; ++j) {
-        const uint32_t par = (j & 1) ^ 1;   // slot-free parity for tile j; tile j+1 uses par ^ 1
-        const int nxt = it.next();
-        load_v(blk, 0, par);
-        if (nxt >= 0) load_k(nxt, 0, par ^ 1);
-        load_v(blk, 1, par);
-        if (nxt >= 0) load_k(nxt, 1, par ^ 1);
-        blk = nxt;
-      }
-#else
       int j = 0;
       for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
-        const uint32_t par = (j & 1) ^ 1;
-        load_k(blk, 0, par);
-        load_k(blk, 1, par);
-        load_v(blk, 0, par);
-        load_v(blk, 1, par);
-      }
-#endif
-    }
-  } else if (warp == 1) {
-    // =============================== tcgen05 issuer ===============================
-    if (n_tiles > 0 && elect_one()) {
-      constexpr uint32_t idesc_qk = umma_idesc_f16(kBF16, /*b_mn_major=*/false, 128, kHalf);
-      constexpr uint32_t idesc_pv = umma_idesc_f16(kBF16, /*b_mn_major=*/true, 128, kHeadDim);
-      // K-major SW128 operands: 8-row groups are 1024 B apart (SBO); LBO unused (=16 B).
-      // Q: 128 rows, d-halves 16 KB apart.  K_h: 64 rows, d-halves 8 KB apart.
-      const uint64_t q_desc = umma_smem_desc(smem_u32(sQ), 16, 1024, UMMA_LAYOUT_SW128);
-      // MN-major SW128 operand V_h: 64-wide d chunks are one 8 KB box apart (LBO), 8-key
-      // groups are 1024 B apart (SBO).
-      auto issue_qk = [&](int hh) {
-        const uint64_t k_desc =
-            umma_smem_desc(smem_u32(sK + hh * kKVBoxBytes), 16, 1024, UMMA_LAYOUT_SW128);
-#pragma unroll
-        for (int kk = 0; kk < kHeadDim / 16; ++kk) {
-          const uint64_t qoff = static_cast<uint64_t>(((kk & 3) * 32 + (kk >> 2) * kQHalfBytes) >> 4);
-          const uint64_t koff = static_cast<uint64_t>(((kk & 3) * 32 + (kk >> 2) * 2 * kKVBoxBytes) >> 4);
-          umma_ss(tmem_base + hh * kHalf, q_desc + qoff, k_desc + koff, idesc_qk, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(&bars[K_EMPTY0 + hh]);
-        umma_commit(&bars[S_FULL0 + hh]);
-      };
-      // One N=128 issue for the whole key block: Q (the A operand, 4 KB per k-step) is read
-      // from shared memory once instead of once per half.
-      auto issue_qk_full = [&]() {
-        constexpr uint32_t idesc_full = umma_idesc_f16(kBF16, false, 128, kBlock);
-        const uint64_t k_desc = umma_smem_desc(smem_u32(sK), 16, 1024, UMMA_LAYOUT_SW128);
-#pragma unroll
-        for (int kk = 0; kk < kHeadDim / 16; ++kk) {
-          const uint64_t off = static_cast<uint64_t>(((kk & 3) * 32 + (kk >> 2) * kQHalfBytes) >> 4);
-          umma_ss(tmem_base, q_desc + off, k_desc + off, idesc_full, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(&bars[K_EMPTY0]);
-        umma_commit(&bars[K_EMPTY1]);
-        umma_commit(&bars[S_FULL0]);
-        umma_commit(&bars[S_FULL1]);
-      };
-      auto issue_pv = [&](int hh, bool first) {
-        const uint64_t v_desc =
-            umma_smem_desc(smem_u32(sV + hh * kKVSlotBytes), kKVBoxBytes, 1024, UMMA_LAYOUT_SW128);
-        if constexpr (kPvFp8) {
-          // MN-major SW128 operand, one byte per channel: a key row is one 128-byte swizzle span;
-          // K = 32 keys per MMA = 32 rows = 4096 B; P advances 8 columns (4 e4m3 per column)
-          constexpr uint32_t idesc_pv8 = (1u << 4) | (1u << 16) | ((kHeadDim >> 3) << 17) | ((128u >> 4) << 24);
-#pragma unroll
-          for (int kk = 0; kk < kHalf / 32; ++kk) {
-            const uint64_t off = static_cast<uint64_t>((kk * 32 * 128) >> 4);
-            umma_ts_f8(tmem_O, tmem_base + hh * kHalf + kk * 8, v_desc + off, idesc_pv8,
-                       (!first || kk > 0) ? 1u : 0u);
-          }
+        const int s = j % kStages;
+        const uint32_t par = ((j / kStages) & 1) ^ 1;   // slot-free parity (a fresh barrier passes)
+        const int row0 = blk * kBlock;
+        uint8_t* k_dst = sK + s * kTileBytes;
+        uint8_t* v_dst = sV + s * kTileBytes;
+        mbar_wait(&bars[K_EMPTY + s], par, p.err_flag);
+        mbar_arrive_expect_tx(&bars[K_FULL + s], kTileBytes);
+        tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
+        tma_load_4d(k_dst + kBoxBytes, &tm_k, &bars[K_FULL + s], 64, row0, h, b);
+        mbar_wait(&bars[V_EMPTY + s], par, p.err_flag);
+        if constexpr (kPvFp8) {   // 128 keys x 128 one-byte channels = one 16 KB box
+          mbar_arrive_expect_tx(&bars[V_FULL + s], kBoxBytes);
+          tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
         } else {
-#pragma unroll
-          for (int kk = 0; kk < kHalf / 16; ++kk) {
-            // 16 keys = 16 rows x 128 B inside each V box; P advances 8 packed columns
-            const uint64_t off = static_cast<uint64_t>((kk * 16 * 128) >> 4);
-            umma_ts(tmem_O, tmem_base + hh * kHalf + kk * 8, v_desc + off, idesc_pv,
-                    (!first || kk > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(&bars[V_EMPTY0 + hh]);
-      };
-
-      mbar_wait(&bars[Q_READY], 0, p.err_flag);
-      if constexpr (kQKFull) {
-        mbar_wait(&bars[K_FULL0], 0, p.err_flag);
-        mbar_wait(&bars[K_FULL1], 0, p.err_flag);
-        tc_fence_after();
-        issue_qk_full();
-      } else {
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          mbar_wait(&bars[K_FULL0 + hh], 0, p.err_flag);
-          tc_fence_after();
-          issue_qk(hh);
-        }
-      }
-      for (int j = 0; j < n_tiles; ++j) {
-        const uint32_t par = j & 1;
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          mbar_wait(&bars[V_FULL0 + hh], par, p.err_flag);
-          mbar_wait(&bars[P_FULL0 + hh], par, p.err_flag);
-          tc_fence_after();
-          issue_pv(hh, j == 0 && hh == 0);
-          if (j + 1 < n_tiles) {
-            if constexpr (kQKFull) {
-              if (hh == 1) {
-                mbar_wait(&bars[K_FULL0], par ^ 1, p.err_flag);
-                mbar_wait(&bars[K_FULL1], par ^ 1, p.err_flag);
-                tc_fence_after();
-                issue_qk_full();
-              }
-            } else {
-              mbar_wait(&bars[K_FULL0 + hh], par ^ 1, p.err_flag);
-              tc_fence_after();
-              issue_qk(hh);  // overwrites S_h / P_h(j) strictly after PV_h(j): in-order pipe
-            }
-          }
+          mbar_arrive_expect_tx(&bars[V_FULL + s], kTileBytes);
+          tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
+          tma_load_4d(v_dst + kBoxBytes, &tm_v, &bars[V_FULL + s], 64, row0, h, b);
         }
       }
     }
-  } else {
-    // =============================== softmax / epilogue ===============================
-    const int quad = warp & 3;            // TMEM lane quadrant this warp may touch
-    const int row = quad * 32 + lane;     // query row inside the block
-    const int st = threadIdx.x - 64;      // 0..127
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-    const long long q_row = q_row0 + row;
+    return;
+  }
 
-    float m_used = -INFINITY;  // running (possibly stale) max, in scaled log2 units
-    float l_sum = 0.f;
-    // sparse class: Q~ = round(Q * qk_scale) and raw S is already in log2 units (c = 1)
-    // dense class : raw S, scaled inside the exponent (c = qk_scale), like FlashAttention
-    const float c = dense ? p.qk_scale : 1.0f;
+  // =============================== consumers ===============================
+  const int wg = warp >> 2;                       // warpgroup: query rows [64 wg, 64 wg + 64)
+  const int g = lane >> 2, qd = lane & 3;
+  // accumulator fragment: element i of a thread is row g + 8 ((i >> 1) & 1) of the warp's 16 rows,
+  // column 8 (i >> 2) + 2 qd + (i & 1)
+  const int row_lo = wg * 64 + (warp & 3) * 16 + g;
+  float m_used[2] = {-INFINITY, -INFINITY};  // running (possibly stale) max, in scaled log2 units
+  float l_sum[2] = {0.f, 0.f};               // this thread's partial sums (its 32 columns)
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  // sparse class: Q~ = round(Q * qk_scale) and raw S is already in log2 units (c = 1)
+  // dense class : raw S, scaled inside the exponent (c = qk_scale), like FlashAttention
+  const float c = dense ? p.qk_scale : 1.0f;
 
-    if (n_tiles > 0) {
-      mbar_wait(&bars[Q_FULL], 0, p.err_flag);
-      if (!dense) {
-        // ref :87-88  q = (q * qk_scale).to(dtype) — elementwise, so swizzle-agnostic
-        uint4* q4 = reinterpret_cast<uint4*>(sQ);
+  if (n_tiles > 0) {
+    mbar_wait(&bars[Q_FULL], 0, p.err_flag);
+    if (!dense) {
+      // ref :87-88  q = (q * qk_scale).to(dtype) — elementwise, so swizzle-agnostic
+      uint4* q4 = reinterpret_cast<uint4*>(sQ);
 #pragma unroll 4
-        for (int i = 0; i < kQTileBytes / 16 / 128; ++i) {
-          uint4 v = q4[st + i * 128];
-          uint32_t* e = reinterpret_cast<uint32_t*>(&v);
+      for (int i = 0; i < kTileBytes / 16 / kConsumerThreads; ++i) {
+        uint4 v = q4[threadIdx.x + i * kConsumerThreads];
+        uint32_t* e = reinterpret_cast<uint32_t*>(&v);
 #pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const float2 f = unpack2<kBF16>(e[t]);
-            e[t] = pack2<kBF16>(f.x * p.qk_scale, f.y * p.qk_scale);
-          }
-          q4[st + i * 128] = v;
+        for (int t = 0; t < 4; ++t) {
+          const float2 f = unpack2<kBF16>(e[t]);
+          e[t] = pack2<kBF16>(f.x * p.qk_scale, f.y * p.qk_scale);
         }
-        fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core proxy
+        q4[threadIdx.x + i * kConsumerThreads] = v;
       }
-      mbar_arrive(&bars[Q_READY]);
-
-      BlockWalker it(s_mask, nwords);
-      int j = 0;
-      for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
-        // ref :113-114 — text_amp is a constant added to every score of a text key block, in
-        // log2 units (sparse class only, where c == 1): fold it into the exponent offset.
-        const float amp = (!dense && blk >= p.text_block_start) ? p.text_amp : 0.f;
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const uint32_t tmem_S = tmem_base + hh * kHalf + lane_base;
-          mbar_wait(&bars[S_FULL0 + hh], j & 1, p.err_flag);
-          tc_fence_after();
-          float s[kHalf];
-          {
-            uint32_t* su = reinterpret_cast<uint32_t*>(s);
-            tmem_ld32(tmem_S, su);
-            tmem_ld32(tmem_S + 32, su + 32);
-            tmem_ld_wait();
-          }
-          const long long col0 = static_cast<long long>(blk) * kBlock + hh * kHalf;
-          if (col0 + kHalf > kv_limit) {  // rare: only the half tile that straddles seqlen
-            asm volatile("" ::: "memory");  // keep this a branch, not 64 predicated selects
-#pragma unroll
-            for (int i = 0; i < kHalf; ++i)
-              if (col0 + i >= kv_limit) s[i] = -INFINITY;  // ref :117-118
-          }
-          float mx0 = fmaxf(s[0], s[1]), mx1 = fmaxf(s[2], s[3]);
-#pragma unroll
-          for (int i = 4; i < kHalf; i += 4) {
-            mx0 = fmaxf(mx0, fmaxf(s[i], s[i + 1]));
-            mx1 = fmaxf(mx1, fmaxf(s[i + 2], s[i + 3]));
-          }
-          const float mx = fmaf(fmaxf(mx0, mx1), c, amp);
-          const float m_cand = fmaxf(m_used, mx);
-          // Lazy rescale: the reference rescales acc by exp2(m_old - m_new) every tile
-          // (:121-132).  O/l is invariant to the reference point, so we only move it when the
-          // max grew by more than 2^8 — the final O/l is the same up to fp32 rounding.
-          const bool need = (m_cand - m_used) > 8.0f;  // false for NaN (-inf - -inf)
-          if (__any_sync(0xffffffffu, need)) {
-            if (j > 0 || hh > 0) {
-              // every PV issued so far must have retired before O is touched: the most recent
-              // one is PV_{1-hh} of tile (hh ? j : j-1)
-              if (hh == 0) mbar_wait(&bars[V_EMPTY1], (j - 1) & 1, p.err_flag);
-              else mbar_wait(&bars[V_EMPTY0], j & 1, p.err_flag);
-              tc_fence_after();
-              const float alpha = (m_cand == -INFINITY) ? 1.0f : fast_exp2(m_used - m_cand);
-#pragma unroll 1
-              for (int cc = 0; cc < 128; cc += 16) {
-                uint32_t o[16];
-                tmem_ld16(tmem_O + lane_base + cc, o);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                tmem_st16(tmem_O + lane_base + cc, o);
-              }
-              tmem_st_wait();
-              l_sum *= alpha;
-            }
-            m_used = m_cand;
-          }
-          const float off = amp - ((m_used == -INFINITY) ? 0.f : m_used);
-          // p = exp2(s*c + off) on packed pairs.  Every third pair takes the polynomial path
-          // (FMA/ALU pipes) so the MUFU — 16 ex2/clk/SM, as long as the tile's MMAs — is not
-          // the co-bottleneck; l accumulates the unrounded p (ref :131), P is rounded to the
-          // input dtype for the PV product (ref :128).
-          const f32x2 c2 = f2_pack(c, c), off2 = f2_pack(off, off);
-          f32x2 sum2 = f2_pack(0.f, 0.f);
-#pragma unroll
-          for (int cc = 0; cc < kHalf; cc += 32) {
-            uint32_t pk[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const f32x2 x = f2_fma(f2_pack(s[cc + 2 * i], s[cc + 2 * i + 1]), c2, off2);
-              float x0, x1, p0, p1;
-              f2_unpack(x, x0, x1);
-              f32x2 pp;
-              if (kPolyEvery > 0 && (i % kPolyEvery) == kPolyEvery - 1) {
-                pp = f2_exp2_poly(f2_pack(fmaxf(x0, -125.f), fmaxf(x1, -125.f)));
-                f2_unpack(pp, p0, p1);
-              } else {
-                p0 = fast_exp2(x0);
-                p1 = fast_exp2(x1);
-                pp = f2_pack(p0, p1);
-              }
-              sum2 = f2_add(sum2, pp);
-              if constexpr (kPvFp8) {
-                // two e4m3 per cvt (low byte = first operand), four keys per 32-bit column
-                const uint32_t h16 = pack2_e4m3(p0, p1);
-                if (i & 1) pk[i >> 1] |= h16 << 16; else pk[i >> 1] = h16;
-              } else {
-                pk[i] = pack2<kBF16>(p0, p1);
-              }
-            }
-            if constexpr (kPvFp8) {
-              uint32_t pk8[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) pk8[i] = pk[i];
-              tmem_st8(tmem_S + (cc >> 2), pk8);
-            } else {
-              tmem_st16(tmem_S + (cc >> 1), pk);
-            }
-          }
-          float sum0, sum1;
-          f2_unpack(sum2, sum0, sum1);
-          l_sum += sum0 + sum1;
-          tmem_st_wait();
-          tc_fence_before();
-          mbar_arrive(&bars[P_FULL0 + hh]);
-        }
-      }
-      mbar_wait(&bars[V_EMPTY1], (n_tiles - 1) & 1, p.err_flag);  // last PV retired (in-order)
-      tc_fence_after();
+      fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core proxy
+      named_bar_sync(1, kConsumerThreads);
     }
+    const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128;   // this warpgroup's 64 rows of each d half
 
-    // ---- epilogue: O / l -> global (ref :135-136); rows past the limit are zeros (:156) ----
+    BlockWalker it(s_mask, nwords);
+    int j = 0;
+    for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
+      const int s = j % kStages;
+      const uint32_t par = (j / kStages) & 1;
+      // ref :113-114 — text_amp is a constant added to every score of a text key block, in
+      // log2 units (sparse class only, where c == 1): fold it into the exponent offset.
+      const float amp = (!dense && blk >= p.text_block_start) ? p.text_amp : 0.f;
+
+      // ---- S = Q~ K^T (64 x 128 per warpgroup, K = 128 in 8 steps) ----
+      float sc[64];
+      mbar_wait(&bars[K_FULL + s], par, p.err_flag);
+      {
+        const uint32_t k_addr = smem_u32(sK + s * kTileBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kHeadDim / 16; ++kk) {
+          const uint32_t off = (kk & 3) * 32 + (kk >> 2) * kBoxBytes;
+          wgmma_128_ss<kBF16>(sc, gmma_desc_sw128(q_addr + off, 16, 1024),
+                              gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(sc);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars[K_EMPTY + s]);
+
+      // ---- online softmax on the registers ----
+      const long long col0 = static_cast<long long>(blk) * kBlock;
+      if (col0 + kBlock > kv_limit) {  // rare: only the tile that straddles seqlen
+#pragma unroll
+        for (int i = 0; i < 64; ++i)
+          if (col0 + (i >> 2) * 8 + qd * 2 + (i & 1) >= kv_limit) sc[i] = -INFINITY;  // ref :117-118
+      }
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < 64; i += 4) {
+        mx[0] = fmaxf(mx[0], fmaxf(sc[i], sc[i + 1]));
+        mx[1] = fmaxf(mx[1], fmaxf(sc[i + 2], sc[i + 3]));
+      }
+      float m_cand[2];
+      bool need = false;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+        m_cand[r] = fmaxf(m_used[r], fmaf(mx[r], c, amp));
+        // Lazy rescale: the reference rescales acc by exp2(m_old - m_new) every tile
+        // (:121-132).  O/l is invariant to the reference point, so it only moves when the
+        // max grew by more than 2^8 — the final O/l is the same up to fp32 rounding.
+        need = need || (m_cand[r] - m_used[r]) > 8.0f;   // false for NaN (-inf - -inf)
+      }
+      if (__any_sync(0xffffffffu, need)) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const float alpha = (m_cand[r] == -INFINITY) ? 1.0f : fast_exp2(m_used[r] - m_cand[r]);
+          l_sum[r] *= alpha;
+#pragma unroll
+          for (int i = 2 * r; i < 64; i += 4) {
+            o[i] *= alpha;
+            o[i + 1] *= alpha;
+          }
+          m_used[r] = m_cand[r];
+        }
+      }
+      // p = exp2(s*c + off); l accumulates the unrounded p (ref :131), P is rounded to the
+      // input dtype for the PV product (ref :128)
+      float off[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) off[r] = amp - ((m_used[r] == -INFINITY) ? 0.f : m_used[r]);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        const int r = (i >> 1) & 1;
+        sc[i] = fast_exp2(fmaf(sc[i], c, off[r]));
+        l_sum[r] += sc[i];
+      }
+
+      // ---- O += P V ----
+      mbar_wait(&bars[V_FULL + s], par, p.err_flag);
+      uint8_t* vs = sV + s * kTileBytes;
+      if constexpr (kPvFp8) {
+        // V^T[d][32 g + L] = V[32 g + perm(L)][d], perm(4 t + u) = {2t, 2t+1, 2t+8, 2t+9}[u] (+16 for
+        // t >= 4): the k-order of the e4m3 A fragment (4 consecutive k per byte quad) read off the
+        // f32 accumulator fragment (pairs of adjacent columns, 8 apart)
+        uint8_t* vt = vs + kBoxBytes;
+#pragma unroll
+        for (int it4 = 0; it4 < 4; ++it4) {
+          const int u = threadIdx.x + it4 * kConsumerThreads;
+          const int dc = u & 31, lc = u >> 5;
+          const int t = lc & 7;
+          const int k0 = (lc >> 3) * 32 + (t >= 4 ? 16 : 0) + 2 * (t & 3);
+          const uint32_t r0 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0, 4 * dc));
+          const uint32_t r1 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 1, 4 * dc));
+          const uint32_t r2 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 8, 4 * dc));
+          const uint32_t r3 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 9, 4 * dc));
+          const uint32_t lo01 = __byte_perm(r0, r1, 0x5140), hi01 = __byte_perm(r0, r1, 0x7362);
+          const uint32_t lo23 = __byte_perm(r2, r3, 0x5140), hi23 = __byte_perm(r2, r3, 0x7362);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 0, 4 * lc)) = __byte_perm(lo01, lo23, 0x5410);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 1, 4 * lc)) = __byte_perm(lo01, lo23, 0x7632);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 2, 4 * lc)) = __byte_perm(hi01, hi23, 0x5410);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 3, 4 * lc)) = __byte_perm(hi01, hi23, 0x7632);
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(2, kConsumerThreads);
+        uint32_t a[4][4];
+#pragma unroll
+        for (int kc = 0; kc < 4; ++kc) {
+          const float* x = sc + 16 * kc;
+          a[kc][0] = pack4_e4m3(x[0], x[1], x[4], x[5]);
+          a[kc][1] = pack4_e4m3(x[2], x[3], x[6], x[7]);
+          a[kc][2] = pack4_e4m3(x[8], x[9], x[12], x[13]);
+          a[kc][3] = pack4_e4m3(x[10], x[11], x[14], x[15]);
+        }
+        const uint32_t vt_addr = smem_u32(vt);
+        fence_regs(o);
+        wgmma_fence();
+#pragma unroll
+        for (int kc = 0; kc < 4; ++kc)
+          wgmma_128_rs_e4m3(o, a[kc], gmma_desc_sw128(vt_addr + kc * 32, 16, 1024), 1u);
+      } else {
+        uint32_t a[8][4];
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+          for (int t = 0; t < 4; ++t) a[kk][t] = pack2<kBF16>(sc[8 * kk + 2 * t], sc[8 * kk + 2 * t + 1]);
+        const uint32_t v_addr = smem_u32(vs);
+        fence_regs(o);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)   // 16 keys = 16 rows x 128 B inside each V box
+          wgmma_128_rs_bmn<kBF16>(o, a[kk], gmma_desc_sw128(v_addr + kk * 16 * 128, kBoxBytes, 1024), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars[V_EMPTY + s]);
+    }
+  }
+
+  // ---- epilogue: O / l -> global (ref :135-136); rows past the limit are zeros (:156) ----
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_sum[r] += __shfl_xor_sync(0xffffffffu, l_sum[r], 1);
+    l_sum[r] += __shfl_xor_sync(0xffffffffu, l_sum[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const long long q_row = q_row0 + row_lo + 8 * r;
     const bool in_tensor = q_row < p.q_rows;
     const bool zero_row = (n_tiles == 0) || (!dense && q_row >= q_limit_sparse);
-    float inv_l = zero_row ? 0.f : 1.0f / l_sum;
+    float inv_l = zero_row ? 0.f : 1.0f / l_sum[r];
     if constexpr (kPvFp8) inv_l *= __ldg(p.v_fp8_amax + b * p.heads + h) * (1.0f / 448.0f);   // undo the V scale
-    if (p.lse_out && dense && in_tensor) {
+    if (p.lse_out && dense && in_tensor && qd == 0) {
       // softmax_lse of flash_attn (natural log): ln sum_j exp(s_j * sm_scale) = (m + log2 l) * ln 2
       p.lse_out[(static_cast<long long>(b) * p.heads + h) * p.q_rows + q_row] =
-          zero_row ? -INFINITY : (m_used + log2f(l_sum)) * 0.6931471805599453f;
+          zero_row ? -INFINITY : (m_used[r] + log2f(l_sum[r])) * 0.6931471805599453f;
     }
+    if (!in_tensor) continue;
     // destination(s) of this row
     long long o_off = b * p.o_stride_b + q_row * p.o_stride_s + static_cast<long long>(h) * p.o_stride_h;
     uint16_t* obase = reinterpret_cast<uint16_t*>(p.out);
@@ -515,55 +372,21 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
         o_off = ((p.sp_rows + (q_row - n_img)) * p.sp_heads_total + gh) * kHeadDim;
       }
     }
-#pragma unroll 1
-    for (int cc = 0; cc < 128; cc += 32) {
-      uint32_t o[32];
-      if (n_tiles > 0) {
-        tmem_ld32(tmem_O + lane_base + cc, o);
-        tmem_ld_wait();
-      } else {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = 0;
-      }
-      if (in_tensor) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 v;
-          uint32_t* e = reinterpret_cast<uint32_t*>(&v);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const float a = zero_row ? 0.f : __uint_as_float(o[i + 2 * t]) * inv_l;
-            const float bb = zero_row ? 0.f : __uint_as_float(o[i + 2 * t + 1]) * inv_l;
-            e[t] = pack2<kBF16>(a, bb);
-          }
-          if (n_dst > 1) {
-            for (int r = 0; r < n_dst; ++r)
-              *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.peer_out[r]) + o_off + cc + i) = v;
-          } else if (!p.out_f32) {
-#if JENGA_ATTN_L2HINT
-            __stcs(reinterpret_cast<uint4*>(obase + o_off + cc + i), v);
-#else
-            *reinterpret_cast<uint4*>(obase + o_off + cc + i) = v;
-#endif
-          } else {  // wan/…:530-532: the 16-bit result is widened back to the query dtype
-            float* orow32 = reinterpret_cast<float*>(p.out) + o_off;
-            float2 t0 = unpack2<kBF16>(e[0]), t1 = unpack2<kBF16>(e[1]);
-            const float4 f0 = make_float4(t0.x, t0.y, t1.x, t1.y);
-            t0 = unpack2<kBF16>(e[2]);
-            t1 = unpack2<kBF16>(e[3]);
-            const float4 f1 = make_float4(t0.x, t0.y, t1.x, t1.y);
-            *reinterpret_cast<float4*>(orow32 + cc + i) = f0;
-            *reinterpret_cast<float4*>(orow32 + cc + i + 4) = f1;
-          }
-        }
+    for (int n8 = 0; n8 < 16; ++n8) {
+      const int i = 4 * n8 + 2 * r;
+      const int col = 8 * n8 + 2 * qd;
+      const uint32_t v = pack2<kBF16>(zero_row ? 0.f : o[i] * inv_l, zero_row ? 0.f : o[i + 1] * inv_l);
+      if (n_dst > 1) {
+        for (int rr = 0; rr < n_dst; ++rr)
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.peer_out[rr]) + o_off + col) = v;
+      } else if (!p.out_f32) {
+        *reinterpret_cast<uint32_t*>(obase + o_off + col) = v;
+      } else {  // wan/…:530-532: the 16-bit result is widened back to the query dtype
+        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + o_off + col) = unpack2<kBF16>(v);
       }
     }
   }
-
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 }  // namespace
@@ -589,13 +412,13 @@ static int make_tile_map(CUtensorMap* map, const void* base, int dtype, long lon
                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-// V as FP8: contiguous [B, S, H, 128] bytes; box {128 channels, 64 keys}
+// V as FP8: contiguous [B, S, H, 128] bytes; box {128 channels, 128 keys}
 static int make_v8_map(CUtensorMap* map, const void* base, long long rows, int heads, int batch) {
   const cuuint64_t dims[4] = {static_cast<cuuint64_t>(kHeadDim), static_cast<cuuint64_t>(rows),
                               static_cast<cuuint64_t>(heads), static_cast<cuuint64_t>(batch)};
   const cuuint64_t strides[3] = {static_cast<cuuint64_t>(heads) * kHeadDim, static_cast<cuuint64_t>(kHeadDim),
                                  static_cast<cuuint64_t>(rows) * heads * kHeadDim};
-  const cuuint32_t box[4] = {128, static_cast<cuuint32_t>(kHalf), 1, 1};
+  const cuuint32_t box[4] = {128, static_cast<cuuint32_t>(kBlock), 1, 1};
   const cuuint32_t elem_strides[4] = {1, 1, 1, 1};
   return encode_tensor_map(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void*>(base), dims, strides, box,
                            elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -646,19 +469,10 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream) {
        sp_head_base + a->heads > a->sp_heads_total))
     return set_error(JENGA_E_INVALID, "bad Ulysses head range");
 
-  // Kernel generation: 2 (default) or the experimental generation 6 via JENGA_ATTN_KERNEL=v6
-  // (tuning switch, same results up to fp32 rounding; profiles/README.md has the comparison).
-  static const int gen = [] {
-    const char* e = std::getenv("JENGA_ATTN_KERNEL");
-    if (e && std::strcmp(e, "v6") == 0) return 6;
-    if (e && std::strcmp(e, "v7") == 0) return 7;
-    return 2;
-  }();
-  const int kv_box_rows = gen == 6 ? kBlock : kHalf;
   const bool pv_fp8 = a->v_fp8 != nullptr;
   if (pv_fp8) {
-    if (!a->v_fp8_amax || gen != 2 || a->dtype != JENGA_BF16)
-      return set_error(JENGA_E_UNSUPPORTED, "fp8 P.V: needs v_fp8_amax, bf16 q/k and the default kernel generation");
+    if (!a->v_fp8_amax || a->dtype != JENGA_BF16)
+      return set_error(JENGA_E_UNSUPPORTED, "fp8 P.V: needs v_fp8_amax and bf16 q/k");
     if (reinterpret_cast<uintptr_t>(a->v_fp8) % 16) return set_error(JENGA_E_INVALID, "v_fp8 must be 16-byte aligned");
   }
   CUtensorMap tm_q, tm_k, tm_v;
@@ -667,12 +481,12 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream) {
                           a->q_stride_s, a->q_stride_h, kBlock)))
     return rc;
   if ((rc = make_tile_map(&tm_k, a->k, a->dtype, a->kv_rows, a->heads, a->batch, a->k_stride_b,
-                          a->k_stride_s, a->k_stride_h, kv_box_rows)))
+                          a->k_stride_s, a->k_stride_h, kBlock)))
     return rc;
   if (pv_fp8) {
     if ((rc = make_v8_map(&tm_v, a->v_fp8, a->kv_rows, a->heads, a->batch))) return rc;
   } else if ((rc = make_tile_map(&tm_v, a->v, a->dtype, a->kv_rows, a->heads, a->batch, a->v_stride_b,
-                                 a->v_stride_s, a->v_stride_h, kv_box_rows)))
+                                 a->v_stride_s, a->v_stride_h, kBlock)))
     return rc;
 
   KernelParams p{};
@@ -706,14 +520,9 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream) {
   p.err_flag = a->err_flag;
   p.lse_out = a->lse_out;
   p.v_fp8_amax = a->v_fp8_amax;
-  if (a->lse_out && gen == 6) return set_error(JENGA_E_UNSUPPORTED, "lse_out: not in generation 6");
 
   const long long grid = static_cast<long long>(a->batch) * a->heads * (a->nq_sparse + a->nq_dense);
   if (grid > 0x7fffffffll) return set_error(JENGA_E_UNSUPPORTED, "grid too large");
-  if (gen == 7)
-    return launch_carved_attn_v7(tm_q, tm_k, tm_v, p, a->batch * a->heads, a->dtype == JENGA_BF16, stream);
-  if (gen == 6)
-    return launch_carved_attn_v6(tm_q, tm_k, tm_v, p, static_cast<unsigned>(grid), a->dtype == JENGA_BF16, stream);
   auto kern = pv_fp8 ? carved_attn_fwd_kernel<true, true>
                      : (a->dtype == JENGA_BF16 ? carved_attn_fwd_kernel<true> : carved_attn_fwd_kernel<false>);
   cudaError_t ce = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);

@@ -1,6 +1,6 @@
-// Shared between the carved-attention kernel generations (carved_attn.cu, carved_attn_v6.cu).
+// Parameters and mask walker of the carved-attention kernel (carved_attn.cu).
 #pragma once
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "jenga_internal.h"
 
 namespace jenga {
@@ -56,10 +56,4 @@ struct BlockWalker {
 
 }  // namespace attn
 
-// kernel generation 6 (carved_attn_v6.cu): three tiles in flight over one accumulator
-int launch_carved_attn_v6(const CUtensorMap& tm_q, const CUtensorMap& tm_k, const CUtensorMap& tm_v,
-                          const attn::KernelParams& p, unsigned grid, bool bf16, cudaStream_t stream);
-// kernel generation 7 (carved_attn_v7.cu): two q blocks per CTA, interleaved P.V / Q.K^T issue
-int launch_carved_attn_v7(const CUtensorMap& tm_q, const CUtensorMap& tm_k, const CUtensorMap& tm_v,
-                          const attn::KernelParams& p, int batch_heads, bool bf16, cudaStream_t stream);
 }  // namespace jenga

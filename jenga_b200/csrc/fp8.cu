@@ -88,7 +88,7 @@ extern "C" int jenga_quantize_v_fp8(const void* v, int32_t dtype, int32_t batch,
   cudaError_t ce = cudaMemsetAsync(amax, 0, sizeof(float) * batch * heads, s);
   if (ce != cudaSuccess) return set_cuda_error(ce, "quantize_v_fp8 memset");
   long long per_head = (rows * 16 + 255) / 256;
-  const long long cap = (148ll * 8 + heads * batch - 1) / (heads * batch);
+  const long long cap = (static_cast<long long>(kNumSMs) * 8 + heads * batch - 1) / (heads * batch);
   if (per_head > cap) per_head = cap > 0 ? cap : 1;
   dim3 grid(static_cast<unsigned>(per_head), heads, batch);
   const uint16_t* vp = static_cast<const uint16_t*>(v);

@@ -194,7 +194,7 @@ extern "C" int jenga_gilbert_mapping_device(int t, int h, int w, int sliced, int
   if (!linear_to_hilbert && !hilbert_to_linear) return set_error(JENGA_E_INVALID, "gilbert_device: no output");
   const long long n = static_cast<long long>(t) * h * w;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148ll * 8) blocks = 148ll * 8;
+  if (blocks > static_cast<long long>(kNumSMs) * 8) blocks = static_cast<long long>(kNumSMs) * 8;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (sliced)
     gilbert_sliced_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(t, h, w, reinterpret_cast<long long*>(linear_to_hilbert),
@@ -217,7 +217,7 @@ extern "C" int jenga_block_neighbor_bits_device(int t, int h, int w, int block, 
   cudaError_t ce = cudaMemsetAsync(bits, 0, static_cast<size_t>(nb) * words * 4, s);
   if (ce != cudaSuccess) return set_cuda_error(ce, "neighbor_bits_device memset");
   long long blocks = (n + 255) / 256;
-  if (blocks > 148ll * 8) blocks = 148ll * 8;
+  if (blocks > static_cast<long long>(kNumSMs) * 8) blocks = static_cast<long long>(kNumSMs) * 8;
   neighbour_bits_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(t, h, w, block,
                                                                      reinterpret_cast<const long long*>(linear_to_hilbert), bits, words);
   ce = cudaGetLastError();

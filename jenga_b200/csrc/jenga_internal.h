@@ -8,6 +8,10 @@
 
 namespace jenga {
 
+// SMs of an H100 SXM: sizes the grids of the grid-stride (bandwidth-bound) kernels, whose results
+// do not depend on it.
+constexpr int kNumSMs = 132;
+
 // Records a thread-local message and returns `code` (printf-style).
 int set_error(int code, const char* fmt, ...);
 int set_cuda_error(cudaError_t e, const char* what);

@@ -25,7 +25,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "jenga_internal.h"
 
 namespace jenga {
@@ -161,8 +161,8 @@ __device__ __forceinline__ void cluster_sync_all() {
 }
 
 // kSplit == 1 (default): one CTA walks a 128-token block.  kSplit == 4 (experiment, see the launcher):
-// a thread-block cluster shares the block, 32 tokens per CTA, to shorten the last wave (903 uniform
-// work items on 296 CTA slots are 3.05 waves that run as 4); every CTA keeps fp32 partial sums of its
+// a thread-block cluster shares the block, 32 tokens per CTA, to shorten the partly filled last wave
+// of the 903 uniform work items at HY-720p; every CTA keeps fp32 partial sums of its
 // tokens, ranks 1..3 store theirs into rank 0's shared memory (st.shared::cluster) and rank 0 adds
 // them in rank order, so the pooled means stay deterministic.
 template <bool kBF16, int kSplit>
@@ -362,14 +362,13 @@ int hy_prologue_impl(const JengaHyPrologueArgs* a, cudaStream_t stream) {
   if (threads > 384) threads = 384;
   threads = ((threads + 31) / 32) * 32;
   // Default: one CTA per 128-token block.  JENGA_PROLOGUE_SPLIT=4 selects the experimental form with
-  // 4 CTAs per block (one thread-block cluster, DSMEM combine of the pooling sums).  Measured at
-  // HY-720p (profiles/README.md): 1.55 ms vs 1.12 ms — the 96 KB of partial-sum shared memory per CTA
-  // leaves the 24 heads of a token no L1 to share their cos/sin row in, and that costs more than the
-  // shorter last wave saves.  Its pooled means may differ from the default's in the last fp32 bit
+  // 4 CTAs per block (one thread-block cluster, DSMEM combine of the pooling sums).  The 96 KB of
+  // partial-sum shared memory per CTA leaves the 24 heads of a token no L1 to share their cos/sin row
+  // in.  Its pooled means may differ from the default's in the last fp32 bit
   // before the 16-bit rounding (4 x 32-token partial sums instead of one 128-token chain).
   static const int split = [] { const char* e = std::getenv("JENGA_PROLOGUE_SPLIT"); return (e && e[0] == '4') ? 4 : 1; }();
-  // Default: the bulk-async (cp.async.bulk) persistent form in prologue_bulk.cu — 0.75 ms against this
-  // file's 1.12 ms at HY-720p, q/k/v bit-identical (profiles/README.md).  It returns a positive value for
+  // Default: the bulk-async (cp.async.bulk) persistent form in prologue_bulk.cu, q/k/v bit-identical
+  // to this file's kernel.  It returns a positive value for
   // layouts it does not take (head stride != 128, > 24 heads, misaligned rows, first use on a stream
   // that is being captured into a graph) and then the register-staged kernel below runs instead.
   // JENGA_PROLOGUE=classic forces the kernel below (read per call: tests switch it in-process).
@@ -516,7 +515,7 @@ wan_prologue_kernel(const WanPrologueParams p) {
 // Experimental vector form (JENGA_WAN_PROLOGUE=vector|vector64; C % 8 == 0, 16-byte aligned rows): 128 threads
 // per token, the token's channels stay in registers (kVec 8-channel vectors per thread), one block reduction for
 // mean(x^2), 16-byte loads and stores.  Same arithmetic per element as wan_prologue_kernel above (the default);
-// only the fp32 summation order of mean(x^2) differs.  Measured slower than the default (see the launcher).
+// only the fp32 summation order of mean(x^2) differs.  Not the default (see the launcher).
 constexpr int kWanThreads = 128;
 
 template <int kVec>
@@ -653,10 +652,9 @@ int wan_prologue_impl(const JengaWanPrologueArgs* a, cudaStream_t stream) {
   p.remap = reinterpret_cast<const long long*>(a->freq_remap);
   p.out = static_cast<uint16_t*>(a->out);
   p.hilo = a->freqs ? a->freqs_hilo : nullptr;
-  // Default: the one-warp-per-token kernel (64 independent warps per SM; 0.64-0.72 ms at Wan-14B size = 0.37-0.49
-  // of the HBM peak).  JENGA_WAN_PROLOGUE=vector / vector64 select the experimental 128-threads-per-token kernel
+  // Default: the one-warp-per-token kernel (64 independent warps per SM).  JENGA_WAN_PROLOGUE=vector / vector64 select the experimental 128-threads-per-token kernel
   // (row in registers, 16-byte accesses, four complex factors per token and thread; rotation on the FP32 pipe
-  // with the (hi, lo) table, or in fp64): same results (tests), but 0.90-0.98 ms — with 120 registers it runs 16
+  // with the (hi, lo) table, or in fp64): same results (tests), but with 120 registers it runs 16
   // warps per SM behind one block barrier per token pair and cannot overlap its load and compute phases.
   const int esz = p.x_f32 ? 4 : 2, wsz = p.w_f32 ? 4 : 2;
   const char* wmode = std::getenv("JENGA_WAN_PROLOGUE");
@@ -670,7 +668,7 @@ int wan_prologue_impl(const JengaWanPrologueArgs* a, cudaStream_t stream) {
   (void)wsz;
   if (vec_ok) {
     long long pairs = (a->tokens + 1) / 2;
-    if (pairs > 148ll * 24) pairs = 148ll * 24;
+    if (pairs > static_cast<long long>(kNumSMs) * 24) pairs = static_cast<long long>(kNumSMs) * 24;
     dim3 grid(static_cast<unsigned>(pairs), static_cast<unsigned>(a->batch));
     const int per_thread = (p.C / 8 + kWanThreads - 1) / kWanThreads;
     switch (per_thread) {

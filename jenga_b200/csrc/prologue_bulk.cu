@@ -30,7 +30,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "jenga_internal.h"
 
 namespace jenga {

@@ -20,7 +20,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include "jenga_internal.h"
 
 namespace jenga {
@@ -475,7 +475,7 @@ pooled_scores_kernel(const uint16_t* __restrict__ q_pool, const uint16_t* __rest
 // Tensor-core form of the pooled-score GEMM (the reference does this step with a bf16 cuBLAS
 // bmm, …triton_diffres.py:227): mma.sync m16n8k16, 16-bit operands, fp32 accumulate, same two
 // rounding points on the way out.  Legacy warp-level MMA on purpose: the whole problem is
-// 5 GFLOP (24 heads x 900 x 900 x 128) — a tcgen05/TMEM pipeline would cost more to set up than
+// 5 GFLOP (24 heads x 900 x 900 x 128) — a wgmma pipeline would cost more to set up than
 // the math takes.  64x64 outputs per CTA, 4 warps of 32x32.
 __device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_ptr) {
   const uint32_t a = static_cast<uint32_t>(__cvta_generic_to_shared(smem_ptr));
@@ -717,15 +717,14 @@ int block_pool_impl(const void* x, void* pooled, void* cast_out, int in_dtype, i
   dim3 grid(n_blocks, batch);
   const int vecs = heads * head_dim / 8;
   // Threads per CTA: the largest multiple of 32 up to 192 that divides the CTA's 16-byte vectors, so every
-  // pass over a row is fully populated.  H=24 used 256 threads = one full pass + one half-empty pass:
-  // 0.162 ms; 128 or 192 threads: 0.131 ms = 0.82 of the measured HBM peak (L2 flushed between launches).
+  // pass over a row is fully populated (at H=24, 256 threads would be one full pass + one half-empty pass).
   int threads = vecs >= 256 ? 256 : ((vecs + 31) / 32) * 32;
   for (int t = 192; t >= 64; t -= 32)
     if (vecs % t == 0) {
       threads = t;
       break;
     }
-  if (const char* e = std::getenv("JENGA_POOL_THREADS")) {   // tuning experiment (profiles/README.md)
+  if (const char* e = std::getenv("JENGA_POOL_THREADS")) {   // tuning experiment
     const int t = std::atoi(e);
     if (t >= 32 && t <= 256 && t % 32 == 0) threads = t;
   }

@@ -67,7 +67,7 @@ residual_f32_kernel(const float* a, const float* __restrict__ b, float* out, lon
 int launch_residual(const void* a, const void* b, void* out, long long n, int dtype, bool sub, cudaStream_t s) {
   if (!a || !b || !out || n < 0) return set_error(JENGA_E_INVALID, "residual: null pointer / negative size");
   if (n == 0) return JENGA_OK;
-  const int grid = 148 * 8;
+  const int grid = kNumSMs * 8;
   if (dtype == JENGA_F32) {
     residual_f32_kernel<<<grid, 256, 0, s>>>(static_cast<const float*>(a), static_cast<const float*>(b),
                                              static_cast<float*>(out), n, sub ? 1 : 0);
@@ -254,7 +254,7 @@ extern "C" int jenga_prores_switch(const float* latents, const float* noise_pred
     return set_error(JENGA_E_INVALID, "prores_switch: bad shape");
   const long long total = static_cast<long long>(batch_channels) * out_t * out_h * out_w;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148ll * 16) blocks = 148ll * 16;
+  if (blocks > static_cast<long long>(kNumSMs) * 16) blocks = static_cast<long long>(kNumSMs) * 16;
   prores_switch_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       latents, noise_pred, noise, out, batch_channels, in_t, in_h, in_w, out_t, out_h, out_w, d_sigma, sigma_next);
   const cudaError_t ce = cudaGetLastError();

@@ -2,7 +2,7 @@
 steps run the 60-block loop, with which sa-drop rate, and a harness that executes exactly that
 many hot-path calls on synthetic activations to measure DiT-loop seconds per video for the
 part of the loop this repository implements (prologue + selection + carved attention; the
-dense layers of the DiT are out of scope, DESIGN.md §7).
+dense layers of the DiT are out of scope).
 
 Reference: jenga_hyvideo.py:28 (non_skip_steps), :128-179 (skip / residual reuse);
 pipeline_hunyuan_video_prores.py:697-698,763-767 (stage switch -> sa_drop_rates[stage], forced

@@ -1,4 +1,4 @@
-"""FlashAttention call sites of the hot path, served by the dense mode of the sm_100a kernel.
+"""FlashAttention call sites of the hot path, served by the dense mode of the sm_90a kernel.
 
 Shadows exactly what the reference imports (SURVEY §8b):
   flash_attn.flash_attn_func                       attention_block_triton_diffres.py:15,377

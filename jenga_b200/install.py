@@ -1,5 +1,5 @@
 """Makes the UNMODIFIED reference scripts (jenga_hyvideo.py, jenga_hyvideo_multigpu.py,
-jenga_hyi2v.py, jenga_wan.py) import the B200 path instead of Triton / FlashAttention / the
+jenga_hyi2v.py, jenga_wan.py) import the H100 path instead of Triton / FlashAttention / the
 Python gilbert module.
 
 The reference binds names at import time

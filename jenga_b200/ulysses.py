@@ -72,7 +72,7 @@ def gather_heads(x: torch.Tensor, group=None) -> torch.Tensor:
 class UlyssesCarvedAttention:
     """Callable with the signature the DiT blocks use for `hybrid_seq_parallel_attn`
     (xdit_ring_atten.py:61-85).  `attn_fn` is injectable so the CPU tests can exercise the
-    layout logic with the oracle; by default it is the sm_100a operator."""
+    layout logic with the oracle; by default it is the sm_90a operator."""
 
     def __init__(self, group=None, attn_fn=None, variant: str = "hyvideo"):
         self.group = group
@@ -186,15 +186,16 @@ class UlyssesFusedAttention:
     @staticmethod
     def _n_groups(h: int, want: int | None, q_blocks: int | None = None) -> int:
         """Head sub-groups per rank.  Each sub-group is its own attention launch of
-        (h/G) * q_blocks CTAs on 148 SMs x 2 CTAs: a launch of only a few waves pays its nearly
-        empty last wave (902 CTAs = 3.05 waves run as 4), which costs more than the exposed exchange
-        saves — so sub-groups are used only while every launch stays >= 12 waves."""
+        (h/G) * q_blocks CTAs, one per SM at a time on the 132 SMs of an H100: a launch of only a few
+        waves pays its nearly empty last wave (902 CTAs = 6.8 waves run as 7), which costs more than
+        the exposed exchange saves — so sub-groups are used only while every launch stays >= 12
+        waves."""
         if want:
             if h % want:
                 raise ValueError(f"{h} heads per rank do not split into {want} groups")
             return want
         for g in (3, 2):
-            if h % g == 0 and h >= g and (q_blocks is None or (h // g) * q_blocks >= 12 * 296):
+            if h % g == 0 and h >= g and (q_blocks is None or (h // g) * q_blocks >= 12 * 132):
                 return g
         return 1
 

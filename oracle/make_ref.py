@@ -16,6 +16,7 @@ tests/test_install_reference_*.py, bench.py's `gpu_reference` leg.
 from __future__ import annotations
 
 import hashlib
+import os
 import json
 import shutil
 import sys
@@ -61,7 +62,7 @@ FILES = [
 def materialise(src: Path = SRC, dst: Path = DST, quiet: bool = False) -> Path | None:
     """Copies FILES from `src` to `dst`.  Returns dst, or None when the reference is not mounted
     and nothing was materialised earlier (callers skip reference-backed checks then)."""
-    if not src.is_dir():
+    if not os.access(src, os.R_OK | os.X_OK) or not src.is_dir():   # absent, or not readable by this user
         return dst if (dst / "MANIFEST.json").exists() else None
     manifest = {}
     for rel in FILES:

@@ -35,7 +35,7 @@ def ref_root() -> Path | None:
     """The directory holding the unmodified reference files, or None."""
     import os
     live = Path("/root/reference")
-    if (live / "gilbert.py").is_file() and os.environ.get("JENGA_ORACLE_REF") != "staged":
+    if os.access(live / "gilbert.py", os.R_OK) and os.environ.get("JENGA_ORACLE_REF") != "staged":
         return live
     staged = HERE / "_ref"
     if (staged / "MANIFEST.json").is_file():
@@ -148,7 +148,7 @@ def reference_packages(product: bool = False):
     """Context in which `import hyvideo.modules.<file>` / `import wan.modules.<file>` resolve to the
     unmodified reference files.  product=False: the files see the reference's own Triton/FA2
     operator.  product=True: jenga_b200.install.install() has pre-seeded sys.modules first, so the
-    same unmodified files bind the B200 path at import time (the drop-in under test).
+    same unmodified files bind the H100 path at import time (the drop-in under test).
     Module objects imported inside stay usable after exit; sys.modules is restored so that a
     second context can import the same files with the other binding."""
     root = ref_root()

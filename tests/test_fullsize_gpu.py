@@ -1,4 +1,4 @@
-"""Full-size (BASELINE.json configs[1]: HunyuanVideo 720x1280x125f, S=115456, H=24) checks through
+"""Full-size (HunyuanVideo 720x1280x125f, S=115456, H=24: bench.py's hy720p workload) checks through
 size-independent properties, plus sampled rows against an fp32 torch evaluation on the GPU."""
 import math
 import sys
@@ -137,7 +137,7 @@ def _check_rows(q, k, v, out4, oh, n_img_blocks, seqlen, S_pad, rows_to_check, h
 
 
 def test_wan_1_3b_full_size_fp32_inputs():
-    """BASELINE configs[0]: Wan2.1-1.3B 832x480x81f — q,k fp32 [1,32760,12,128] (rope_apply returns
+    """Wan2.1-1.3B 832x480x81f — q,k fp32 [1,32760,12,128] (rope_apply returns
     .float()), v bf16, 8 zero-padded rows, sliced-gilbert adjacency, first-frame rule, fp32 output."""
     import bench
     from jenga_b200 import gilbert, wan
@@ -167,7 +167,7 @@ def test_wan_1_3b_full_size_fp32_inputs():
 
 
 def test_hyvideo_i2v_full_size_ragged():
-    """BASELINE configs[4] shape: 115200 image + 400 text tokens -> 904 blocks, text_blocks=4, the
+    """HunyuanVideo-I2V shape: 115200 image + 400 text tokens -> 904 blocks, text_blocks=4, the
     last block has 112 zero-padded rows that text queries DO attend (SURVEY A-3)."""
     import bench
     from jenga_b200 import gilbert

@@ -6,12 +6,14 @@ import pytest
 
 def test_ulysses_subgroup_rule_keeps_twelve_waves_per_launch():
     """Head sub-groups are used only while each sub-group's attention launch keeps >= 12 waves of CTAs on
-    148 SMs x 2 CTAs (jenga_b200/ulysses.py); an explicit request must divide the heads."""
+    132 SMs x 1 CTA (jenga_b200/ulysses.py); an explicit request must divide the heads."""
     from jenga_b200.ulysses import UlyssesFusedAttention as U
     n = U._n_groups
-    assert n(12, None, 902) == 3          # N=2 at HY-720p: 4 heads x 902 q blocks = 12.2 waves per launch
-    assert n(3, None, 902) == 1           # N=8: one head per launch would be 3.05 waves
-    assert n(6, None, 902) == 1           # N=4: 2 x 902 = 6.1 waves (3 groups), 3 x 902 = 9.1 (2 groups): neither reaches 12
+    assert n(12, None, 902) == 3          # N=2 at HY-720p: 4 heads x 902 q blocks = 27.3 waves per launch
+    assert n(3, None, 902) == 1           # N=8: one head per launch would be 6.8 waves
+    assert n(6, None, 902) == 3           # N=4: 2 x 902 = 13.7 waves per launch (3 groups)
+    assert n(6, None, 600) == 2           # 2 x 600 = 9.1 waves (3 groups) is too few, 3 x 600 = 13.6 (2 groups)
+    assert n(6, None, 400) == 1           # 6.1 waves (3 groups), 9.1 (2 groups): neither reaches 12
     assert n(12, None, None) == 3         # no shape given: the head count decides
     assert n(12, 2, 902) == 2 and n(12, 1, 902) == 1
     with pytest.raises(ValueError):

@@ -45,7 +45,7 @@ CASES = [
     (2, 333, 45, 5, torch.bfloat16, True, True, True, 4),       # odd head count, batch 2, ragged
     (1, 512, 0, 24, torch.float16, False, True, True, 3),       # fp16, no weights, no text
     (1, 384, 64, 8, torch.bfloat16, True, False, False, 0),     # no RoPE
-    (1, 148 * 128 + 5 * 128 + 17, 256, 4, torch.bfloat16, True, True, True, 0),  # > 148 blocks on the real grid
+    (1, 148 * 128 + 5 * 128 + 17, 256, 4, torch.bfloat16, True, True, True, 0),  # > 132 blocks (H100 SMs) on the real grid
 ]
 
 
