@@ -22,46 +22,63 @@ def pad_rows(x: torch.Tensor, rows: int) -> torch.Tensor:
 
 
 @torch.no_grad()
-def fp64_truth(q, k, v, onehot, qblocks, *, n_img_blocks, seqlen, text_amp=0.0, sm_scale=None):
-    """Exact softmax attention in fp64 for the query blocks `qblocks` of every head.
+def fp64_truth(q, k, v, onehot, qblocks, *, n_img_blocks, seqlen, text_amp=0.0, sm_scale=None,
+               text_block_start=None, kv_limit=None, q_limit=None, kv_limit_dense=None, return_lse=False):
+    """Exact softmax attention in fp64 for the query blocks `qblocks` of every batch and head.
 
-    q,k,v: [1,S,H,D] device tensors (any float dtype; values are taken as they are),
-    onehot: [1,H,n_img_blocks,nb] bool — the block mask of the image rows.
-    Image rows (block < n_img_blocks): keys = mask-selected blocks, key columns >= seqlen hidden,
-    text key blocks (>= n_img_blocks) biased by text_amp in log2 units
-    (…triton_diffres.py:96-118).  Text rows: dense over ALL nb*128 keys incl. padding, no bias
-    (:371-380).  Returns {qb: [H,128,D] float64}."""
-    _, S, H, D = q.shape
+    q: [B,Sq,H,D], k,v: [B,Sk,H,D] tensors on one device (any float dtype; values are taken as
+    they are; Sq and Sk are independent, keys past Sk are zeros),
+    onehot: [B,H,n_img_blocks,nb] bool — the block mask of the image rows, nb*128 >= Sk.
+    Image rows (block < n_img_blocks): keys = mask-selected blocks, key columns >= kv_limit
+    (default seqlen) hidden, key blocks >= text_block_start (default n_img_blocks) biased by
+    text_amp in log2 units (…triton_diffres.py:96-118); when q_limit is given, rows >= q_limit
+    are zeros (:59-61, :136).  Text rows: dense over ALL nb*128 keys incl. padding, no bias
+    (:371-380), or over the keys below kv_limit_dense when it is given.
+    Returns {qb: [H,128,D] float64} for B == 1 and {qb: [B,H,128,D]} otherwise; with
+    return_lse=True also {qb: [H,128] or [B,H,128]}, the natural-log logsumexp of s * sm_scale of
+    the text rows (flash_attn's softmax_lse)."""
+    B, Sq, H, D = q.shape
     nb = onehot.shape[-1]
     Sp = nb * BLOCK
     sm_scale = D ** -0.5 if sm_scale is None else sm_scale
-    kd = pad_rows(k, Sp)[0].transpose(0, 1).double()          # [H,Sp,D]
-    vd = pad_rows(v, Sp)[0].transpose(0, 1).double()
-    qd = pad_rows(q, Sp)[0].transpose(0, 1)
+    kv_limit = seqlen if kv_limit is None else kv_limit
+    text_block_start = n_img_blocks if text_block_start is None else text_block_start
+    Sqp = (max(qblocks) + 1) * BLOCK
+    kd = pad_rows(k, Sp).transpose(1, 2).double()                # [B,H,Sp,D]
+    vd = pad_rows(v, Sp).transpose(1, 2).double()
+    qd = pad_rows(q[:, :Sqp], Sqp).transpose(1, 2)
     cols = torch.arange(Sp, device=q.device)
-    out = {}
+    rows = torch.arange(BLOCK, device=q.device)
+    out, lse = {}, {}
     for qb in qblocks:
-        Q = qd[:, qb * BLOCK:(qb + 1) * BLOCK].double()        # [H,128,D]
-        s = torch.matmul(Q, kd.transpose(1, 2)) * sm_scale     # [H,128,Sp]
+        Q = qd[:, :, qb * BLOCK:(qb + 1) * BLOCK].double()      # [B,H,128,D]
+        s = torch.matmul(Q, kd.transpose(-1, -2)) * sm_scale     # [B,H,128,Sp]
         if qb < n_img_blocks:
-            live = onehot[0, :, qb].repeat_interleave(BLOCK, dim=-1)            # [H,Sp]
+            live = onehot[:, :, qb].repeat_interleave(BLOCK, dim=-1)             # [B,H,Sp]
             if text_amp != 0.0:
-                s[:, :, n_img_blocks * BLOCK:] += text_amp * LN2
-            dead = (~live)[:, None, :] | (cols >= seqlen)[None, None, :]
+                s[..., text_block_start * BLOCK:] += text_amp * LN2
+            dead = (~live)[:, :, None, :] | (cols >= kv_limit)
             s = s.masked_fill(dead, float("-inf"))
+        elif kv_limit_dense is not None:
+            s = s.masked_fill(cols >= kv_limit_dense, float("-inf"))
         p = torch.softmax(s, dim=-1)
-        out[qb] = torch.matmul(p, vd)
+        o = torch.matmul(p, vd)
+        if qb < n_img_blocks and q_limit is not None:
+            o[:, :, qb * BLOCK + rows >= q_limit] = 0.0
+        if return_lse and qb >= n_img_blocks:
+            lse[qb] = torch.logsumexp(s, dim=-1)[0] if B == 1 else torch.logsumexp(s, dim=-1)
+        out[qb] = o[0] if B == 1 else o
         del s, p
-    return out
+    return (out, lse) if return_lse else out
 
 
 def error_stats(got, truth: dict, *, seqlen_rows=None):
-    """got: [1,S,H*D] or [1,S,H,D]; truth from fp64_truth.  Returns (max|e|/rms, mean|e|/rms, rms)
+    """got: [B,S,H*D] or [B,S,H,D]; truth from fp64_truth.  Returns (max|e|/rms, mean|e|/rms, rms)
     over the sampled blocks (rows >= seqlen_rows of a block are skipped: both implementations
     leave them zero / undefined)."""
     any_t = next(iter(truth.values()))
-    H, _, D = any_t.shape
-    g = got.reshape(1, got.shape[1], H, D)
+    H, D = any_t.shape[-3], any_t.shape[-1]
+    g = got.reshape(got.shape[0], got.shape[1], H, D)
     num_max, num_sum, cnt, sq = 0.0, 0.0, 0, 0.0
     for qb, t in truth.items():
         r0 = qb * BLOCK
@@ -70,8 +87,10 @@ def error_stats(got, truth: dict, *, seqlen_rows=None):
             r1 = min(r1, seqlen_rows)
         if r1 <= r0:
             continue
-        x = g[0, r0:r1].transpose(0, 1).double()
-        tt = t[:, : r1 - r0]
+        x = g[:, r0:r1].transpose(1, 2).double()
+        if t.dim() == 3:
+            x = x[0]
+        tt = t[..., : r1 - r0, :]
         e = (x - tt).abs()
         num_max = max(num_max, e.max().item())
         num_sum += e.sum().item()
