@@ -4,15 +4,27 @@
 //   hyvideo/modules/attention_block_triton_diffres.py:38-136 (+ launcher :139-196)
 // and its text-row flash_attn_func call (:371-380) with ONE launch.
 //
-// Work decomposition: one CTA per (batch*head, 128-row query block); 288 threads:
-//   warps 0..7  two consumer warpgroups of 64 query rows each: S = Q~ K^T by wgmma (Q and K from
-//               shared memory, S in registers), online softmax in base 2 on the registers, then
-//               O += P V by wgmma with P as the register A operand; final O / l -> global
-//   warp 8      TMA producer: Q once, then one K tile and one V tile per live key block into a
-//               two-stage ring (K and V slots are released separately, so the next K tile lands
-//               while the P.V product of the current one runs)
+// Work decomposition: one CTA per (batch*head, 128-row query block); 384 threads, three warpgroups:
+//   warpgroups 0, 1  consumers, 64 query rows each: S = Q~ K^T by wgmma (Q and K from shared
+//                    memory, S in registers), online softmax in base 2 on the registers, then
+//                    O += P V by wgmma with P as the register A operand; final O / l -> global
+//   warpgroup 2      producer: warp 8 issues TMA — Q once, then one K tile and one V tile per live
+//                    key block into a two-stage ring (K and V slots are released separately);
+//                    with FP8 P.V, warps 9..11 transpose each V tile (see kPvFp8)
+// setmaxnreg moves registers from the producer (24, or 40 with the FP8 transpose) to the consumers
+// (240, or 232): S, O and the packed P of the previous tile are all live in a consumer at once.
+//
+// Consumer schedule (FlashAttention-3's):
+//   - in-warpgroup pipelining: iteration j issues S_j = Q~ K_j^T, then O += P_{j-1} V_{j-1}; it
+//     waits for S_j alone, runs softmax_j while P_{j-1} V_{j-1} is still on the tensor cores, then
+//     waits for that and applies the lazy rescale O *= alpha_j.  The prologue computes S_0 and its
+//     softmax, the epilogue issues the last P V.  O and l see the same operations in the same
+//     order as a plain S, softmax, P V loop, so the result is the same bit for bit.
+//   - ping-pong: the two warpgroups take turns to issue their GEMMs (named barriers kBarTurn and
+//     kBarTurn + 1), so one warpgroup's softmax runs while the other's GEMMs occupy the tensor
+//     cores.  Warpgroup 0 goes first.
 // S and O are fp32 register accumulators (64 + 64 registers per thread); one CTA per SM with
-// ~164 KB of shared memory, two warpgroups whose softmax and MMA phases interleave on the SM.
+// ~164 KB of shared memory.
 //
 // HBM/L2 layout: q,k,v stay in the caller's [B,S,H,D] layout; TMA boxes are {64 d, 128 rows}
 // with 128-byte swizzle.  K boxes are K-major wgmma operands, V boxes MN-major (no transpose).
@@ -29,11 +41,14 @@ using attn::KernelParams;
 constexpr int kBlock = 128;           // rows per q block == keys per kv block
 constexpr int kHeadDim = 128;
 constexpr int kConsumerThreads = 256;
-constexpr int kThreads = kConsumerThreads + 32;
+constexpr int kThreads = kConsumerThreads + 128;  // + the producer warpgroup
+constexpr int kTransposeWarps = 3;               // producer warps 9..11 (FP8 P.V only)
 constexpr int kStages = 2;                       // K/V ring depth
 constexpr int kBoxBytes = kBlock * 64 * 2;       // 16 KB: 128 rows x 64 d (one TMA box)
 constexpr int kTileBytes = 2 * kBoxBytes;        // 32 KB: 128 rows x 128 d (two d halves)
 constexpr int kMaxMaskWords = 256;               // up to 8192 key blocks (1M tokens)
+constexpr uint32_t kBarQScaled = 1;              // named barrier: Q~ written by both consumer warpgroups
+constexpr uint32_t kBarTurn = 3;                 // named barriers 3, 4: consumer warpgroup 0's, 1's turn
 
 // shared-memory carve-up (offsets from the 1024-aligned base)
 constexpr int kOffQ = 0;
@@ -47,7 +62,8 @@ enum BarId {
   Q_FULL = 0,
   K_FULL = 1, V_FULL = K_FULL + kStages,
   K_EMPTY = V_FULL + kStages, V_EMPTY = K_EMPTY + kStages,   // one arrival per consumer warp
-  NUM_BARS = V_EMPTY + kStages
+  VT_FULL = V_EMPTY + kStages,                                // FP8: one arrival per transpose warp
+  NUM_BARS = VT_FULL + kStages
 };
 static_assert(NUM_BARS * 8 <= 128, "barrier block overflow");
 
@@ -59,9 +75,11 @@ __device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t col) {
 // kPvFp8 (opt-in): P and V enter the P.V product as FP8 e4m3 — V quantised per head by
 // jenga_quantize_v_fp8 (scale = absmax/448), P converted with cvt.rn.satfinite.e4m3x2 (p <= 2^8 by
 // the lazy-rescale bound, e4m3 max 448) — through wgmma m64n128k32 e4m3 (half the P.V tensor cycles).
-// 8-bit wgmma operands must be K-major, so the consumers transpose each V tile in shared memory
-// into V^T with the keys of every 32-key group permuted to match the order in which the S
-// accumulator fragment already holds P: no shuffles of P.  Q.K^T, the softmax and l are unchanged.
+// 8-bit wgmma operands must be K-major, so three producer warps transpose each V tile in shared
+// memory into V^T (the upper half of the V slot) with the keys of every 32-key group permuted to
+// match the order in which the S accumulator fragment already holds P: no shuffles of P.  The
+// consumers wait for V^T on VT_FULL instead of V_FULL and otherwise run the same schedule.
+// Q.K^T, the softmax and l are unchanged.
 template <bool kBF16, bool kPvFp8 = false>
 __global__ void __launch_bounds__(kThreads, 1)
 carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
@@ -118,7 +136,8 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
 #pragma unroll
-    for (int i = 0; i < NUM_BARS; ++i) mbar_init(&bars[i], i >= K_EMPTY ? 8u : 1u);
+    for (int i = 0; i < NUM_BARS; ++i)
+      mbar_init(&bars[i], i >= VT_FULL ? kTransposeWarps : (i >= K_EMPTY ? 8u : 1u));
     fence_mbar_init();
   }
   __syncthreads();
@@ -126,39 +145,73 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
   int n_tiles = 0;
   for (int w = 0; w < nwords; ++w) n_tiles += __popc(s_mask[w]);
 
-  if (warp == kConsumerThreads / 32) {
-    // =============================== TMA producer ===============================
-    if (n_tiles > 0 && lane == 0) {
-      mbar_arrive_expect_tx(&bars[Q_FULL], kTileBytes);
-      tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
-      tma_load_4d(sQ + kBoxBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b);
-      BlockWalker it(s_mask, nwords);
-      int j = 0;
-      for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
-        const int s = j % kStages;
-        const uint32_t par = ((j / kStages) & 1) ^ 1;   // slot-free parity (a fresh barrier passes)
-        const int row0 = blk * kBlock;
-        uint8_t* k_dst = sK + s * kTileBytes;
-        uint8_t* v_dst = sV + s * kTileBytes;
-        mbar_wait(&bars[K_EMPTY + s], par, p.err_flag);
-        mbar_arrive_expect_tx(&bars[K_FULL + s], kTileBytes);
-        tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
-        tma_load_4d(k_dst + kBoxBytes, &tm_k, &bars[K_FULL + s], 64, row0, h, b);
-        mbar_wait(&bars[V_EMPTY + s], par, p.err_flag);
-        if constexpr (kPvFp8) {   // 128 keys x 128 one-byte channels = one 16 KB box
-          mbar_arrive_expect_tx(&bars[V_FULL + s], kBoxBytes);
-          tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
-        } else {
-          mbar_arrive_expect_tx(&bars[V_FULL + s], kTileBytes);
-          tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
-          tma_load_4d(v_dst + kBoxBytes, &tm_v, &bars[V_FULL + s], 64, row0, h, b);
+  if (warp >= kConsumerThreads / 32) {
+    // =============================== producer warpgroup ===============================
+    setmaxnreg_dec<kPvFp8 ? 40 : 24>();
+    if (warp == kConsumerThreads / 32) {
+      if (n_tiles > 0 && lane == 0) {   // TMA
+        mbar_arrive_expect_tx(&bars[Q_FULL], kTileBytes);
+        tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
+        tma_load_4d(sQ + kBoxBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b);
+        BlockWalker it(s_mask, nwords);
+        int j = 0;
+        for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
+          const int s = j % kStages;
+          const uint32_t par = ((j / kStages) & 1) ^ 1;   // slot-free parity (a fresh barrier passes)
+          const int row0 = blk * kBlock;
+          uint8_t* k_dst = sK + s * kTileBytes;
+          uint8_t* v_dst = sV + s * kTileBytes;
+          mbar_wait(&bars[K_EMPTY + s], par, p.err_flag);
+          mbar_arrive_expect_tx(&bars[K_FULL + s], kTileBytes);
+          tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
+          tma_load_4d(k_dst + kBoxBytes, &tm_k, &bars[K_FULL + s], 64, row0, h, b);
+          mbar_wait(&bars[V_EMPTY + s], par, p.err_flag);
+          if constexpr (kPvFp8) {   // 128 keys x 128 one-byte channels = one 16 KB box
+            mbar_arrive_expect_tx(&bars[V_FULL + s], kBoxBytes);
+            tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
+          } else {
+            mbar_arrive_expect_tx(&bars[V_FULL + s], kTileBytes);
+            tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
+            tma_load_4d(v_dst + kBoxBytes, &tm_v, &bars[V_FULL + s], 64, row0, h, b);
+          }
         }
+      }
+    } else if constexpr (kPvFp8) {
+      // V^T[d][32 g + L] = V[32 g + perm(L)][d], perm(4 t + u) = {2t, 2t+1, 2t+8, 2t+9}[u] (+16 for
+      // t >= 4): the k-order of the e4m3 A fragment (4 consecutive k per byte quad) read off the
+      // f32 accumulator fragment (pairs of adjacent columns, 8 apart).  V^T is written into the
+      // unused upper half of the slot, which the consumers free together with V (V_EMPTY).
+      const int t0 = threadIdx.x - kConsumerThreads - 32;
+      for (int j = 0; j < n_tiles; ++j) {
+        const int s = j % kStages;
+        mbar_wait(&bars[V_FULL + s], (j / kStages) & 1, p.err_flag);
+        const uint8_t* vs = sV + s * kTileBytes;
+        uint8_t* vt = sV + s * kTileBytes + kBoxBytes;
+        for (int u = t0; u < kBlock * kHeadDim / 16; u += kTransposeWarps * 32) {
+          const int dc = u & 31, lc = u >> 5;
+          const int t = lc & 7;
+          const int k0 = (lc >> 3) * 32 + (t >= 4 ? 16 : 0) + 2 * (t & 3);
+          const uint32_t r0 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0, 4 * dc));
+          const uint32_t r1 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 1, 4 * dc));
+          const uint32_t r2 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 8, 4 * dc));
+          const uint32_t r3 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 9, 4 * dc));
+          const uint32_t lo01 = __byte_perm(r0, r1, 0x5140), hi01 = __byte_perm(r0, r1, 0x7362);
+          const uint32_t lo23 = __byte_perm(r2, r3, 0x5140), hi23 = __byte_perm(r2, r3, 0x7362);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 0, 4 * lc)) = __byte_perm(lo01, lo23, 0x5410);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 1, 4 * lc)) = __byte_perm(lo01, lo23, 0x7632);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 2, 4 * lc)) = __byte_perm(hi01, hi23, 0x5410);
+          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 3, 4 * lc)) = __byte_perm(hi01, hi23, 0x7632);
+        }
+        fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core proxy
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars[VT_FULL + s]);
       }
     }
     return;
   }
 
   // =============================== consumers ===============================
+  setmaxnreg_inc<kPvFp8 ? 232 : 240>();
   const int wg = warp >> 2;                       // warpgroup: query rows [64 wg, 64 wg + 64)
   const int g = lane >> 2, qd = lane & 3;
   // accumulator fragment: element i of a thread is row g + 8 ((i >> 1) & 1) of the warp's 16 rows,
@@ -190,39 +243,57 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
         q4[threadIdx.x + i * kConsumerThreads] = v;
       }
       fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core proxy
-      named_bar_sync(1, kConsumerThreads);
+      named_bar_sync(kBarQScaled, kConsumerThreads);
     }
     const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128;   // this warpgroup's 64 rows of each d half
 
-    BlockWalker it(s_mask, nwords);
-    int j = 0;
-    for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
-      const int s = j % kStages;
-      const uint32_t par = (j / kStages) & 1;
+    float sc[64];                      // S_j, then P_j in fp32
+    uint32_t pa[kPvFp8 ? 4 : 8][4];    // P_{j-1}: A operand of the P.V wgmma; untouched while it runs
+    float alpha[2];
+
+    // Turns: a warpgroup waits on its own barrier before it issues GEMMs and arrives on the
+    // other's once they are issued.  Warpgroup 1 arrives ahead for warpgroup 0's first turn and
+    // skips the hand-over after its own last turn: both take the same number of turns, so every
+    // barrier sees as many arrivals as waits.
+    auto turn_begin = [&] { named_bar_sync(kBarTurn + wg, kConsumerThreads); };
+    auto turn_end = [&](bool last) {
+      if (!(last && wg == 1)) named_bar_arrive(kBarTurn + (wg ^ 1), kConsumerThreads);
+    };
+    auto release = [&](int bar) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars[bar]);
+    };
+    // ---- S = Q~ K^T (64 x 128 per warpgroup, K = 128 in 8 steps) ----
+    auto issue_qk = [&](int s) {
+      const uint32_t k_addr = smem_u32(sK + s * kTileBytes);
+#pragma unroll
+      for (int kk = 0; kk < kHeadDim / 16; ++kk) {
+        const uint32_t off = (kk & 3) * 32 + (kk >> 2) * kBoxBytes;
+        wgmma_128_ss<kBF16>(sc, gmma_desc_sw128(q_addr + off, 16, 1024),
+                            gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+    };
+    // ---- O += P V ----
+    auto issue_pv = [&](int s) {
+      if constexpr (kPvFp8) {
+        const uint32_t vt_addr = smem_u32(sV + s * kTileBytes + kBoxBytes);
+#pragma unroll
+        for (int kc = 0; kc < 4; ++kc)
+          wgmma_128_rs_e4m3(o, pa[kc], gmma_desc_sw128(vt_addr + kc * 32, 16, 1024), 1u);
+      } else {
+        const uint32_t v_addr = smem_u32(sV + s * kTileBytes);
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)   // 16 keys = 16 rows x 128 B inside each V box
+          wgmma_128_rs_bmn<kBF16>(o, pa[kk], gmma_desc_sw128(v_addr + kk * 16 * 128, kBoxBytes, 1024), 1u);
+      }
+      wgmma_commit();
+    };
+    // ---- online softmax of key block blk on sc; true when O must be rescaled by alpha ----
+    auto softmax = [&](int blk) -> bool {
       // ref :113-114 — text_amp is a constant added to every score of a text key block, in
       // log2 units (sparse class only, where c == 1): fold it into the exponent offset.
       const float amp = (!dense && blk >= p.text_block_start) ? p.text_amp : 0.f;
-
-      // ---- S = Q~ K^T (64 x 128 per warpgroup, K = 128 in 8 steps) ----
-      float sc[64];
-      mbar_wait(&bars[K_FULL + s], par, p.err_flag);
-      {
-        const uint32_t k_addr = smem_u32(sK + s * kTileBytes);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < kHeadDim / 16; ++kk) {
-          const uint32_t off = (kk & 3) * 32 + (kk >> 2) * kBoxBytes;
-          wgmma_128_ss<kBF16>(sc, gmma_desc_sw128(q_addr + off, 16, 1024),
-                              gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(sc);
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[K_EMPTY + s]);
-
-      // ---- online softmax on the registers ----
       const long long col0 = static_cast<long long>(blk) * kBlock;
       if (col0 + kBlock > kv_limit) {  // rare: only the tile that straddles seqlen
 #pragma unroll
@@ -247,16 +318,12 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
         // max grew by more than 2^8 — the final O/l is the same up to fp32 rounding.
         need = need || (m_cand[r] - m_used[r]) > 8.0f;   // false for NaN (-inf - -inf)
       }
-      if (__any_sync(0xffffffffu, need)) {
+      const bool rescale = __any_sync(0xffffffffu, need);
+      if (rescale) {
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-          const float alpha = (m_cand[r] == -INFINITY) ? 1.0f : fast_exp2(m_used[r] - m_cand[r]);
-          l_sum[r] *= alpha;
-#pragma unroll
-          for (int i = 2 * r; i < 64; i += 4) {
-            o[i] *= alpha;
-            o[i + 1] *= alpha;
-          }
+          alpha[r] = (m_cand[r] == -INFINITY) ? 1.0f : fast_exp2(m_used[r] - m_cand[r]);
+          l_sum[r] *= alpha[r];
           m_used[r] = m_cand[r];
         }
       }
@@ -271,68 +338,82 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
         sc[i] = fast_exp2(fmaf(sc[i], c, off[r]));
         l_sum[r] += sc[i];
       }
-
-      // ---- O += P V ----
-      mbar_wait(&bars[V_FULL + s], par, p.err_flag);
-      uint8_t* vs = sV + s * kTileBytes;
-      if constexpr (kPvFp8) {
-        // V^T[d][32 g + L] = V[32 g + perm(L)][d], perm(4 t + u) = {2t, 2t+1, 2t+8, 2t+9}[u] (+16 for
-        // t >= 4): the k-order of the e4m3 A fragment (4 consecutive k per byte quad) read off the
-        // f32 accumulator fragment (pairs of adjacent columns, 8 apart)
-        uint8_t* vt = vs + kBoxBytes;
+      return rescale;
+    };
+    auto rescale_o = [&] {
 #pragma unroll
-        for (int it4 = 0; it4 < 4; ++it4) {
-          const int u = threadIdx.x + it4 * kConsumerThreads;
-          const int dc = u & 31, lc = u >> 5;
-          const int t = lc & 7;
-          const int k0 = (lc >> 3) * 32 + (t >= 4 ? 16 : 0) + 2 * (t & 3);
-          const uint32_t r0 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0, 4 * dc));
-          const uint32_t r1 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 1, 4 * dc));
-          const uint32_t r2 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 8, 4 * dc));
-          const uint32_t r3 = *reinterpret_cast<const uint32_t*>(vs + sw128(k0 + 9, 4 * dc));
-          const uint32_t lo01 = __byte_perm(r0, r1, 0x5140), hi01 = __byte_perm(r0, r1, 0x7362);
-          const uint32_t lo23 = __byte_perm(r2, r3, 0x5140), hi23 = __byte_perm(r2, r3, 0x7362);
-          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 0, 4 * lc)) = __byte_perm(lo01, lo23, 0x5410);
-          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 1, 4 * lc)) = __byte_perm(lo01, lo23, 0x7632);
-          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 2, 4 * lc)) = __byte_perm(hi01, hi23, 0x5410);
-          *reinterpret_cast<uint32_t*>(vt + sw128(4 * dc + 3, 4 * lc)) = __byte_perm(hi01, hi23, 0x7632);
+      for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int i = 2 * r; i < 64; i += 4) {
+          o[i] *= alpha[r];
+          o[i + 1] *= alpha[r];
         }
-        fence_proxy_async_smem();
-        named_bar_sync(2, kConsumerThreads);
-        uint32_t a[4][4];
+    };
+    auto pack_p = [&] {
+      if constexpr (kPvFp8) {
 #pragma unroll
         for (int kc = 0; kc < 4; ++kc) {
           const float* x = sc + 16 * kc;
-          a[kc][0] = pack4_e4m3(x[0], x[1], x[4], x[5]);
-          a[kc][1] = pack4_e4m3(x[2], x[3], x[6], x[7]);
-          a[kc][2] = pack4_e4m3(x[8], x[9], x[12], x[13]);
-          a[kc][3] = pack4_e4m3(x[10], x[11], x[14], x[15]);
+          pa[kc][0] = pack4_e4m3(x[0], x[1], x[4], x[5]);
+          pa[kc][1] = pack4_e4m3(x[2], x[3], x[6], x[7]);
+          pa[kc][2] = pack4_e4m3(x[8], x[9], x[12], x[13]);
+          pa[kc][3] = pack4_e4m3(x[10], x[11], x[14], x[15]);
         }
-        const uint32_t vt_addr = smem_u32(vt);
-        fence_regs(o);
-        wgmma_fence();
-#pragma unroll
-        for (int kc = 0; kc < 4; ++kc)
-          wgmma_128_rs_e4m3(o, a[kc], gmma_desc_sw128(vt_addr + kc * 32, 16, 1024), 1u);
       } else {
-        uint32_t a[8][4];
 #pragma unroll
         for (int kk = 0; kk < 8; ++kk)
 #pragma unroll
-          for (int t = 0; t < 4; ++t) a[kk][t] = pack2<kBF16>(sc[8 * kk + 2 * t], sc[8 * kk + 2 * t + 1]);
-        const uint32_t v_addr = smem_u32(vs);
-        fence_regs(o);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)   // 16 keys = 16 rows x 128 B inside each V box
-          wgmma_128_rs_bmn<kBF16>(o, a[kk], gmma_desc_sw128(v_addr + kk * 16 * 128, kBoxBytes, 1024), 1u);
+          for (int t = 0; t < 4; ++t) pa[kk][t] = pack2<kBF16>(sc[8 * kk + 2 * t], sc[8 * kk + 2 * t + 1]);
       }
-      wgmma_commit();
+    };
+    constexpr int kVReady = kPvFp8 ? VT_FULL : V_FULL;
+
+    if (wg == 1) named_bar_arrive(kBarTurn, kConsumerThreads);
+    BlockWalker it(s_mask, nwords);
+    // prologue: S_0 and its softmax
+    int blk = it.next();
+    mbar_wait(&bars[K_FULL], 0, p.err_flag);
+    turn_begin();
+    wgmma_fence();
+    issue_qk(0);
+    turn_end(false);
+    wgmma_wait<0>();
+    fence_regs(sc);
+    release(K_EMPTY);
+    if (softmax(blk)) rescale_o();
+    pack_p();
+    int j = 1;
+    for (blk = it.next(); blk >= 0; blk = it.next(), ++j) {   // S_j and P_{j-1} V_{j-1}
+      const int s = j % kStages, sv = (j - 1) % kStages;
+      mbar_wait(&bars[kVReady + sv], ((j - 1) / kStages) & 1, p.err_flag);
+      mbar_wait(&bars[K_FULL + s], (j / kStages) & 1, p.err_flag);
+      turn_begin();
+      fence_regs(o);
+      wgmma_fence();
+      issue_qk(s);
+      issue_pv(sv);
+      turn_end(false);
+      wgmma_wait<1>();
+      fence_regs(sc);
+      release(K_EMPTY + s);
+      const bool rescale = softmax(blk);
       wgmma_wait<0>();
       fence_regs(o);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[V_EMPTY + s]);
+      release(V_EMPTY + sv);
+      if (rescale) rescale_o();
+      pack_p();
     }
+    // epilogue: P V of the last tile
+    const int sv = (j - 1) % kStages;
+    mbar_wait(&bars[kVReady + sv], ((j - 1) / kStages) & 1, p.err_flag);
+    turn_begin();
+    fence_regs(o);
+    wgmma_fence();
+    issue_pv(sv);
+    turn_end(true);
+    wgmma_wait<0>();
+    fence_regs(o);
+    release(V_EMPTY + sv);
   }
 
   // ---- epilogue: O / l -> global (ref :135-136); rows past the limit are zeros (:156) ----

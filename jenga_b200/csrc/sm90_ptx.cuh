@@ -169,6 +169,21 @@ __device__ __forceinline__ uint32_t pack4_e4m3(float a, float b, float c, float 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// counts the calling threads towards barrier `id` without waiting for it to complete
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// Per-warpgroup register budget (all 128 threads of the warpgroup execute it).  N is a multiple
+// of 8 in [24, 256]; the CTA's total may not exceed what it was launched with.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 // ---------------------------------------------------------------------------------------------
 // Small numeric helpers
