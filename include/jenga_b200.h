@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define JENGA_B200_ABI_VERSION 2
+#define JENGA_B200_ABI_VERSION 3
 
 enum {
   JENGA_OK = 0,
@@ -303,13 +303,6 @@ typedef struct JengaWanPrologueArgs {
   int32_t grid_f, grid_h, grid_w;
   const int64_t* freq_remap;
   void* out;
-  /* optional, used by the experimental vector kernel only (JENGA_WAN_PROLOGUE=vector; the default kernel
-   * rotates in fp64 like the reference): the same table split into fp32 pairs,
-   * [freq_rows, 64, 4] = (re_hi, im_hi, re_lo, im_lo) with hi = (float)x, lo = (float)(x - hi).  The
-   * rotation then runs on the FP32 pipe with compensated products and sums (error ~2^-45 relative, i.e.
-   * the correctly rounded fp32 of the complex128 product except ~1e-6 of the elements by one fp32 ulp,
-   * invisible after the bf16 cast). */
-  const float* freqs_hilo;
 } JengaWanPrologueArgs;
 
 int jenga_wan_prologue(const JengaWanPrologueArgs* args, void* stream);

@@ -8,11 +8,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-import os
-
-_PKG = Path(__file__).resolve().parent
-# JENGA_B200_LIB selects a tuning variant built by `python -m jenga_b200.build --variant ...`
-LIB_PATH = Path(os.environ.get("JENGA_B200_LIB") or (_PKG / "_C" / "libjenga_b200.so"))
+LIB_PATH = Path(__file__).resolve().parent / "_C" / "libjenga_b200.so"
 
 JENGA_BF16, JENGA_F16, JENGA_F32 = 0, 1, 2
 
@@ -92,7 +88,7 @@ class JengaWanPrologueArgs(C.Structure):
         ("stride_b", C.c_int64), ("stride_s", C.c_int64), ("eps", C.c_float),
         ("freqs", C.c_void_p), ("freq_rows", C.c_int32),
         ("grid_f", C.c_int32), ("grid_h", C.c_int32), ("grid_w", C.c_int32),
-        ("freq_remap", C.c_void_p), ("out", C.c_void_p), ("freqs_hilo", C.c_void_p),
+        ("freq_remap", C.c_void_p), ("out", C.c_void_p),
     ]
 
 
@@ -176,7 +172,7 @@ def _load() -> C.CDLL:
     lib.jenga_quantize_v_fp8.restype = C.c_int
     lib.jenga_gilbert_xyz2d.argtypes = [C.c_int] * 6
     lib.jenga_gilbert_xyz2d.restype = C.c_int64
-    if lib.jenga_abi_version() != 2:
+    if lib.jenga_abi_version() != 3:
         raise JengaError("libjenga_b200.so ABI version mismatch")
     return lib
 

@@ -55,14 +55,9 @@ def _fingerprint() -> str:
     return h.hexdigest()
 
 
-def build(force: bool = False, verbose: bool = False, defines: tuple[str, ...] = (),
-          variant: str | None = None) -> Path:
-    """Compile every translation unit and link the shared library.  Idempotent.
-    `defines`/`variant` build a tuning variant (libjenga_b200.<variant>.so) next to the default
-    library; select it at run time with JENGA_B200_LIB=<path> (kernel-tuning sweeps only)."""
+def build(force: bool = False, verbose: bool = False) -> Path:
+    """Compile every translation unit and link the shared library.  Idempotent."""
     OUT_DIR.mkdir(exist_ok=True)
-    if variant:
-        return _build_variant(defines, variant, verbose)
     fp = _fingerprint()
     if not force and LIB.exists() and STAMP.exists() and STAMP.read_text().strip() == fp:
         return LIB
@@ -93,38 +88,6 @@ def build(force: bool = False, verbose: bool = False, defines: tuple[str, ...] =
     return LIB
 
 
-def _build_variant(defines, variant, verbose):
-    nvcc = _nvcc()
-    vdir = OUT_DIR / f"variant_{variant}"
-    vdir.mkdir(exist_ok=True)
-    objs = []
-    for src in _sources():
-        obj = vdir / (src.stem + ".o")
-        cmd = [nvcc, *NVCC_FLAGS, *[f"-D{d}" for d in defines], "-I", str(ROOT / "include"), "-I", str(CSRC),
-               "-x", "cu", "-c", str(src), "-o", str(obj)]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        if r.returncode != 0:
-            sys.stderr.write(r.stdout + r.stderr)
-            raise RuntimeError(f"nvcc failed on {src.name}")
-        if verbose:
-            print(r.stderr)
-        objs.append(obj)
-    out = OUT_DIR / f"libjenga_b200.{variant}.so"
-    cmd = [nvcc, "-shared", "-o", str(out), *map(str, objs), *GENCODE,
-           "-Xcompiler", "-fPIC", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(r.stdout + r.stderr)
-        raise RuntimeError("link failed")
-    return out
-
-
 if __name__ == "__main__":
-    if "--variant" in sys.argv:
-        i = sys.argv.index("--variant")
-        name = sys.argv[i + 1]
-        defs = tuple(a[2:] for a in sys.argv if a.startswith("-D"))
-        print(build(defines=defs, variant=name, verbose="-v" in sys.argv))
-        sys.exit(0)
     p = build(force="--force" in sys.argv, verbose="-v" in sys.argv)
     print(p)

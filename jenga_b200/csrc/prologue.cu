@@ -20,7 +20,6 @@
 // (8 channels per lane), so the norm reduction is 4 shuffles and each lane keeps the pooling
 // partial sums of its own 8 channels across the 128 tokens of the block.
 #include <cstdlib>
-#include <cstring>
 
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -66,17 +65,6 @@ struct PrologueParams {
   int nb;                       // ceil(S / 128)
 };
 
-template <bool kBF16>
-__device__ __forceinline__ void load8(const uint16_t* p, float (&f)[8]) {
-  const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 t = unpack2<kBF16>(w[i]);
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
-}
 template <bool kBF16>
 __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   uint4 v;
@@ -130,57 +118,18 @@ __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
   }
 }
 
-// Tokens are processed in groups of kGroup with all of a group's q/k/v loads issued before any
-// arithmetic: the kernel is a pure stream (37 KB in + out per token per CTA), so what matters is
-// bytes in flight per SM — ~1.7 us of HBM latency x 44 GB/s per SM ~ 75 KB.
-#ifndef JENGA_PRO_GROUP
-#define JENGA_PRO_GROUP 1
-#endif
-#ifndef JENGA_PRO_MINB
-#define JENGA_PRO_MINB 2
-#endif
-constexpr int kGroup = JENGA_PRO_GROUP;
-
-// ---- thread-block-cluster helpers (distributed shared memory) ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t map_to_rank(uint32_t smem_addr, uint32_t rank) {
-  uint32_t a;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_addr), "r"(rank));
-  return a;
-}
-__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float4 v) {
-  asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-               : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// kSplit == 1 (default): one CTA walks a 128-token block.  kSplit == 4 (experiment, see the launcher):
-// a thread-block cluster shares the block, 32 tokens per CTA, to shorten the partly filled last wave
-// of the 903 uniform work items at HY-720p; every CTA keeps fp32 partial sums of its
-// tokens, ranks 1..3 store theirs into rank 0's shared memory (st.shared::cluster) and rank 0 adds
-// them in rank order, so the pooled means stay deterministic.
-template <bool kBF16, int kSplit>
-__global__ void __launch_bounds__(384, (kSplit == 1 ? JENGA_PRO_MINB : 2))
+template <bool kBF16>
+__global__ void __launch_bounds__(384, 2)
 hy_prologue_kernel(const PrologueParams p) {
-  constexpr int kGroup = kSplit == 1 ? JENGA_PRO_GROUP : 1;
   __shared__ float s_w[4][128];  // img_q, img_k, txt_q, txt_k norm weights
-  extern __shared__ float s_part[];   // [kSplit][H][2 (q,k)][128] partial sums (rank 0's copy is used)
-  constexpr int kTokPerCta = kBlock / kSplit;
-  const int blk = blockIdx.x / kSplit;
-  const int part = kSplit > 1 ? static_cast<int>(cluster_ctarank()) : 0;
+  const int blk = blockIdx.x;
   const int b = blockIdx.y;
   const int S = p.L + p.T;
   const int lane16 = threadIdx.x & 15;  // 8-channel chunk inside the head row
   const int d0 = lane16 * 8;
   const int rows_per_iter = blockDim.x >> 4;  // (token, head) rows handled per pass
-  const long long tok0 = static_cast<long long>(blk) * kBlock + part * kTokPerCta;
-  const int n_tok = static_cast<int>(max(0ll, min(static_cast<long long>(kTokPerCta), S - tok0)));
+  const long long tok0 = static_cast<long long>(blk) * kBlock;
+  const int n_tok = static_cast<int>(max(0ll, min(static_cast<long long>(kBlock), S - tok0)));
   const bool has_w = p.w_img_q != nullptr;
   if (has_w) {
     for (int i = threadIdx.x; i < 4 * 128; i += blockDim.x) {
@@ -191,7 +140,6 @@ hy_prologue_kernel(const PrologueParams p) {
     }
   }
   __syncthreads();
-  const uint32_t part_base = smem_u32(s_part);
 
   // A thread always serves the same head set {h : (h - hslot) % rows_per_iter == 0} so its
   // pooling accumulators are per (head, chunk).  With H <= rows_per_iter (24 <= 24) that is
@@ -203,112 +151,62 @@ hy_prologue_kernel(const PrologueParams p) {
     float qsum[8], ksum[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) qsum[i] = ksum[i] = 0.f;
-    for (int t0 = 0; t0 < n_tok; t0 += kGroup) {
-      // all of a group's loads are issued before any arithmetic: the kernel is a pure stream, what
-      // matters is bytes in flight per SM (~1.7 us of HBM latency x 44 GB/s per SM ~ 75 KB)
-      uint4 rq[kGroup], rk[kGroup], rv[kGroup];
-      float4 rc[kGroup][2], rs[kGroup][2];
+    for (int t = 0; t < n_tok; ++t) {
+      const long long tok = tok0 + t;
+      const bool is_img = tok < p.L;
+      const uint16_t* src = is_img ? p.img + b * p.img_sb + tok * p.img_ss + h * p.img_sh + d0
+                                   : p.txt + b * p.txt_sb + (tok - p.L) * p.txt_ss + h * p.txt_sh + d0;
+      const long long sw = is_img ? p.img_sw : p.txt_sw;
+      const uint4 rq = __ldg(reinterpret_cast<const uint4*>(src));
+      const uint4 rk = __ldg(reinterpret_cast<const uint4*>(src + sw));
+      const uint4 rv = __ldg(reinterpret_cast<const uint4*>(src + 2 * sw));
+      float4 rc[2], rs[2];
+      if (is_img && p.cos_t) {
+        const long long row = p.rope_index ? __ldg(p.rope_index + tok) : tok;
+        const float4* cp = reinterpret_cast<const float4*>(p.cos_t + row * 128 + d0);
+        const float4* sp = reinterpret_cast<const float4*>(p.sin_t + row * 128 + d0);
+        rc[0] = __ldg(cp);
+        rc[1] = __ldg(cp + 1);
+        rs[0] = __ldg(sp);
+        rs[1] = __ldg(sp + 1);
+      }
+      float q[8], k[8], wq[8], wk[8];
+      unpack8<kBF16>(rq, q);
+      unpack8<kBF16>(rk, k);
+      if (has_w) {
+        const float* wqs = s_w[is_img ? 0 : 2] + d0;
+        const float* wks = s_w[is_img ? 1 : 3] + d0;
 #pragma unroll
-      for (int g = 0; g < kGroup; ++g) {
-        const long long tok = tok0 + t0 + g;
-        if (t0 + g < n_tok) {
-          const bool is_img = tok < p.L;
-          const uint16_t* src = is_img ? p.img + b * p.img_sb + tok * p.img_ss + h * p.img_sh + d0
-                                       : p.txt + b * p.txt_sb + (tok - p.L) * p.txt_ss + h * p.txt_sh + d0;
-          const long long sw = is_img ? p.img_sw : p.txt_sw;
-          rq[g] = __ldg(reinterpret_cast<const uint4*>(src));
-          rk[g] = __ldg(reinterpret_cast<const uint4*>(src + sw));
-          rv[g] = __ldg(reinterpret_cast<const uint4*>(src + 2 * sw));
-          if (is_img && p.cos_t) {
-            const long long row = p.rope_index ? __ldg(p.rope_index + tok) : tok;
-            const float4* cp = reinterpret_cast<const float4*>(p.cos_t + row * 128 + d0);
-            const float4* sp = reinterpret_cast<const float4*>(p.sin_t + row * 128 + d0);
-            rc[g][0] = __ldg(cp);
-            rc[g][1] = __ldg(cp + 1);
-            rs[g][0] = __ldg(sp);
-            rs[g][1] = __ldg(sp + 1);
-          }
+        for (int i = 0; i < 8; ++i) {
+          wq[i] = wqs[i];
+          wk[i] = wks[i];
         }
       }
+      // tested again rather than reusing is_img: with is_img kept live across the loads, the f16
+      // instantiation spills 8 more bytes per thread
+      const bool rotate = tok < p.L && p.cos_t != nullptr;
+      norm_rope8<kBF16>(q, wq, has_w, p.eps, rotate, rc, rs, half_mask);
+      norm_rope8<kBF16>(k, wk, has_w, p.eps, rotate, rc, rs, half_mask);
+      const long long o = ((static_cast<long long>(b) * S + tok) * p.H + h) * 128 + d0;
+      *reinterpret_cast<uint4*>(p.q + o) = pack8<kBF16>(q);
+      *reinterpret_cast<uint4*>(p.k + o) = pack8<kBF16>(k);
+      *reinterpret_cast<uint4*>(p.v + o) = rv;
 #pragma unroll
-      for (int g = 0; g < kGroup; ++g) {
-        const long long tok = tok0 + t0 + g;
-        if (t0 + g < n_tok) {   // uniform across the CTA
-          const bool is_img = tok < p.L;
-          float q[8], k[8], wq[8], wk[8];
-          unpack8<kBF16>(rq[g], q);
-          unpack8<kBF16>(rk[g], k);
-          if (has_w) {
-            const float* wqs = s_w[is_img ? 0 : 2] + d0;
-            const float* wks = s_w[is_img ? 1 : 3] + d0;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              wq[i] = wqs[i];
-              wk[i] = wks[i];
-            }
-          }
-          const bool rotate = is_img && p.cos_t != nullptr;
-          norm_rope8<kBF16>(q, wq, has_w, p.eps, rotate, rc[g], rs[g], half_mask);
-          norm_rope8<kBF16>(k, wk, has_w, p.eps, rotate, rc[g], rs[g], half_mask);
-          const long long o = ((static_cast<long long>(b) * S + tok) * p.H + h) * 128 + d0;
-          *reinterpret_cast<uint4*>(p.q + o) = pack8<kBF16>(q);
-          *reinterpret_cast<uint4*>(p.k + o) = pack8<kBF16>(k);
-          *reinterpret_cast<uint4*>(p.v + o) = rv[g];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            qsum[i] += q[i];
-            ksum[i] += k[i];
-          }
-        }
+      for (int i = 0; i < 8; ++i) {
+        qsum[i] += q[i];
+        ksum[i] += k[i];
       }
     }
     if (p.q_pool) {
-      if constexpr (kSplit == 1) {
-        float qm[8], km[8];
+      float qm[8], km[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          qm[i] = qsum[i] * (1.0f / kBlock);  // missing tail rows count as zeros (padding)
-          km[i] = ksum[i] * (1.0f / kBlock);
-        }
-        const long long o = ((static_cast<long long>(b) * p.H + h) * p.nb + blk) * 128 + d0;
-        *reinterpret_cast<uint4*>(p.q_pool + o) = pack8<kBF16>(qm);
-        *reinterpret_cast<uint4*>(p.k_pool + o) = pack8<kBF16>(km);
-      } else {
-        // [part][h][q|k][128] floats in rank 0's shared memory
-        const uint32_t local = part_base + static_cast<uint32_t>((((part * p.H + h) * 2) * 128 + d0) * 4);
-        const uint32_t dst = map_to_rank(local, 0);
-        st_cluster_f4(dst, make_float4(qsum[0], qsum[1], qsum[2], qsum[3]));
-        st_cluster_f4(dst + 16, make_float4(qsum[4], qsum[5], qsum[6], qsum[7]));
-        st_cluster_f4(dst + 512, make_float4(ksum[0], ksum[1], ksum[2], ksum[3]));
-        st_cluster_f4(dst + 528, make_float4(ksum[4], ksum[5], ksum[6], ksum[7]));
+      for (int i = 0; i < 8; ++i) {
+        qm[i] = qsum[i] * (1.0f / kBlock);  // missing tail rows count as zeros (padding)
+        km[i] = ksum[i] * (1.0f / kBlock);
       }
-    }
-  }
-  if constexpr (kSplit > 1) {
-    cluster_sync_all();   // every rank's partial sums have landed in rank 0's shared memory
-    if (p.q_pool && part == 0) {
-      for (int h = hslot; h < p.H; h += rows_per_iter) {
-        float qm[8], km[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) qm[i] = km[i] = 0.f;
-#pragma unroll
-        for (int r = 0; r < kSplit; ++r) {
-          const float* src = s_part + (((r * p.H + h) * 2) * 128 + d0);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            qm[i] = r == 0 ? src[i] : qm[i] + src[i];
-            km[i] = r == 0 ? src[128 + i] : km[i] + src[128 + i];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          qm[i] *= (1.0f / kBlock);
-          km[i] *= (1.0f / kBlock);
-        }
-        const long long o = ((static_cast<long long>(b) * p.H + h) * p.nb + blk) * 128 + d0;
-        *reinterpret_cast<uint4*>(p.q_pool + o) = pack8<kBF16>(qm);
-        *reinterpret_cast<uint4*>(p.k_pool + o) = pack8<kBF16>(km);
-      }
+      const long long o = ((static_cast<long long>(b) * p.H + h) * p.nb + blk) * 128 + d0;
+      *reinterpret_cast<uint4*>(p.q_pool + o) = pack8<kBF16>(qm);
+      *reinterpret_cast<uint4*>(p.k_pool + o) = pack8<kBF16>(km);
     }
   }
 }
@@ -361,12 +259,6 @@ int hy_prologue_impl(const JengaHyPrologueArgs* a, cudaStream_t stream) {
   int threads = a->heads * 16;
   if (threads > 384) threads = 384;
   threads = ((threads + 31) / 32) * 32;
-  // Default: one CTA per 128-token block.  JENGA_PROLOGUE_SPLIT=4 selects the experimental form with
-  // 4 CTAs per block (one thread-block cluster, DSMEM combine of the pooling sums).  The 96 KB of
-  // partial-sum shared memory per CTA leaves the 24 heads of a token no L1 to share their cos/sin row
-  // in.  Its pooled means may differ from the default's in the last fp32 bit
-  // before the 16-bit rounding (4 x 32-token partial sums instead of one 128-token chain).
-  static const int split = [] { const char* e = std::getenv("JENGA_PROLOGUE_SPLIT"); return (e && e[0] == '4') ? 4 : 1; }();
   // Default: the bulk-async (cp.async.bulk) persistent form in prologue_bulk.cu, q/k/v bit-identical
   // to this file's kernel.  It returns a positive value for
   // layouts it does not take (head stride != 128, > 24 heads, misaligned rows, first use on a stream
@@ -374,35 +266,15 @@ int hy_prologue_impl(const JengaHyPrologueArgs* a, cudaStream_t stream) {
   // JENGA_PROLOGUE=classic forces the kernel below (read per call: tests switch it in-process).
   const char* mode = std::getenv("JENGA_PROLOGUE");
   const bool classic = mode && mode[0] == 'c';
-  if (!classic && split == 1) {
+  if (!classic) {
     const int r = hy_prologue_bulk_try(a, stream);
     if (r <= 0) return r;
   }
-  const size_t part_bytes = static_cast<size_t>(4) * a->heads * 2 * 128 * sizeof(float);
-  if (split == 4 && part_bytes <= 200 * 1024) {
-    auto kern = a->dtype == JENGA_BF16 ? hy_prologue_kernel<true, 4> : hy_prologue_kernel<false, 4>;
-    cudaError_t ce0 = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(part_bytes));
-    if (ce0 != cudaSuccess) return set_cuda_error(ce0, "cudaFuncSetAttribute(hy_prologue)");
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(p.nb) * 4u, a->batch);
-    cfg.blockDim = dim3(threads);
-    cfg.dynamicSmemBytes = part_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 4;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    ce0 = cudaLaunchKernelEx(&cfg, kern, p);
-    return ce0 == cudaSuccess ? JENGA_OK : set_cuda_error(ce0, "hy_prologue cluster launch");
-  }
   dim3 grid(p.nb, a->batch);
   if (a->dtype == JENGA_BF16)
-    hy_prologue_kernel<true, 1><<<grid, threads, 0, stream>>>(p);
+    hy_prologue_kernel<true><<<grid, threads, 0, stream>>>(p);
   else
-    hy_prologue_kernel<false, 1><<<grid, threads, 0, stream>>>(p);
+    hy_prologue_kernel<false><<<grid, threads, 0, stream>>>(p);
   cudaError_t ce = cudaGetLastError();
   return ce == cudaSuccess ? JENGA_OK : set_cuda_error(ce, "hy_prologue launch");
 }
@@ -430,20 +302,7 @@ struct WanPrologueParams {
   int gf, gh, gw;       // latent grid (F, H, W); tokens >= F*H*W get no rotation (:66)
   const long long* remap;  // optional [F*H*W]: position of token i (hilbert_order)
   uint16_t* out;        // [B, L, H, 128] bf16, contiguous
-  const float* hilo;    // optional [rows, 64, 4] fp32 split of freqs (vector kernel, FP32-pipe rotation)
 };
-
-// a*fa - b*fb with fa = fah + fal, fb = fbh + fbl: products split exactly with an FMA, the difference
-// of the leading terms with a two-sum, everything small added in plain fp32 (relative error ~2^-45)
-__device__ __forceinline__ float comp_diff(float a, float fah, float fal, float b, float fbh, float fbl) {
-  const float p1 = __fmul_rn(a, fah), e1 = __fmaf_rn(a, fah, -p1);
-  const float p2 = __fmul_rn(b, fbh), e2 = __fmaf_rn(b, fbh, -p2);
-  const float s = __fsub_rn(p1, p2);
-  const float bb = __fsub_rn(s, p1);
-  const float err = __fadd_rn(__fsub_rn(p1, __fsub_rn(s, bb)), __fsub_rn(-p2, bb));
-  const float small = __fadd_rn(__fadd_rn(__fsub_rn(e1, e2), err), __fsub_rn(__fmul_rn(a, fal), __fmul_rn(b, fbl)));
-  return __fadd_rn(s, small);
-}
 
 __device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
@@ -511,125 +370,6 @@ wan_prologue_kernel(const WanPrologueParams p) {
   }
 }
 
-
-// Experimental vector form (JENGA_WAN_PROLOGUE=vector|vector64; C % 8 == 0, 16-byte aligned rows): 128 threads
-// per token, the token's channels stay in registers (kVec 8-channel vectors per thread), one block reduction for
-// mean(x^2), 16-byte loads and stores.  Same arithmetic per element as wan_prologue_kernel above (the default);
-// only the fp32 summation order of mean(x^2) differs.  Not the default (see the launcher).
-constexpr int kWanThreads = 128;
-
-template <int kVec>
-__global__ void __launch_bounds__(2 * kWanThreads)
-wan_prologue_vec_kernel(const WanPrologueParams p) {
-  __shared__ float s_red[2][2][4];                    // [iteration parity][token of the CTA][warp]
-  const int sub = threadIdx.x / kWanThreads;          // two tokens per CTA
-  const int t = threadIdx.x - sub * kWanThreads;
-  const int warp = t >> 5, lane = t & 31;
-  const int b = blockIdx.y;
-  const int nvec = p.C / 8;
-  const long long n_grid = static_cast<long long>(p.gf) * p.gh * p.gw;
-  const int c3 = 64 / 3;              // 21
-  const int s0 = 64 - 2 * c3;         // 22: split sizes [22, 21, 21] (:44)
-  int par = 0;
-  for (long long pair = blockIdx.x; pair * 2 < p.L; pair += gridDim.x, par ^= 1) {
-    const long long tok = pair * 2 + sub;
-    const bool live = tok < p.L;                      // both halves of the CTA take the barrier
-    float f[kVec][8];
-    float ss = 0.f;
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) {
-      const int v = t + j * kWanThreads;
-      if (live && v < nvec) {
-        if (p.x_f32) {
-          const float4* src = reinterpret_cast<const float4*>(static_cast<const float*>(p.x) + b * p.sb + tok * p.ss) + 2 * v;
-          const float4 lo = __ldg(src), hi = __ldg(src + 1);
-          f[j][0] = lo.x; f[j][1] = lo.y; f[j][2] = lo.z; f[j][3] = lo.w;
-          f[j][4] = hi.x; f[j][5] = hi.y; f[j][6] = hi.z; f[j][7] = hi.w;
-        } else {
-          const uint4 raw = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.x) + b * p.sb + tok * p.ss) + v);
-          unpack8<true>(raw, f[j]);
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) ss = fmaf(f[j][i], f[j][i], ss);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f[j][i] = 0.f;
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    if (lane == 0) s_red[par][sub][warp] = ss;
-    __syncthreads();   // the other parity's slots are rewritten only after the next iteration's barrier
-    const float* rr = s_red[par][sub];
-    const float r = rsqrtf((rr[0] + rr[1] + rr[2] + rr[3]) / static_cast<float>(p.C) + p.eps);
-    if (!live) continue;
-    const bool rotate = tok < n_grid && p.freqs != nullptr;
-    // The rotation of a channel depends on its position inside the head only, and a thread's vectors
-    // t, t+128, ... all sit at the same position ((8t) mod 128): four complex factors per token serve
-    // every vector of the thread.
-    float4 fr32[4];
-    double2 fr64[4];
-    if (rotate) {
-      const long long pos = p.remap ? __ldg(p.remap + tok) : tok;
-      const int fi = static_cast<int>(pos / (static_cast<long long>(p.gh) * p.gw));
-      const int rem = static_cast<int>(pos - static_cast<long long>(fi) * p.gh * p.gw);
-      const int hi_ = rem / p.gw;
-      const int wi = rem - hi_ * p.gw;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int jj = (t & 15) * 4 + i;                     // complex index inside the head
-        const int row = jj < s0 ? fi : (jj < s0 + c3 ? hi_ : wi);
-        const long long idx = static_cast<long long>(row) * 64 + jj;
-        if (p.hilo) fr32[i] = __ldg(reinterpret_cast<const float4*>(p.hilo) + idx);
-        else fr64[i] = __ldg(reinterpret_cast<const double2*>(p.freqs) + idx);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) {
-      const int v = t + j * kWanThreads;
-      if (v >= nvec) continue;
-      float wv[8];
-      if (!p.w) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) wv[i] = 1.0f;
-      } else if (p.w_f32) {
-        const float4* wp = reinterpret_cast<const float4*>(static_cast<const float*>(p.w)) + 2 * v;
-        const float4 lo = __ldg(wp), hi = __ldg(wp + 1);
-        wv[0] = lo.x; wv[1] = lo.y; wv[2] = lo.z; wv[3] = lo.w; wv[4] = hi.x; wv[5] = hi.y; wv[6] = hi.z; wv[7] = hi.w;
-      } else {
-        unpack8<true>(__ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.w)) + v), wv);
-      }
-      uint32_t packed[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float y[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float val = __fmul_rn(f[j][2 * i + e], r);        // _norm in fp32
-          if (!p.x_f32) val = bf16_round(val);               // .type_as(x)
-          val = __fmul_rn(val, wv[2 * i + e]);               // * self.weight (promotes to fp32 unless both bf16)
-          if (!p.x_f32 && !p.w_f32) val = bf16_round(val);
-          y[e] = val;
-        }
-        float o0 = y[0], o1 = y[1];
-        if (rotate) {
-          if (p.hilo) {   // (re_hi, im_hi, re_lo, im_lo): the complex128 product rounded to fp32, on the FP32 pipe
-            o0 = comp_diff(y[0], fr32[i].x, fr32[i].z, y[1], fr32[i].y, fr32[i].w);      // a*re - b*im
-            o1 = comp_diff(y[0], fr32[i].y, fr32[i].w, -y[1], fr32[i].x, fr32[i].z);     // a*im + b*re
-          } else {
-            const double a = static_cast<double>(y[0]), bb = static_cast<double>(y[1]);
-            o0 = static_cast<float>(a * fr64[i].x - bb * fr64[i].y);      // complex128 product, then .float()
-            o1 = static_cast<float>(a * fr64[i].y + bb * fr64[i].x);
-          }
-        }
-        packed[i] = pack2<true>(o0, o1);
-      }
-      *(reinterpret_cast<uint4*>(p.out + (static_cast<long long>(b) * p.L + tok) * p.C) + v) =
-          make_uint4(packed[0], packed[1], packed[2], packed[3]);
-    }
-  }
-}
-
 }  // namespace
 
 int wan_prologue_impl(const JengaWanPrologueArgs* a, cudaStream_t stream) {
@@ -651,37 +391,6 @@ int wan_prologue_impl(const JengaWanPrologueArgs* a, cudaStream_t stream) {
   p.gf = a->grid_f; p.gh = a->grid_h; p.gw = a->grid_w;
   p.remap = reinterpret_cast<const long long*>(a->freq_remap);
   p.out = static_cast<uint16_t*>(a->out);
-  p.hilo = a->freqs ? a->freqs_hilo : nullptr;
-  // Default: the one-warp-per-token kernel (64 independent warps per SM).  JENGA_WAN_PROLOGUE=vector / vector64 select the experimental 128-threads-per-token kernel
-  // (row in registers, 16-byte accesses, four complex factors per token and thread; rotation on the FP32 pipe
-  // with the (hi, lo) table, or in fp64): same results (tests), but with 120 registers it runs 16
-  // warps per SM behind one block barrier per token pair and cannot overlap its load and compute phases.
-  const int esz = p.x_f32 ? 4 : 2, wsz = p.w_f32 ? 4 : 2;
-  const char* wmode = std::getenv("JENGA_WAN_PROLOGUE");
-  const bool want64 = wmode && wmode[0] == 'v' && wmode[1] == 'e' && std::strlen(wmode) >= 8;   // "vector64"
-  if (want64) p.hilo = nullptr;
-  const bool vec_ok = (wmode && wmode[0] == 'v') && (p.hilo || !p.freqs || want64) && p.C % 8 == 0 && p.C / 8 <= 6 * kWanThreads &&
-                      reinterpret_cast<uintptr_t>(p.x) % 16 == 0 && (p.sb * esz) % 16 == 0 && (p.ss * esz) % 16 == 0 &&
-                      (!p.w || reinterpret_cast<uintptr_t>(p.w) % 16 == 0) && reinterpret_cast<uintptr_t>(p.out) % 16 == 0 &&
-                      (!p.freqs || reinterpret_cast<uintptr_t>(p.freqs) % 16 == 0) &&
-                      (!p.hilo || reinterpret_cast<uintptr_t>(p.hilo) % 16 == 0);
-  (void)wsz;
-  if (vec_ok) {
-    long long pairs = (a->tokens + 1) / 2;
-    if (pairs > static_cast<long long>(kNumSMs) * 24) pairs = static_cast<long long>(kNumSMs) * 24;
-    dim3 grid(static_cast<unsigned>(pairs), static_cast<unsigned>(a->batch));
-    const int per_thread = (p.C / 8 + kWanThreads - 1) / kWanThreads;
-    switch (per_thread) {
-      case 1: wan_prologue_vec_kernel<1><<<grid, 2 * kWanThreads, 0, stream>>>(p); break;
-      case 2: wan_prologue_vec_kernel<2><<<grid, 2 * kWanThreads, 0, stream>>>(p); break;
-      case 3: wan_prologue_vec_kernel<3><<<grid, 2 * kWanThreads, 0, stream>>>(p); break;
-      case 4: wan_prologue_vec_kernel<4><<<grid, 2 * kWanThreads, 0, stream>>>(p); break;
-      case 5: wan_prologue_vec_kernel<5><<<grid, 2 * kWanThreads, 0, stream>>>(p); break;
-      default: wan_prologue_vec_kernel<6><<<grid, 2 * kWanThreads, 0, stream>>>(p); break;
-    }
-    const cudaError_t cev = cudaGetLastError();
-    return cev == cudaSuccess ? JENGA_OK : set_cuda_error(cev, "wan_prologue (vector) launch");
-  }
   dim3 grid(static_cast<unsigned>((a->tokens + 7) / 8), static_cast<unsigned>(a->batch));
   wan_prologue_kernel<<<grid, 256, 0, stream>>>(p);
   cudaError_t ce = cudaGetLastError();

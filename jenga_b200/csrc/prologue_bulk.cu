@@ -38,14 +38,8 @@ namespace jenga {
 namespace {
 
 constexpr int kBlock = 128;
-#ifndef JENGA_PB_STAGES
-#define JENGA_PB_STAGES 10
-#endif
-#ifndef JENGA_PB_STORE_LAG
-#define JENGA_PB_STORE_LAG 3
-#endif
-constexpr int kStages = JENGA_PB_STAGES;
-constexpr int kStoreLag = JENGA_PB_STORE_LAG;   // bulk-store groups whose shared-memory reads may still be pending
+constexpr int kStages = 10;
+constexpr int kStoreLag = 3;   // bulk-store groups whose shared-memory reads may still be pending
 constexpr int kGroupThreads = 384;                 // 24 heads x 16 lanes
 constexpr int kComputeThreads = 2 * kGroupThreads; // even / odd tokens
 constexpr int kThreads = kComputeThreads + 64;     // + producer warp + store warp (one thread each)

@@ -724,10 +724,6 @@ int block_pool_impl(const void* x, void* pooled, void* cast_out, int in_dtype, i
       threads = t;
       break;
     }
-  if (const char* e = std::getenv("JENGA_POOL_THREADS")) {   // tuning experiment
-    const int t = std::atoi(e);
-    if (t >= 32 && t <= 256 && t % 32 == 0) threads = t;
-  }
   uint16_t* po = static_cast<uint16_t*>(pooled);
   uint16_t* co = static_cast<uint16_t*>(cast_out);
   if (in_dtype == JENGA_F32)

@@ -31,7 +31,7 @@ _FREQ_CACHE: dict = {}
 
 
 def _device_freqs(freqs: torch.Tensor, dev) -> torch.Tensor:
-    """The complex128 table as doubles [rows, 64, 2] on `dev`, and its fp32 (hi, lo) split [rows, 64, 4].  WanModel keeps `self.freqs` on the CPU
+    """The complex128 table as doubles [rows, 64, 2] on `dev`.  WanModel keeps `self.freqs` on the CPU
     (model_mul.py:502-507) and the reference moves it every forward; here the device copy is made once
     per table (keyed by the tensor object, dropped with it)."""
     import weakref
@@ -40,11 +40,8 @@ def _device_freqs(freqs: torch.Tensor, dev) -> torch.Tensor:
     if hit is not None and hit[0]() is freqs and hit[2] == freqs._version:
         return hit[1]
     fr = torch.view_as_real(freqs.to(torch.complex128)).to(dev).contiguous()
-    hi = fr.to(torch.float32)
-    lo = (fr - hi.to(torch.float64)).to(torch.float32)
-    hilo = torch.cat([hi, lo], dim=-1).contiguous()          # [rows, 64, 4] = re_hi, im_hi, re_lo, im_lo
-    _FREQ_CACHE[key] = (weakref.ref(freqs, lambda _r, k=key: _FREQ_CACHE.pop(k, None)), (fr, hilo), freqs._version)
-    return fr, hilo
+    _FREQ_CACHE[key] = (weakref.ref(freqs, lambda _r, k=key: _FREQ_CACHE.pop(k, None)), fr, freqs._version)
+    return fr
 
 
 def norm_rope(x: torch.Tensor, weight: torch.Tensor | None, heads: int, grid_size, freqs: torch.Tensor,
@@ -72,9 +69,8 @@ def norm_rope(x: torch.Tensor, weight: torch.Tensor | None, heads: int, grid_siz
         a.w, a.w_dtype = None, _lib.JENGA_F32
     a.batch, a.heads, a.head_dim, a.tokens = B, heads, 128, L
     a.stride_b, a.stride_s, a.eps = x.stride(0), x.stride(1), eps
-    fr, hilo = _device_freqs(freqs, dev)
+    fr = _device_freqs(freqs, dev)
     a.freqs, a.freq_rows = fr.data_ptr(), fr.shape[0]
-    a.freqs_hilo = hilo.data_ptr()
     a.grid_f, a.grid_h, a.grid_w = (int(v) for v in grid_size)
     if freq_remap is not None:
         freq_remap = freq_remap.to(device=dev, dtype=torch.int64).contiguous()

@@ -87,3 +87,45 @@ def test_wan_prologue_matches_reference_golden():
         assert d.max() <= 1.0, (tag, d.max().item())
         assert (got.view(torch.int16) == ref.view(torch.int16)).float().mean() >= 0.995
     assert wan.block_counts(32760, 0.5) == (128, 12) and wan.block_counts(75600, 0.7) == (177, 28)
+
+
+def _wan_norm_rope_torch(x, w, heads, grid, freqs, remap, eps):
+    """WanRMSNorm + rope_apply (the chain make_golden.py runs from the reference) restated in torch, then
+    the operator's bf16 cast."""
+    B, L, _ = x.shape
+    xf = x.float()
+    y = (xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps)).type_as(x) * w
+    y = y.view(B, L, heads, 128)
+    f, h, wd = grid
+    n = f * h * wd
+    parts = freqs.to(x.device).split([22, 21, 21], dim=1)
+    fr = torch.cat([parts[0][:f].view(f, 1, 1, -1).expand(f, h, wd, -1),
+                    parts[1][:h].view(1, h, 1, -1).expand(f, h, wd, -1),
+                    parts[2][:wd].view(1, 1, wd, -1).expand(f, h, wd, -1)], dim=-1).reshape(n, 1, -1)[remap]
+    rot = torch.view_as_real(torch.view_as_complex(y[:, :n].double().reshape(B, n, heads, 64, 2)) * fr).flatten(3)
+    return torch.cat([rot, y[:, n:].double()], dim=1).float().bfloat16()
+
+
+@pytest.mark.parametrize("dt,heads,grid", [(torch.float32, 12, (3, 6, 8)), (torch.bfloat16, 12, (3, 6, 8)),
+                                           (torch.float32, 40, (2, 5, 7)), (torch.bfloat16, 5, (4, 4, 4))])
+def test_wan_prologue_matches_torch_restatement(dt, heads, grid):
+    """fp32 and bf16 input (bf16 weights with bf16 input), batch 2, odd and large head counts, a remapped
+    grid and 37 tokens past it that get no rotation.  >= 99.5 % bit-identical, as in the golden test.  The
+    residue again comes from the fp32 summation order of mean(x^2): a rounding of the normalised pair that
+    falls the other way moves it by about one bf16 ulp of its magnitude, and the rotation can carry that
+    into a component much smaller than the pair.  So the error of every element is bounded relative to
+    the magnitude of its complex pair, not to the element itself."""
+    from jenga_b200 import wan
+    dev = "cuda"
+    L = grid[0] * grid[1] * grid[2] + 37
+    g = torch.Generator().manual_seed(99 + heads)
+    x = (torch.randn((2, L, heads * 128), generator=g) * 1.3).to(dt).to(dev)
+    w = (1 + 0.2 * torch.randn(heads * 128, generator=g)).to(dt).to(dev)
+    remap = torch.randperm(grid[0] * grid[1] * grid[2], generator=g).to(dev)
+    freqs = wan.rope_freqs(128)
+    got = wan.norm_rope(x, w, heads, grid, freqs, remap, eps=1e-6)
+    ref = _wan_norm_rope_torch(x, w, heads, grid, freqs, remap, 1e-6)
+    assert (got.view(torch.int16) == ref.view(torch.int16)).float().mean() >= 0.995
+    pair = ref.float().view(*ref.shape[:-1], 64, 2).norm(dim=-1, keepdim=True)
+    err = (got.float() - ref.float()).view(*ref.shape[:-1], 64, 2).abs()
+    assert (err <= 2.0 ** -5 * pair).all(), (err / pair).max().item()
