@@ -390,6 +390,32 @@ int jenga_quantize_v_fp8(const void* v, int32_t dtype, int32_t batch, int64_t ro
                          int64_t stride_b, int64_t stride_s, int64_t stride_h, void* out_fp8, float* amax,
                          void* stream);
 
+/* (f-3) INT8 operands for the opt-in INT8 Q.K^T variant.  x: [B, rows, H, 128] bf16/f16, element strides.
+ * smooth != 0: mean[b*H+h][0..128) = fp32 mean of x over its `rows` rows (written; caller-allocated
+ *              f32 [B*H*128]), subtracted before quantising.  smooth == 0: nothing subtracted.
+ * Per (b, h) and per group of `group_rows` rows (64 or 128):
+ *   scale = max|x - mean| / 127 ;  out = clamp(rint((x - mean) / scale), -127, 127)   (0 where scale == 0)
+ * out: contiguous int8 [B, out_rows, H, 128], out_rows a multiple of 128 and >= round_up(rows, 128).
+ * Rows in [rows, out_rows) hold the quantised value of (0 - mean): they stand for the zero padding
+ * that dense rows attend.  scale: f32 [B*H, out_rows / group_rows].  With smooth != 0, `out` also
+ * serves as scratch for the per-block partial sums of the mean (deterministic, no atomics). */
+int jenga_quantize_int8(const void* x, int32_t dtype, int32_t batch, int64_t rows, int32_t heads,
+                        int64_t stride_b, int64_t stride_s, int64_t stride_h, int32_t group_rows,
+                        int32_t smooth, float* mean, int8_t* out, int64_t out_rows, float* scale, void* stream);
+
+/* (f-3) opt-in INT8 Q.K^T variant of jenga_carved_attn_fwd (SageAttention's recipe): Q.K^T runs as
+ * s8 x s8 -> s32 on the tensor cores from per-block-scaled int8 Q (64-row groups) and K (128-key
+ * blocks, K smoothed by its per-head mean, which leaves every softmax unchanged).  `args` means what
+ * it means for jenga_carved_attn_fwd (the FP8 P.V variant included) except that Q.K^T reads these
+ * operands.  Not built: lse_out (smoothing shifts the LSE by q.mean), the Ulysses epilogue
+ * (sp_world > 0), FP8 P.V with f16.  Lower precision than the default path; never implicit. */
+typedef struct JengaQkInt8Args {
+  const int8_t* q_i8;   const float* q_scale;   /* from jenga_quantize_int8(q, group_rows 64, smooth 0)  */
+  const int8_t* k_i8;   const float* k_scale;   /* from jenga_quantize_int8(k, group_rows 128, smooth 1) */
+  int64_t q_rows_padded, kv_rows_padded;        /* the out_rows used for each                           */
+} JengaQkInt8Args;
+int jenga_carved_attn_fwd_qk_int8(const JengaAttnArgs* args, const JengaQkInt8Args* qk, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

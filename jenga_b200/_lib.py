@@ -41,6 +41,13 @@ class JengaAttnArgs(C.Structure):
     ]
 
 
+class JengaQkInt8Args(C.Structure):
+    _fields_ = [
+        ("q_i8", C.c_void_p), ("q_scale", C.c_void_p), ("k_i8", C.c_void_p), ("k_scale", C.c_void_p),
+        ("q_rows_padded", C.c_int64), ("kv_rows_padded", C.c_int64),
+    ]
+
+
 class JengaUlyssesScatterArgs(C.Structure):
     _fields_ = [
         ("x", C.c_void_p * 3), ("joint", C.c_void_p * 3),
@@ -170,6 +177,12 @@ def _load() -> C.CDLL:
     lib.jenga_quantize_v_fp8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int64, C.c_int64,
                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.jenga_quantize_v_fp8.restype = C.c_int
+    lib.jenga_quantize_int8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int64, C.c_int64,
+                                        C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_void_p]
+    lib.jenga_quantize_int8.restype = C.c_int
+    lib.jenga_carved_attn_fwd_qk_int8.argtypes = [C.POINTER(JengaAttnArgs), C.POINTER(JengaQkInt8Args), C.c_void_p]
+    lib.jenga_carved_attn_fwd_qk_int8.restype = C.c_int
     lib.jenga_gilbert_xyz2d.argtypes = [C.c_int] * 6
     lib.jenga_gilbert_xyz2d.restype = C.c_int64
     if lib.jenga_abi_version() != 3:

@@ -154,11 +154,41 @@ def quantize_v_fp8(v: torch.Tensor):
     return v8, amax
 
 
+def quantize_int8(x: torch.Tensor, group_rows: int, smooth: bool):
+    """Per-group int8 quantisation of x [B,S,H,128] (C-ABI jenga_quantize_int8).  Returns (x8 int8
+    [B, round_up(S,128), H, 128] contiguous, scale f32 [B*H, round_up(S,128) / group_rows], mean f32
+    [B*H, 128] or None).  Rows past S hold the quantised (0 - mean)."""
+    _require_cuda(x)
+    B, S, H, D = x.shape
+    if D != 128 or x.stride(3) != 1:
+        raise ValueError("x must be [B,S,H,128] with contiguous channels")
+    rows_p = (S + BLOCK - 1) // BLOCK * BLOCK
+    x8 = torch.empty((B, rows_p, H, D), dtype=torch.int8, device=x.device)
+    scale = torch.empty((B * H, rows_p // group_rows), dtype=torch.float32, device=x.device)
+    mean = torch.empty((B * H, D), dtype=torch.float32, device=x.device) if smooth else None
+    with torch.cuda.device(x.device):
+        check(lib.jenga_quantize_int8(x.data_ptr(), _dtype_code(x), B, S, H, x.stride(0), x.stride(1), x.stride(2),
+                                      group_rows, int(smooth), mean.data_ptr() if smooth else None, x8.data_ptr(),
+                                      rows_p, scale.data_ptr(), _stream_ptr(x.device)), "quantize_int8")
+    return x8, scale, mean
+
+
+def quantize_qk_int8(q: torch.Tensor, k: torch.Tensor):
+    """Operands of the opt-in INT8 Q.K^T variant: Q per 64-row group, K per 128-key block after
+    subtracting its per-head channel mean.  Returns (q8, q_scale, k8, k_scale)."""
+    q8, q_scale, _ = quantize_int8(q, 64, False)
+    k8, k_scale, _ = quantize_int8(k, 128, True)
+    return q8, q_scale, k8, k_scale
+
+
 # Opt-in (never the default): route every operator call of this process through the FP8 P.V variant
 # — `jenga_b200.attention.PV_FP8 = True` or JENGA_PV_FP8=1 in the environment.  Lower precision in the
 # second product only (tests/test_fp8_gpu.py has its tolerance row); selection and Q.K^T are unchanged.
 import os as _os
 PV_FP8: bool = _os.environ.get("JENGA_PV_FP8", "0") == "1"
+# Opt-in, the same way: INT8 Q.K^T with K smoothing (`QK_INT8 = True` or JENGA_QK_INT8=1); composes with
+# PV_FP8.  Its own tolerance row (tests/test_qk_int8_gpu.py); the mask selection is unchanged.
+QK_INT8: bool = _os.environ.get("JENGA_QK_INT8", "0") == "1"
 
 _NBR_CACHE: dict = {}
 # tests set this to a list to record every selection result (bit rows, nb) of calls made deep
@@ -247,7 +277,7 @@ def block_sparse_attention_variant(
     max_seqlen_q=None, max_seqlen_kv=None, text_blocks=None, text_amp: float = 0.0,
     block_neighbor_list=None, shape_xfuse: bool = False, p_remain_rates=None,
     first_frame_blocks: int = 0, return_mask_bits: bool = False, out: torch.Tensor | None = None,
-    sp_out: dict | None = None, pv_fp8: bool = False,
+    sp_out: dict | None = None, pv_fp8: bool = False, qk_int8: bool = False,
 ):
     """AttenCarve operator, [B,S,H,D] in -> [B,S,H*D] (or [B,S,H,D] when shape_xfuse).
     Same arguments, defaults and quirks as the reference function of the same name; see the
@@ -322,8 +352,10 @@ def block_sparse_attention_variant(
     # pv_fp8 (opt-in, SURVEY §8 f-3): V is quantised per head to e4m3 and P.V runs on the FP8 tensor
     # path; NOT the reference's arithmetic — its own tolerance row, never enabled implicitly
     v8 = quantize_v_fp8(v) if (pv_fp8 or PV_FP8) and sp_out is None and q.dtype == torch.bfloat16 else None
+    # qk_int8 (opt-in): int8 Q and smoothed int8 K in Q.K^T (for Wan, of the bf16 copies)
+    qk8 = quantize_qk_int8(q, k) if (qk_int8 or QK_INT8) else None
     o = _launch(q, k, v, mask_bits, normal_blocks, text_blocks, D ** -0.5, text_amp, normal_blocks,
-                limit, limit, nb * BLOCK, out, seqlen_dev, a_out_dtype, v_fp8=v8)
+                limit, limit, nb * BLOCK, out, seqlen_dev, a_out_dtype, v_fp8=v8, qk_int8=qk8)
     if not shape_xfuse:
         o = o.reshape(B, S, H * D)
     return (o, mask_bits) if return_mask_bits else o
@@ -331,7 +363,8 @@ def block_sparse_attention_variant(
 
 def _launch(q, k, v, mask_bits, nq_sparse, nq_dense, sm_scale, text_amp, text_block_start,
             kv_limit_sparse, q_limit_sparse, kv_limit_dense, out, seqlen_dev, out_dtype, sp_out=None, lse_out=None,
-            v_fp8=None):
+            v_fp8=None, qk_int8=None):
+    """qk_int8: None, or (q8, q_scale, k8, k_scale) from quantize_qk_int8 — the INT8 Q.K^T variant."""
     B, Sq, H, D = q.shape
     a = JengaAttnArgs()
     a.q, a.k, a.v = q.data_ptr(), k.data_ptr(), v.data_ptr()
@@ -362,7 +395,15 @@ def _launch(q, k, v, mask_bits, nq_sparse, nq_dense, sm_scale, text_amp, text_bl
     a.seqlen_dev = seqlen_dev.data_ptr() if seqlen_dev is not None else None
     a.err_flag = None
     with torch.cuda.device(q.device):
-        check(lib.jenga_carved_attn_fwd(C.byref(a), _stream_ptr(q.device)), "carved_attn_fwd")
+        if qk_int8 is None:
+            check(lib.jenga_carved_attn_fwd(C.byref(a), _stream_ptr(q.device)), "carved_attn_fwd")
+        else:
+            q8, q_scale, k8, k_scale = qk_int8
+            x = _lib.JengaQkInt8Args()
+            x.q_i8, x.q_scale, x.k_i8, x.k_scale = q8.data_ptr(), q_scale.data_ptr(), k8.data_ptr(), k_scale.data_ptr()
+            x.q_rows_padded, x.kv_rows_padded = q8.shape[1], k8.shape[1]
+            check(lib.jenga_carved_attn_fwd_qk_int8(C.byref(a), C.byref(x), _stream_ptr(q.device)),
+                  "carved_attn_fwd_qk_int8")
     return out
 
 

@@ -156,6 +156,11 @@ extern "C" int jenga_carved_attn_fwd(const JengaAttnArgs* args, void* stream) {
   return carved_attn_fwd_impl(args, static_cast<cudaStream_t>(stream));
 }
 
+extern "C" int jenga_carved_attn_fwd_qk_int8(const JengaAttnArgs* args, const JengaQkInt8Args* qk, void* stream) {
+  if (!qk) return set_error(JENGA_E_INVALID, "qk_int8: null pointer");
+  return carved_attn_fwd_impl(args, static_cast<cudaStream_t>(stream), qk);
+}
+
 extern "C" int jenga_gather_rows(const void* src, void* dst, const int64_t* index, int64_t n_index,
                                  int64_t n_src_rows, int64_t row_bytes, int batch,
                                  int64_t src_batch_stride, int64_t dst_batch_stride, void* stream) {

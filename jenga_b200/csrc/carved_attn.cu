@@ -29,6 +29,8 @@
 // HBM/L2 layout: q,k,v stay in the caller's [B,S,H,D] layout; TMA boxes are {64 d, 128 rows}
 // with 128-byte swizzle.  K boxes are K-major wgmma operands, V boxes MN-major (no transpose).
 // CTAs are numbered head-major so that all CTAs in flight read the same head's K/V out of L2.
+#include <cfloat>
+
 #include "carved_attn_common.cuh"
 
 namespace jenga {
@@ -80,7 +82,15 @@ __device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t col) {
 // match the order in which the S accumulator fragment already holds P: no shuffles of P.  The
 // consumers wait for V^T on VT_FULL instead of V_FULL and otherwise run the same schedule.
 // Q.K^T, the softmax and l are unchanged.
-template <bool kBF16, bool kPvFp8 = false>
+//
+// kQkInt8 (opt-in, SageAttention's recipe): Q and K enter Q.K^T as int8 made by jenga_quantize_int8 —
+// Q per 64-row group (one scale per consumer warpgroup), K per 128-key block after subtracting its
+// per-head channel mean (a constant per score row: every softmax is unchanged) — through wgmma
+// m64n128k32 s8 x s8 -> s32 (half the Q.K^T tensor cycles).  Q and K tiles are one 16 KB box each.
+// The s32 scores become fp32 exactly (|S| < 2^22) and both classes scale them inside the exponent by
+// c = q_scale * k_scale[blk] * qk_scale, so the sparse class skips its Q~ pre-scaling.  text_amp,
+// the masks, the lazy rescale and P.V (bf16/f16, or e4m3 with kPvFp8) are unchanged.
+template <bool kBF16, bool kPvFp8 = false, bool kQkInt8 = false>
 __global__ void __launch_bounds__(kThreads, 1)
 carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
                        const __grid_constant__ CUtensorMap tm_k,
@@ -150,9 +160,14 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     setmaxnreg_dec<kPvFp8 ? 40 : 24>();
     if (warp == kConsumerThreads / 32) {
       if (n_tiles > 0 && lane == 0) {   // TMA
-        mbar_arrive_expect_tx(&bars[Q_FULL], kTileBytes);
-        tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
-        tma_load_4d(sQ + kBoxBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b);
+        if constexpr (kQkInt8) {   // 128 rows x 128 one-byte channels = one 16 KB box
+          mbar_arrive_expect_tx(&bars[Q_FULL], kBoxBytes);
+          tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
+        } else {
+          mbar_arrive_expect_tx(&bars[Q_FULL], kTileBytes);
+          tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
+          tma_load_4d(sQ + kBoxBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b);
+        }
         BlockWalker it(s_mask, nwords);
         int j = 0;
         for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
@@ -162,9 +177,14 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
           uint8_t* k_dst = sK + s * kTileBytes;
           uint8_t* v_dst = sV + s * kTileBytes;
           mbar_wait(&bars[K_EMPTY + s], par, p.err_flag);
-          mbar_arrive_expect_tx(&bars[K_FULL + s], kTileBytes);
-          tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
-          tma_load_4d(k_dst + kBoxBytes, &tm_k, &bars[K_FULL + s], 64, row0, h, b);
+          if constexpr (kQkInt8) {
+            mbar_arrive_expect_tx(&bars[K_FULL + s], kBoxBytes);
+            tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
+          } else {
+            mbar_arrive_expect_tx(&bars[K_FULL + s], kTileBytes);
+            tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
+            tma_load_4d(k_dst + kBoxBytes, &tm_k, &bars[K_FULL + s], 64, row0, h, b);
+          }
           mbar_wait(&bars[V_EMPTY + s], par, p.err_flag);
           if constexpr (kPvFp8) {   // 128 keys x 128 one-byte channels = one 16 KB box
             mbar_arrive_expect_tx(&bars[V_FULL + s], kBoxBytes);
@@ -224,11 +244,13 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
   for (int i = 0; i < 64; ++i) o[i] = 0.f;
   // sparse class: Q~ = round(Q * qk_scale) and raw S is already in log2 units (c = 1)
   // dense class : raw S, scaled inside the exponent (c = qk_scale), like FlashAttention
+  // kQkInt8     : integer S, scaled inside the exponent by c = q_scale * k_scale[blk] * qk_scale
   const float c = dense ? p.qk_scale : 1.0f;
+  const float qs = kQkInt8 && n_tiles > 0 ? __ldg(p.q_scale + bh * p.q_groups + 2 * qb + wg) * p.qk_scale : 0.f;
 
   if (n_tiles > 0) {
     mbar_wait(&bars[Q_FULL], 0, p.err_flag);
-    if (!dense) {
+    if (!dense && !kQkInt8) {
       // ref :87-88  q = (q * qk_scale).to(dtype) — elementwise, so swizzle-agnostic
       uint4* q4 = reinterpret_cast<uint4*>(sQ);
 #pragma unroll 4
@@ -248,6 +270,7 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128;   // this warpgroup's 64 rows of each d half
 
     float sc[64];                      // S_j, then P_j in fp32
+    int32_t si[kQkInt8 ? 64 : 1];      // kQkInt8: integer S_j while its wgmma runs
     uint32_t pa[kPvFp8 ? 4 : 8][4];    // P_{j-1}: A operand of the P.V wgmma; untouched while it runs
     float alpha[2];
 
@@ -266,13 +289,37 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     // ---- S = Q~ K^T (64 x 128 per warpgroup, K = 128 in 8 steps) ----
     auto issue_qk = [&](int s) {
       const uint32_t k_addr = smem_u32(sK + s * kTileBytes);
+      if constexpr (kQkInt8) {   // K = 128 in 4 steps of 32 one-byte channels inside the swizzled row
 #pragma unroll
-      for (int kk = 0; kk < kHeadDim / 16; ++kk) {
-        const uint32_t off = (kk & 3) * 32 + (kk >> 2) * kBoxBytes;
-        wgmma_128_ss<kBF16>(sc, gmma_desc_sw128(q_addr + off, 16, 1024),
-                            gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
+        for (int kc = 0; kc < kHeadDim / 32; ++kc)
+          wgmma_128_ss_s8(si, gmma_desc_sw128(q_addr + kc * 32, 16, 1024),
+                          gmma_desc_sw128(k_addr + kc * 32, 16, 1024), kc > 0 ? 1u : 0u);
+      } else {
+#pragma unroll
+        for (int kk = 0; kk < kHeadDim / 16; ++kk) {
+          const uint32_t off = (kk & 3) * 32 + (kk >> 2) * kBoxBytes;
+          wgmma_128_ss<kBF16>(sc, gmma_desc_sw128(q_addr + off, 16, 1024),
+                              gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
+        }
       }
       wgmma_commit();
+    };
+    // S_j has retired: make it visible (and, for kQkInt8, exact fp32: |S| <= 128 * 127^2 < 2^22, so
+    // the s32 value lands in the mantissa of 1.5 * 2^23 — two ALU ops, no 16/clk I2F)
+    auto scores_ready = [&] {
+      if constexpr (kQkInt8) {
+        fence_regs(si);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sc[i] = __int_as_float(si[i] + 0x4B400000) - 12582912.f;
+      } else {
+        fence_regs(sc);
+      }
+    };
+    // exponent factor of key block blk (kQkInt8: read before the tile's waits, so the softmax
+    // never stalls on it; never 0, which would turn the -inf of masked columns into NaN)
+    auto tile_c = [&](int blk) -> float {
+      if constexpr (kQkInt8) return fmaxf(qs * __ldg(p.k_scale + bh * p.k_groups + blk), FLT_MIN);
+      else return c;
     };
     // ---- O += P V ----
     auto issue_pv = [&](int s) {
@@ -290,7 +337,7 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
       wgmma_commit();
     };
     // ---- online softmax of key block blk on sc; true when O must be rescaled by alpha ----
-    auto softmax = [&](int blk) -> bool {
+    auto softmax = [&](int blk, float ct) -> bool {
       // ref :113-114 — text_amp is a constant added to every score of a text key block, in
       // log2 units (sparse class only, where c == 1): fold it into the exponent offset.
       const float amp = (!dense && blk >= p.text_block_start) ? p.text_amp : 0.f;
@@ -312,7 +359,7 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
       for (int r = 0; r < 2; ++r) {
         mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
         mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        m_cand[r] = fmaxf(m_used[r], fmaf(mx[r], c, amp));
+        m_cand[r] = fmaxf(m_used[r], fmaf(mx[r], ct, amp));
         // Lazy rescale: the reference rescales acc by exp2(m_old - m_new) every tile
         // (:121-132).  O/l is invariant to the reference point, so it only moves when the
         // max grew by more than 2^8 — the final O/l is the same up to fp32 rounding.
@@ -335,7 +382,7 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
         const int r = (i >> 1) & 1;
-        sc[i] = fast_exp2(fmaf(sc[i], c, off[r]));
+        sc[i] = fast_exp2(fmaf(sc[i], ct, off[r]));
         l_sum[r] += sc[i];
       }
       return rescale;
@@ -372,19 +419,21 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     BlockWalker it(s_mask, nwords);
     // prologue: S_0 and its softmax
     int blk = it.next();
+    float ct = tile_c(blk);
     mbar_wait(&bars[K_FULL], 0, p.err_flag);
     turn_begin();
     wgmma_fence();
     issue_qk(0);
     turn_end(false);
     wgmma_wait<0>();
-    fence_regs(sc);
+    scores_ready();
     release(K_EMPTY);
-    if (softmax(blk)) rescale_o();
+    if (softmax(blk, ct)) rescale_o();
     pack_p();
     int j = 1;
     for (blk = it.next(); blk >= 0; blk = it.next(), ++j) {   // S_j and P_{j-1} V_{j-1}
       const int s = j % kStages, sv = (j - 1) % kStages;
+      ct = tile_c(blk);
       mbar_wait(&bars[kVReady + sv], ((j - 1) / kStages) & 1, p.err_flag);
       mbar_wait(&bars[K_FULL + s], (j / kStages) & 1, p.err_flag);
       turn_begin();
@@ -394,9 +443,9 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
       issue_pv(sv);
       turn_end(false);
       wgmma_wait<1>();
-      fence_regs(sc);
+      scores_ready();
       release(K_EMPTY + s);
-      const bool rescale = softmax(blk);
+      const bool rescale = softmax(blk, ct);
       wgmma_wait<0>();
       fence_regs(o);
       release(V_EMPTY + sv);
@@ -493,8 +542,8 @@ static int make_tile_map(CUtensorMap* map, const void* base, int dtype, long lon
                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-// V as FP8: contiguous [B, S, H, 128] bytes; box {128 channels, 128 keys}
-static int make_v8_map(CUtensorMap* map, const void* base, long long rows, int heads, int batch) {
+// one-byte operands (FP8 V, int8 Q / K): contiguous [B, S, H, 128] bytes; box {128 channels, 128 rows}
+static int make_bytes_map(CUtensorMap* map, const void* base, long long rows, int heads, int batch) {
   const cuuint64_t dims[4] = {static_cast<cuuint64_t>(kHeadDim), static_cast<cuuint64_t>(rows),
                               static_cast<cuuint64_t>(heads), static_cast<cuuint64_t>(batch)};
   const cuuint64_t strides[3] = {static_cast<cuuint64_t>(heads) * kHeadDim, static_cast<cuuint64_t>(kHeadDim),
@@ -508,7 +557,7 @@ static int make_v8_map(CUtensorMap* map, const void* base, long long rows, int h
 
 static bool stride_ok(long long s) { return s > 0 && (s * 2) % 16 == 0; }
 
-int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream) {
+int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const JengaQkInt8Args* qk) {
   if (!a || !a->q || !a->k || !a->v || (!a->out && a->sp_world <= 0)) return set_error(JENGA_E_INVALID, "null pointer");
   if (a->dtype != JENGA_BF16 && a->dtype != JENGA_F16)
     return set_error(JENGA_E_INVALID, "dtype must be bf16 or f16");
@@ -540,6 +589,23 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream) {
   for (uintptr_t q : ptrs)
     if (q % 16) return set_error(JENGA_E_INVALID, "pointers must be 16-byte aligned");
   if (!(a->sm_scale > 0.f)) return set_error(JENGA_E_INVALID, "sm_scale must be positive");
+  if (qk) {
+    if (!qk->q_i8 || !qk->q_scale || !qk->k_i8 || !qk->k_scale)
+      return set_error(JENGA_E_INVALID, "qk_int8: null int8 operand or scale pointer");
+    if (a->lse_out)
+      return set_error(JENGA_E_UNSUPPORTED, "qk_int8: lse_out is not built (K smoothing shifts the LSE by q.mean)");
+    if (a->sp_world > 0) return set_error(JENGA_E_UNSUPPORTED, "qk_int8: the Ulysses epilogue is not built");
+    const long long q_need = (a->q_rows + kBlock - 1) / kBlock * kBlock;
+    const long long kv_need = (a->kv_rows + kBlock - 1) / kBlock * kBlock;
+    if (qk->q_rows_padded < q_need || qk->kv_rows_padded < kv_need || qk->q_rows_padded % kBlock ||
+        qk->kv_rows_padded % kBlock)
+      return set_error(JENGA_E_INVALID, "qk_int8: padded rows (%lld, %lld) must be multiples of 128 >= (%lld, %lld)",
+                       static_cast<long long>(qk->q_rows_padded), static_cast<long long>(qk->kv_rows_padded),
+                       q_need, kv_need);
+    if (reinterpret_cast<uintptr_t>(qk->q_i8) % 16 || reinterpret_cast<uintptr_t>(qk->k_i8) % 16 ||
+        reinterpret_cast<uintptr_t>(qk->q_scale) % 4 || reinterpret_cast<uintptr_t>(qk->k_scale) % 4)
+      return set_error(JENGA_E_INVALID, "qk_int8: int8 operands must be 16-byte and scales 4-byte aligned");
+  }
   if (a->sp_world != 0 &&
       (a->sp_world < 0 || a->sp_world > 8 || a->sp_rank < 0 || a->sp_rank >= a->sp_world || !a->out_peers_host ||
        a->sp_rows <= 0 || a->batch != 1 || a->out_dtype != a->dtype))
@@ -558,14 +624,19 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream) {
   }
   CUtensorMap tm_q, tm_k, tm_v;
   int rc;
-  if ((rc = make_tile_map(&tm_q, a->q, a->dtype, a->q_rows, a->heads, a->batch, a->q_stride_b,
-                          a->q_stride_s, a->q_stride_h, kBlock)))
-    return rc;
-  if ((rc = make_tile_map(&tm_k, a->k, a->dtype, a->kv_rows, a->heads, a->batch, a->k_stride_b,
-                          a->k_stride_s, a->k_stride_h, kBlock)))
-    return rc;
+  if (qk) {
+    if ((rc = make_bytes_map(&tm_q, qk->q_i8, qk->q_rows_padded, a->heads, a->batch))) return rc;
+    if ((rc = make_bytes_map(&tm_k, qk->k_i8, qk->kv_rows_padded, a->heads, a->batch))) return rc;
+  } else {
+    if ((rc = make_tile_map(&tm_q, a->q, a->dtype, a->q_rows, a->heads, a->batch, a->q_stride_b,
+                            a->q_stride_s, a->q_stride_h, kBlock)))
+      return rc;
+    if ((rc = make_tile_map(&tm_k, a->k, a->dtype, a->kv_rows, a->heads, a->batch, a->k_stride_b,
+                            a->k_stride_s, a->k_stride_h, kBlock)))
+      return rc;
+  }
   if (pv_fp8) {
-    if ((rc = make_v8_map(&tm_v, a->v_fp8, a->kv_rows, a->heads, a->batch))) return rc;
+    if ((rc = make_bytes_map(&tm_v, a->v_fp8, a->kv_rows, a->heads, a->batch))) return rc;
   } else if ((rc = make_tile_map(&tm_v, a->v, a->dtype, a->kv_rows, a->heads, a->batch, a->v_stride_b,
                                  a->v_stride_s, a->v_stride_h, kBlock)))
     return rc;
@@ -601,11 +672,20 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream) {
   p.err_flag = a->err_flag;
   p.lse_out = a->lse_out;
   p.v_fp8_amax = a->v_fp8_amax;
+  if (qk) {
+    p.q_scale = qk->q_scale;
+    p.k_scale = qk->k_scale;
+    p.q_groups = qk->q_rows_padded / 64;
+    p.k_groups = qk->kv_rows_padded / kBlock;
+  }
 
   const long long grid = static_cast<long long>(a->batch) * a->heads * (a->nq_sparse + a->nq_dense);
   if (grid > 0x7fffffffll) return set_error(JENGA_E_UNSUPPORTED, "grid too large");
-  auto kern = pv_fp8 ? carved_attn_fwd_kernel<true, true>
-                     : (a->dtype == JENGA_BF16 ? carved_attn_fwd_kernel<true> : carved_attn_fwd_kernel<false>);
+  const bool bf16 = a->dtype == JENGA_BF16;
+  auto kern = qk ? (pv_fp8 ? carved_attn_fwd_kernel<true, true, true>
+                           : (bf16 ? carved_attn_fwd_kernel<true, false, true> : carved_attn_fwd_kernel<false, false, true>))
+                 : (pv_fp8 ? carved_attn_fwd_kernel<true, true>
+                           : (bf16 ? carved_attn_fwd_kernel<true> : carved_attn_fwd_kernel<false>));
   cudaError_t ce = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
   if (ce != cudaSuccess) return set_cuda_error(ce, "cudaFuncSetAttribute(carved_attn)");
   kern<<<static_cast<unsigned>(grid), kThreads, kSmemBytes, stream>>>(tm_q, tm_k, tm_v, p);

@@ -32,6 +32,10 @@ struct KernelParams {
   unsigned long long peer_out[8];
   float* lse_out;             // optional [B, H, q_rows] natural-log LSE of the dense rows
   const float* v_fp8_amax;    // fp8 P.V variant: per (batch, head) absmax of V (scale = amax / 448)
+  // INT8 Q.K^T variant: per-(b*H+h) rows of scales, 64-row groups of Q and 128-key blocks of K
+  const float* q_scale;
+  const float* k_scale;
+  long long q_groups, k_groups;   // scales per (batch, head): q_rows_padded / 64, kv_rows_padded / 128
   int* err_flag;
 };
 

@@ -132,7 +132,9 @@ def carved_attention_from_pools(q, k, v, pools, *, top_k: int, text_blocks: int 
         raise ValueError("out must be a [B,S,H,D] view with contiguous heads")
     from . import attention as _A
     v8 = _A.quantize_v_fp8(v) if (_A.PV_FP8 and q.dtype == torch.bfloat16) else None   # opt-in FP8 P.V variant
-    _launch(q, k, v, bits, n_img, text_blocks, D ** -0.5, text_amp, n_img, S, S, S, out, seq, q.dtype, v_fp8=v8)
+    qk8 = _A.quantize_qk_int8(q, k) if _A.QK_INT8 else None                              # opt-in INT8 Q.K^T variant
+    _launch(q, k, v, bits, n_img, text_blocks, D ** -0.5, text_amp, n_img, S, S, S, out, seq, q.dtype, v_fp8=v8,
+            qk_int8=qk8)
     if shape_xfuse:
         return out
     return out.reshape(B, S, H * D) if out.is_contiguous() else out.flatten(2)
