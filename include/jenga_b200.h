@@ -363,6 +363,19 @@ int jenga_gate_residual(const void* x, int64_t x_stride, const void* y, int64_t 
 int jenga_gelu_tanh(const void* x, int64_t x_stride, void* out, int64_t out_stride, int64_t rows,
                     int32_t channels, void* stream);
 
+/* Token-replace forms of ln_modulate / gate_residual (HunyuanVideo-I2V, i2v_condition_type ==
+ * "token_replace").  ref: hyvideo_i2v/modules/modulate_layers.py:51-56,84-95.  Row r uses
+ * tr_scale / tr_shift (tr_gate) when row_is_tr[r] != 0 and scale / shift (gate) otherwise; the
+ * per-row arithmetic is that of the plain entry points.  row_is_tr: `rows` bytes on the device
+ * (a torch.bool mask as it is).  Same validation as the plain forms, plus non-null and 16-byte
+ * aligned tr vectors and a non-null row_is_tr. */
+int jenga_ln_modulate_tr(const void* x, int64_t x_stride, const void* scale, const void* shift,
+                         const void* tr_scale, const void* tr_shift, const uint8_t* row_is_tr, void* out,
+                         int64_t out_stride, int64_t rows, int32_t channels, float eps, void* stream);
+int jenga_gate_residual_tr(const void* x, int64_t x_stride, const void* y, int64_t y_stride, const void* gate,
+                           const void* tr_gate, const uint8_t* row_is_tr, void* out, int64_t out_stride,
+                           int64_t rows, int32_t channels, void* stream);
+
 /* (f-2) ProRes stage switch in one kernel: out = trilinear_up(latents + noise_pred*d_sigma) *
  * (1 - sigma_next) + noise * sigma_next, fp32, NCDHW contiguous.
  * ref: pipeline_hunyuan_video_prores.py:721-731; scheduling_flow_match_discrete.py:258-299.

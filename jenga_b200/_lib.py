@@ -165,6 +165,12 @@ def _load() -> C.CDLL:
     lib.jenga_gate_residual.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_int64, C.c_int32, C.c_void_p]
     lib.jenga_gate_residual.restype = C.c_int
+    lib.jenga_ln_modulate_tr.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]
+    lib.jenga_ln_modulate_tr.restype = C.c_int
+    lib.jenga_gate_residual_tr.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]
+    lib.jenga_gate_residual_tr.restype = C.c_int
     lib.jenga_gelu_tanh.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]
     lib.jenga_gelu_tanh.restype = C.c_int
     lib.jenga_prores_switch.argtypes = [C.c_void_p] * 4 + [C.c_int32] * 7 + [C.c_float, C.c_float, C.c_void_p]

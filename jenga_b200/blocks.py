@@ -7,6 +7,8 @@ reference module is executed,
 
   MMDoubleStreamBlock.forward / MMSingleStreamBlock.forward
       (hyvideo/modules/models_mul_block_gc_ha_multigpu.py:161-316, :392-500)
+  MMDoubleStreamBlock.forward / MMSingleStreamBlock.forward of HunyuanVideo-I2V
+      (hyvideo_i2v/modules/models_mul.py:136-319, :393-505)
   WanSelfAttention.forward            (wan/modules/model_mul.py:134-180)
 
 with versions whose attention section is `jenga_hy_prologue` / `jenga_wan_prologue` (RMSNorm +
@@ -15,7 +17,14 @@ followed by select_blocks + the carved-attention launch.  Everything around the 
 section (modulation, linear layers, gates, MLP) is executed by the block's own sub-modules and
 the reference module's own helper functions (`modulate`, `apply_gate`), so those numerics are the
 reference's by construction.  Whenever a call is not the carved configuration (sa_drop_rate == 0,
-no RMS qk-norm, unusual dtype, batch > 1 for Wan, …) the ORIGINAL forward runs.
+no RMS qk-norm, unusual dtype, batch > 1 for Wan, sequence parallel for I2V, …) the ORIGINAL forward
+runs.
+
+The I2V blocks differ from the HunyuanVideo ones in three ways the fused forwards follow: the
+token-replace modulation (rows of the first frame take the `tr_` shift / scale / gate; the
+reference does it with boolean-mask index_put, modulate_layers.py:51-56,84-95, here it is a per-row
+parameter select inside the ln_modulate / gate_residual kernels), a ragged S = L + 400 that the
+operator zero-pads to whole blocks, and the operator's default text_blocks=4.
 
 A second hook routes `x[:, long_index]` / `x[long_index]` on contiguous CUDA activations — the
 token reorder of jenga_hyvideo.py:116-118,226 and jenga_wan.py:559,655 — to `jenga_gather_rows`.
@@ -33,9 +42,13 @@ from . import hyvideo as HY
 from . import wan as WAN
 
 _HY_MODULES = ("hyvideo.modules.models_mul_block_gc_ha_multigpu",)
+_I2V_MODULES = ("hyvideo_i2v.modules.models_mul",)
 _WAN_MODULES = ("wan.modules.model_mul",)
-STATS = {"hy_double": 0, "hy_single": 0, "wan_self": 0, "fallback": 0, "gather": 0, "ln_modulate": 0,
-         "gate_residual": 0, "gelu_cat": 0}
+STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "wan_self": 0, "fallback": 0,
+         "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0}
+# the HunyuanVideo-I2V operator's text_blocks default (hyvideo_i2v/…/attention_block_triton_diffres.py:409);
+# models_mul.py never passes text_blocks, so it holds whatever the text length
+_I2V_TEXT_BLOCKS = 4
 
 
 # ------------------------------------------------------------------------------------------------
@@ -54,27 +67,35 @@ def _carved_call(x, sa_drop_rate, curve_sel):
             and curve_sel is not None and not isinstance(curve_sel, int))
 
 
-def _ln_mod(mod, norm, x, shift, scale):
-    """modulate(norm(x), shift, scale) — one fused pass when it is the autocast-bf16 chain."""
-    if DN.ln_modulate_supported(x, norm, shift, scale):
+def _ln_mod(mod, norm, x, shift, scale, tr=None):
+    """modulate(norm(x), shift, scale) — one fused pass when it is the autocast-bf16 chain.
+    tr=(tr_shift, tr_scale, first_frame_mask): the I2V token-replace form (modulate_layers.py:51-56)."""
+    if DN.ln_modulate_supported(x, norm, shift, scale, tr=tr):
         STATS["ln_modulate"] += 1
-        return DN.ln_modulate(x, shift, scale, eps=norm.eps)
-    return mod.modulate(norm(x), shift=shift, scale=scale)
+        return DN.ln_modulate(x, shift, scale, eps=norm.eps, tr=tr)
+    if tr is None:
+        return mod.modulate(norm(x), shift=shift, scale=scale)
+    return mod.modulate(norm(x), shift=shift, scale=scale, condition_type="token_replace", tr_shift=tr[0],
+                        tr_scale=tr[1], first_frame_mask=tr[2])
 
 
-def _gate_res(mod, x, y, gate):
-    """x + apply_gate(y, gate) — one fused pass for bf16 batch-1 tensors."""
-    if DN.gate_residual_supported(x, y, gate):
+def _gate_res(mod, x, y, gate, tr=None):
+    """x + apply_gate(y, gate) — one fused pass for bf16 batch-1 tensors.
+    tr=(tr_gate, first_frame_mask): the I2V token-replace form (modulate_layers.py:84-95)."""
+    if DN.gate_residual_supported(x, y, gate, tr=tr):
         STATS["gate_residual"] += 1
-        return DN.gate_residual(x, y, gate)
-    return x + mod.apply_gate(y, gate=gate)
+        return DN.gate_residual(x, y, gate, tr=tr)
+    if tr is None:
+        return x + mod.apply_gate(y, gate=gate)
+    return x + mod.apply_gate(y, gate=gate, condition_type="token_replace", tr_gate=tr[0], first_frame_mask=tr[1])
 
 
 def _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis, cu_seqlens_q, cu_seqlens_kv,
                        sa_drop_rate, txt_amp, curve_sel, p_remain_rates, txt_block_num, per_block_token,
-                       text_blocks_default, out=None):
+                       text_blocks_default, out=None, pad_ragged=False):
     """prologue -> (SP exchange | select + carved attention).  Returns attn [B, L+T, H*D]
-    (written into `out`, a [B, L+T, H, D] view, when given and not under SP)."""
+    (written into `out`, a [B, L+T, H, D] view, when given and not under SP).
+    pad_ragged: S = L+T need not be a multiple of 128 (the I2V operator zero-pads it)."""
     (wq_i, eps), (wk_i, _), (wq_t, _), (wk_t, _) = norms
     heads = self.heads_num
     L = img_qkv.shape[1]
@@ -83,7 +104,7 @@ def _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis, cu_seqlens
     sp = getattr(self, "hybrid_seq_parallel_attn", None)
     want_pool = not sp
     S = L + (0 if txt_qkv is None else txt_qkv.shape[1])
-    if want_pool and S % HY.BLOCK:
+    if want_pool and S % HY.BLOCK and not pad_ragged:
         return None
     q, k, v, pools = HY.attention_prologue(img_qkv, txt_qkv, heads, wq_i, wk_i, wq_t, wk_t, eps, freqs_cis,
                                            want_pool=want_pool)
@@ -95,7 +116,8 @@ def _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis, cu_seqlens
                                          p_remain_rates=p_remain_rates)
     return HY.carved_attention_from_pools(q, k, v, pools, top_k=top_k, text_blocks=txt_block_num,
                                           text_amp=txt_amp, block_neighbor_list=block_neighbor_list,
-                                          p_remain_rates=p_remain_rates, cu_seqlens_q=cu_seqlens_q, out=out)
+                                          p_remain_rates=p_remain_rates, cu_seqlens_q=cu_seqlens_q, out=out,
+                                          pad_ragged=pad_ragged)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -191,6 +213,123 @@ def _make_single_forward(orig, mod, text_blocks_default):
 
 
 # ------------------------------------------------------------------------------------------------
+# HunyuanVideo-I2V blocks
+# ------------------------------------------------------------------------------------------------
+def _i2v_eligible(self, x, sa_drop_rate, curve_sel, norms, per_block_token, cu_seqlens_q, S, tr, mask):
+    """the carved configuration the fused I2V forwards take; anything else runs the original"""
+    return (_carved_call(x, sa_drop_rate, curve_sel) and None not in norms and per_block_token == HY.BLOCK
+            and cu_seqlens_q is not None and x.shape[-1] // self.heads_num == 128
+            # sequence parallel: the reference runs the dense parallel_attention (:264-274, :483-493)
+            and not getattr(self, "hybrid_seq_parallel_attn", None)
+            # the prefix form (frist_frame_token_num) is only reached outside the Jenga forward
+            and not (tr and mask is None)
+            and (S + HY.BLOCK - 1) // HY.BLOCK > _I2V_TEXT_BLOCKS)
+
+
+def _make_i2v_double_forward(orig, mod):
+    def forward(self, img, txt, vec, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
+                max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, first_frame_mask=None,
+                condition_type=None, token_replace_vec=None, frist_frame_token_num=None, txt_amp=0.0,
+                curve_sel=None, p_remain_rates=0.5, per_block_token=128):
+        args = (img, txt, vec, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv, freqs_cis, sa_drop_rate,
+                first_frame_mask, condition_type, token_replace_vec, frist_frame_token_num, txt_amp, curve_sel,
+                p_remain_rates, per_block_token)
+        tr = condition_type == "token_replace"
+        norms = [_rms_params(n) for n in (self.img_attn_q_norm, self.img_attn_k_norm,
+                                          self.txt_attn_q_norm, self.txt_attn_k_norm)]
+        L = img.shape[1]
+        if not _i2v_eligible(self, img, sa_drop_rate, curve_sel, norms, per_block_token, cu_seqlens_q,
+                             L + txt.shape[1], tr, first_frame_mask):
+            STATS["fallback"] += 1
+            return orig(self, *args)
+        if tr:                                                                         # :156-179
+            img_mods, tr_mods = self.img_mod(vec, condition_type=condition_type, token_replace_vec=token_replace_vec)
+            i_shift1, i_scale1, i_gate1, i_shift2, i_scale2, i_gate2 = img_mods.chunk(6, dim=-1)
+            r_shift1, r_scale1, r_gate1, r_shift2, r_scale2, r_gate2 = tr_mods.chunk(6, dim=-1)
+            tr_mod1 = (r_shift1, r_scale1, first_frame_mask)
+            tr_mod2 = (r_shift2, r_scale2, first_frame_mask)
+            tr_gate1, tr_gate2 = (r_gate1, first_frame_mask), (r_gate2, first_frame_mask)
+        else:
+            i_shift1, i_scale1, i_gate1, i_shift2, i_scale2, i_gate2 = self.img_mod(vec).chunk(6, dim=-1)
+            tr_mod1 = tr_mod2 = tr_gate1 = tr_gate2 = None
+        t_shift1, t_scale1, t_gate1, t_shift2, t_scale2, t_gate2 = self.txt_mod(vec).chunk(6, dim=-1)
+        img_qkv = self.img_attn_qkv(_ln_mod(mod, self.img_norm1, img, i_shift1, i_scale1, tr=tr_mod1))
+        txt_qkv = self.txt_attn_qkv(_ln_mod(mod, self.txt_norm1, txt, t_shift1, t_scale1))
+        assert cu_seqlens_q.shape[0] == 2 * img.shape[0] + 1                         # :235-237
+        attn = _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis, cu_seqlens_q, cu_seqlens_kv,
+                                  sa_drop_rate, txt_amp, curve_sel, p_remain_rates, _I2V_TEXT_BLOCKS,
+                                  per_block_token, _I2V_TEXT_BLOCKS, pad_ragged=True)
+        STATS["i2v_double"] += 1
+        img_attn, txt_attn = attn[:, :L], attn[:, L:]
+        img = _gate_res(mod, img, self.img_attn_proj(img_attn), i_gate1, tr=tr_gate1)   # :281-306
+        img = _gate_res(mod, img, self.img_mlp(_ln_mod(mod, self.img_norm2, img, i_shift2, i_scale2, tr=tr_mod2)),
+                        i_gate2, tr=tr_gate2)
+        txt = _gate_res(mod, txt, self.txt_attn_proj(txt_attn), t_gate1)                 # :309-317
+        txt = _gate_res(mod, txt, self.txt_mlp(_ln_mod(mod, self.txt_norm2, txt, t_shift2, t_scale2)), t_gate2)
+        return img, txt
+    forward.__jenga_b200__ = True
+    forward.__wrapped__ = orig
+    return forward
+
+
+def _make_i2v_single_forward(orig, mod):
+    def forward(self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
+                max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, first_frame_mask=None,
+                condition_type=None, token_replace_vec=None, frist_frame_token_num=None, txt_amp=0.0,
+                curve_sel=None, p_remain_rates=0.5, per_block_token=128):
+        args = (x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv, freqs_cis, sa_drop_rate,
+                first_frame_mask, condition_type, token_replace_vec, frist_frame_token_num, txt_amp, curve_sel,
+                p_remain_rates, per_block_token)
+        tr = condition_type == "token_replace"
+        norms = [_rms_params(n) for n in (self.q_norm, self.k_norm)]
+        if (not _i2v_eligible(self, x, sa_drop_rate, curve_sel, norms, per_block_token, cu_seqlens_q, x.shape[1],
+                              tr, first_frame_mask)
+                or freqs_cis is None or not 0 < txt_len < x.shape[1]):
+            STATS["fallback"] += 1
+            return orig(self, *args)
+        if tr:                                                                         # :413-424
+            mods, tr_mods = self.modulation(vec, condition_type=condition_type, token_replace_vec=token_replace_vec)
+            shift, scale, gate = mods.chunk(3, dim=-1)
+            r_shift, r_scale, r_gate = tr_mods.chunk(3, dim=-1)
+            # full_first_frame_mask (jenga_hyi2v.py:129-130): a CPU bool over L+T rows
+            tr_mod, tr_gate = (r_shift, r_scale, first_frame_mask), (r_gate, first_frame_mask)
+        else:
+            shift, scale, gate = self.modulation(vec).chunk(3, dim=-1)
+            tr_mod = tr_gate = None
+        lin1 = self.linear1(_ln_mod(mod, self.pre_norm, x, shift, scale, tr=tr_mod))
+        C3 = 3 * self.hidden_size
+        L = x.shape[1] - txt_len
+        # strided views into linear1's output: no split / rearrange / cat copies (:431-451)
+        img_qkv, txt_qkv = lin1[:, :L, :C3], lin1[:, L:, :C3]
+        mlp = lin1[:, :, C3:]
+        assert cu_seqlens_q.shape[0] == 2 * x.shape[0] + 1                           # :464-466
+        # `torch.cat((attn, self.mlp_act(mlp)), 2)` (:497) without the concatenation copy, as in the
+        # HunyuanVideo single-stream forward above
+        act = self.mlp_act
+        fuse_cat = (isinstance(act, torch.nn.GELU) and getattr(act, "approximate", "none") == "tanh"
+                    and lin1.dtype == torch.bfloat16 and x.shape[0] == 1)
+        cat = attn_view = None
+        if fuse_cat:
+            cat = torch.empty((x.shape[0], x.shape[1], C3 // 3 + mlp.shape[-1]), dtype=lin1.dtype, device=lin1.device)
+            attn_view = cat[:, :, :C3 // 3].unflatten(2, (self.heads_num, -1))
+        attn = _attention_section(self, mod, img_qkv, txt_qkv, [norms[0], norms[1], norms[0], norms[1]],
+                                  freqs_cis, cu_seqlens_q, cu_seqlens_kv, sa_drop_rate, txt_amp, curve_sel,
+                                  p_remain_rates, _I2V_TEXT_BLOCKS, per_block_token, _I2V_TEXT_BLOCKS,
+                                  out=attn_view, pad_ragged=True)
+        STATS["i2v_single"] += 1
+        if fuse_cat:
+            STATS["gelu_cat"] += 1
+            DN.gelu_tanh_into(mlp, cat[:, :, C3 // 3:])
+            out = self.linear2(cat)
+        else:
+            out = self.linear2(torch.cat((attn, act(mlp)), 2))
+        return _gate_res(mod, x, out, gate, tr=tr_gate)                              # :499-505
+    forward.__jenga_b200__ = True
+    forward.__wrapped__ = orig
+    return forward
+
+
+# ------------------------------------------------------------------------------------------------
 # Wan self-attention
 # ------------------------------------------------------------------------------------------------
 def _make_wan_forward(orig, mod):
@@ -230,12 +369,17 @@ def patch_module(mod) -> list[str]:
     """Patches the block classes of an already imported reference module; returns what it did."""
     done = []
     name = mod.__name__
-    # hyvideo_i2v/modules/models_mul.py builds a different token layout in front of the operator
-    # (image-condition tokens, token_replace modulation): it gets the operator hook only.
-    if (name.startswith("hyvideo.") and hasattr(mod, "MMDoubleStreamBlock")
+    # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
+    # a ragged S with four text blocks: its own pair of forwards
+    i2v = name.startswith("hyvideo_i2v.")
+    if ((name.startswith("hyvideo.") or i2v) and hasattr(mod, "MMDoubleStreamBlock")
             and not getattr(mod.MMDoubleStreamBlock.forward, "__jenga_b200__", False)):
-        mod.MMDoubleStreamBlock.forward = _make_double_forward(mod.MMDoubleStreamBlock.forward, mod, 2)
-        mod.MMSingleStreamBlock.forward = _make_single_forward(mod.MMSingleStreamBlock.forward, mod, 2)
+        if i2v:
+            mod.MMDoubleStreamBlock.forward = _make_i2v_double_forward(mod.MMDoubleStreamBlock.forward, mod)
+            mod.MMSingleStreamBlock.forward = _make_i2v_single_forward(mod.MMSingleStreamBlock.forward, mod)
+        else:
+            mod.MMDoubleStreamBlock.forward = _make_double_forward(mod.MMDoubleStreamBlock.forward, mod, 2)
+            mod.MMSingleStreamBlock.forward = _make_single_forward(mod.MMSingleStreamBlock.forward, mod, 2)
         done += [f"{name}.MMDoubleStreamBlock.forward", f"{name}.MMSingleStreamBlock.forward"]
     if hasattr(mod, "WanSelfAttention") and not getattr(mod.WanSelfAttention.forward, "__jenga_b200__", False):
         orig = mod.WanSelfAttention.forward
@@ -266,7 +410,7 @@ class _PatchingLoader(importlib.abc.Loader):
 
 
 class _PatchFinder(importlib.abc.MetaPathFinder):
-    targets = _HY_MODULES + _WAN_MODULES
+    targets = _HY_MODULES + _I2V_MODULES + _WAN_MODULES
 
     def find_spec(self, fullname, path, target=None):
         if fullname not in self.targets:

@@ -3,8 +3,14 @@
 Host mirror of csrc/dense_fused.cu; each function replaces a chain of ATen kernels of
 hyvideo/modules/models_mul_block_gc_ha_multigpu.py (file:line in each docstring) with one pass
 that keeps the chain's rounding points under torch.autocast(bf16).  bf16 CUDA tensors only; the
-callers (jenga_b200/blocks.py) fall back to the reference's own ops for anything else."""
+callers (jenga_b200/blocks.py) fall back to the reference's own ops for anything else.
+
+`ln_modulate` and `gate_residual` also take the token-replace form of HunyuanVideo-I2V
+(hyvideo_i2v/modules/modulate_layers.py:51-56,84-95): `tr=(tr_shift, tr_scale, row_mask)` /
+`tr=(tr_gate, row_mask)`, where rows whose mask entry is true take the tr_ parameters."""
 from __future__ import annotations
+
+import weakref
 
 import torch
 
@@ -30,51 +36,112 @@ def _rows2d(x: torch.Tensor):
     return rows, stride
 
 
-def ln_modulate_supported(x: torch.Tensor, norm: torch.nn.Module, shift, scale) -> bool:
+_MASK_CACHE: dict = {}
+
+
+def _tr_supported(x: torch.Tensor, vecs, mask) -> bool:
+    """token-replace parameters: bf16 vectors and a 1-D bool mask with one entry per row of x
+    (on x's device, or on the CPU)"""
+    return (all(v is not None and v.dtype == torch.bfloat16 for v in vecs) and isinstance(mask, torch.Tensor)
+            and mask.dtype == torch.bool and mask.dim() == 1 and mask.numel() == x.shape[-2]
+            and (mask.device == x.device or mask.device.type == "cpu"))
+
+
+def _row_mask(mask: torch.Tensor, device: torch.device) -> torch.Tensor:
+    """One byte per row on `device`.  A contiguous bool mask already there is used as it is; a CPU
+    mask (the single-stream block's `full_first_frame_mask`, jenga_hyi2v.py:129-130, built anew on
+    every forward and shared by all blocks) is copied once and cached by tensor identity and
+    version, as attention.neighbour_bits caches the adjacency."""
+    if mask.device == device:
+        return mask if mask.dtype == torch.bool and mask.is_contiguous() else mask.to(torch.bool).contiguous()
+    key = (mask.data_ptr(), mask.numel(), mask._version, str(device))
+    hit = _MASK_CACHE.get(key)
+    # the entry remembers WHICH tensor it was copied from: a freed mask whose address is reused by
+    # the next forward's mask must not hit
+    if hit is not None and hit[0]() is mask:
+        return hit[1]
+    dev = mask.to(device=device, dtype=torch.bool).contiguous()
+    if len(_MASK_CACHE) > 8:
+        _MASK_CACHE.clear()
+    _MASK_CACHE[key] = (weakref.ref(mask), dev)
+    return dev
+
+
+def _per_channel(v: torch.Tensor, C: int, what: str) -> torch.Tensor:
+    v = v.reshape(-1).contiguous()
+    if v.numel() != C:
+        raise ValueError(f"{what} must hold one value per channel (batch 1)")
+    return v
+
+
+def ln_modulate_supported(x: torch.Tensor, norm: torch.nn.Module, shift, scale, tr=None) -> bool:
     return (isinstance(norm, torch.nn.LayerNorm) and norm.weight is None and norm.bias is None
             and x.is_cuda and x.dtype == torch.bfloat16 and torch.is_autocast_enabled()
             and torch.get_autocast_dtype("cuda") == torch.bfloat16 and x.dim() == 3 and x.shape[0] == 1
             and shift is not None and scale is not None and shift.dtype == torch.bfloat16
             and scale.dtype == torch.bfloat16 and x.shape[-1] % 8 == 0 and x.shape[-1] <= 6144
-            and x.stride(-1) == 1 and x.stride(-2) % 8 == 0)
+            and x.stride(-1) == 1 and x.stride(-2) % 8 == 0
+            and (tr is None or _tr_supported(x, tr[:2], tr[2])))
 
 
-def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6) -> torch.Tensor:
+def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6,
+                tr=None) -> torch.Tensor:
     """`modulate(LayerNorm(x), shift=shift, scale=scale)` followed by the bf16 cast the next Linear
     applies under autocast (models_mul…:196-199,297-304,409; modulate_layers.py:31-49).
-    x [1, L, C] bf16, shift/scale [1, C] bf16 -> [1, L, C] bf16."""
+    x [1, L, C] bf16, shift/scale [1, C] bf16 -> [1, L, C] bf16.
+    tr=(tr_shift, tr_scale, row_mask): the token-replace form (hyvideo_i2v/…/modulate_layers.py:51-56),
+    row_mask a bool [L] on x's device or on the CPU."""
     _require_cuda(x, shift, scale)
     rows, xs = _rows2d(x)
     C = x.shape[-1]
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    sc, sh = scale.reshape(-1).contiguous(), shift.reshape(-1).contiguous()
-    if sc.numel() != C or sh.numel() != C:
-        raise ValueError("shift / scale must hold one value per channel (batch 1)")
+    sc, sh = _per_channel(scale, C, "scale"), _per_channel(shift, C, "shift")
     with torch.cuda.device(x.device):
-        check(lib.jenga_ln_modulate(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(), C, rows, C,
-                                    float(eps), _stream_ptr(x.device)), "ln_modulate")
+        if tr is None:
+            check(lib.jenga_ln_modulate(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(), C, rows, C,
+                                        float(eps), _stream_ptr(x.device)), "ln_modulate")
+            return out
+        tr_shift, tr_scale, mask = tr
+        _require_cuda(tr_shift, tr_scale)
+        tsc, tsh = _per_channel(tr_scale, C, "tr_scale"), _per_channel(tr_shift, C, "tr_shift")
+        if mask.dim() != 1 or mask.numel() != rows:
+            raise ValueError("row mask must hold one entry per row")
+        m = _row_mask(mask, x.device)
+        check(lib.jenga_ln_modulate_tr(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), tsc.data_ptr(), tsh.data_ptr(),
+                                       m.data_ptr(), out.data_ptr(), C, rows, C, float(eps), _stream_ptr(x.device)),
+              "ln_modulate_tr")
     return out
 
 
-def gate_residual_supported(x, y, gate) -> bool:
+def gate_residual_supported(x, y, gate, tr=None) -> bool:
     return (x.is_cuda and x.dtype == y.dtype == torch.bfloat16 and gate is not None and gate.dtype == torch.bfloat16
             and x.shape == y.shape and x.dim() == 3 and x.shape[0] == 1 and x.shape[-1] % 8 == 0
-            and x.stride(-1) == 1 and y.stride(-1) == 1 and x.stride(-2) % 8 == 0 and y.stride(-2) % 8 == 0)
+            and x.stride(-1) == 1 and y.stride(-1) == 1 and x.stride(-2) % 8 == 0 and y.stride(-2) % 8 == 0
+            and (tr is None or _tr_supported(x, tr[:1], tr[1])))
 
 
-def gate_residual(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
-    """`x + apply_gate(y, gate=gate)` (models_mul…:295-315,:500; modulate_layers.py:52-68)."""
+def gate_residual(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor, tr=None) -> torch.Tensor:
+    """`x + apply_gate(y, gate=gate)` (models_mul…:295-315,:500; modulate_layers.py:52-68).
+    tr=(tr_gate, row_mask): the token-replace form (hyvideo_i2v/…/modulate_layers.py:84-95)."""
     _require_cuda(x, y, gate)
     rows, xs = _rows2d(x)
     _, ys = _rows2d(y)
     C = x.shape[-1]
-    g = gate.reshape(-1).contiguous()
-    if g.numel() != C:
-        raise ValueError("gate must hold one value per channel (batch 1)")
+    g = _per_channel(gate, C, "gate")
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     with torch.cuda.device(x.device):
-        check(lib.jenga_gate_residual(x.data_ptr(), xs, y.data_ptr(), ys, g.data_ptr(), out.data_ptr(), C, rows, C,
-                                      _stream_ptr(x.device)), "gate_residual")
+        if tr is None:
+            check(lib.jenga_gate_residual(x.data_ptr(), xs, y.data_ptr(), ys, g.data_ptr(), out.data_ptr(), C, rows,
+                                          C, _stream_ptr(x.device)), "gate_residual")
+            return out
+        tr_gate, mask = tr
+        _require_cuda(tr_gate)
+        tg = _per_channel(tr_gate, C, "tr_gate")
+        if mask.dim() != 1 or mask.numel() != rows:
+            raise ValueError("row mask must hold one entry per row")
+        m = _row_mask(mask, x.device)
+        check(lib.jenga_gate_residual_tr(x.data_ptr(), xs, y.data_ptr(), ys, g.data_ptr(), tg.data_ptr(), m.data_ptr(),
+                                         out.data_ptr(), C, rows, C, _stream_ptr(x.device)), "gate_residual_tr")
     return out
 
 

@@ -111,13 +111,19 @@ def attention_prologue(img_qkv: torch.Tensor, txt_qkv: torch.Tensor | None, head
 
 def carved_attention_from_pools(q, k, v, pools, *, top_k: int, text_blocks: int = 2, text_amp: float = 0.0,
                                 block_neighbor_list=None, p_remain_rates: float = 0.5,
-                                cu_seqlens_q=None, shape_xfuse: bool = False, out: torch.Tensor | None = None):
+                                cu_seqlens_q=None, shape_xfuse: bool = False, out: torch.Tensor | None = None,
+                                pad_ragged: bool = False):
     """block_sparse_attention (…triton_diffres.py:399) when the prologue already produced the
-    pooled block means: select_blocks + one carved-attention launch (2 launches per layer)."""
+    pooled block means: select_blocks + one carved-attention launch (2 launches per layer).
+    pad_ragged: S need not be a multiple of 128 — the HunyuanVideo-I2V operator
+    (hyvideo_i2v/…/attention_block_triton_diffres.py:320-335,385) zero-pads S to nb*128 blocks, the
+    dense (text) query blocks attend all nb*128 keys and the output is trimmed to S.  The
+    HunyuanVideo operator refuses ragged S (its :216 reshape fails), and so does this function
+    without pad_ragged."""
     B, S, H, D = q.shape
-    if S % BLOCK:
+    if S % BLOCK and not pad_ragged:
         raise ValueError("hyvideo variant needs S % 128 == 0")
-    nb = S // BLOCK
+    nb = (S + BLOCK - 1) // BLOCK
     n_img = nb - text_blocks
     qp, kp = pools
     nbr = neighbour_bits(block_neighbor_list, q.device) if block_neighbor_list is not None else None
@@ -133,8 +139,10 @@ def carved_attention_from_pools(q, k, v, pools, *, top_k: int, text_blocks: int 
     from . import attention as _A
     v8 = _A.quantize_v_fp8(v) if (_A.PV_FP8 and q.dtype == torch.bfloat16) else None   # opt-in FP8 P.V variant
     qk8 = _A.quantize_qk_int8(q, k) if _A.QK_INT8 else None                              # opt-in INT8 Q.K^T variant
-    _launch(q, k, v, bits, n_img, text_blocks, D ** -0.5, text_amp, n_img, S, S, S, out, seq, q.dtype, v_fp8=v8,
-            qk_int8=qk8)
+    # kv_limit_dense = nb*128: the padded keys are zeros that the dense rows' softmax still counts
+    # (== S when S % 128 == 0)
+    _launch(q, k, v, bits, n_img, text_blocks, D ** -0.5, text_amp, n_img, S, S, nb * BLOCK, out, seq, q.dtype,
+            v_fp8=v8, qk_int8=qk8)
     if shape_xfuse:
         return out
     return out.reshape(B, S, H * D) if out.is_contiguous() else out.flatten(2)
