@@ -429,6 +429,22 @@ typedef struct JengaQkInt8Args {
 } JengaQkInt8Args;
 int jenga_carved_attn_fwd_qk_int8(const JengaAttnArgs* args, const JengaQkInt8Args* qk, void* stream);
 
+/* jenga_carved_attn_fwd (qk == NULL) or jenga_carved_attn_fwd_qk_int8 (qk != NULL), with the work
+ * ordered first by a small pass on the same stream: every dense query block, then each head's sparse
+ * blocks by live-tile count, longest first.  Blocks that run side by side then walk rows of nearly
+ * equal length, in step, and share K/V tiles through L2.  Every row computes exactly what it computes
+ * without the schedule: the results are the same bit for bit.  The pass writes the order into
+ * `workspace` (device, 4-byte aligned, jenga_carved_attn_sched_workspace_bytes(batch, heads,
+ * nq_sparse, nq_dense) = 4 * batch * heads * (nq_sparse + nq_dense) bytes), which must stay untouched
+ * until the launch completes; concurrent launches need separate workspaces. */
+typedef struct JengaAttnSched {
+  void* workspace;
+  int64_t workspace_bytes;
+} JengaAttnSched;
+int jenga_carved_attn_fwd_sched(const JengaAttnArgs* args, const JengaQkInt8Args* qk /* nullable */,
+                                const JengaAttnSched* sched, void* stream);
+int64_t jenga_carved_attn_sched_workspace_bytes(int32_t batch, int32_t heads, int32_t nq_sparse, int32_t nq_dense);
+
 #ifdef __cplusplus
 }
 #endif

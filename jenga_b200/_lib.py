@@ -48,6 +48,10 @@ class JengaQkInt8Args(C.Structure):
     ]
 
 
+class JengaAttnSched(C.Structure):
+    _fields_ = [("workspace", C.c_void_p), ("workspace_bytes", C.c_int64)]
+
+
 class JengaUlyssesScatterArgs(C.Structure):
     _fields_ = [
         ("x", C.c_void_p * 3), ("joint", C.c_void_p * 3),
@@ -189,6 +193,11 @@ def _load() -> C.CDLL:
     lib.jenga_quantize_int8.restype = C.c_int
     lib.jenga_carved_attn_fwd_qk_int8.argtypes = [C.POINTER(JengaAttnArgs), C.POINTER(JengaQkInt8Args), C.c_void_p]
     lib.jenga_carved_attn_fwd_qk_int8.restype = C.c_int
+    lib.jenga_carved_attn_fwd_sched.argtypes = [C.POINTER(JengaAttnArgs), C.POINTER(JengaQkInt8Args),
+                                                C.POINTER(JengaAttnSched), C.c_void_p]
+    lib.jenga_carved_attn_fwd_sched.restype = C.c_int
+    lib.jenga_carved_attn_sched_workspace_bytes.argtypes = [C.c_int32] * 4
+    lib.jenga_carved_attn_sched_workspace_bytes.restype = C.c_int64
     lib.jenga_gilbert_xyz2d.argtypes = [C.c_int] * 6
     lib.jenga_gilbert_xyz2d.restype = C.c_int64
     if lib.jenga_abi_version() != 3:

@@ -394,16 +394,21 @@ def _launch(q, k, v, mask_bits, nq_sparse, nq_dense, sm_scale, text_amp, text_bl
     a.kv_limit_sparse, a.q_limit_sparse, a.kv_limit_dense = kv_limit_sparse, q_limit_sparse, kv_limit_dense
     a.seqlen_dev = seqlen_dev.data_ptr() if seqlen_dev is not None else None
     a.err_flag = None
+    x = None
+    if qk_int8 is not None:
+        q8, q_scale, k8, k_scale = qk_int8
+        x = _lib.JengaQkInt8Args()
+        x.q_i8, x.q_scale, x.k_i8, x.k_scale = q8.data_ptr(), q_scale.data_ptr(), k8.data_ptr(), k_scale.data_ptr()
+        x.q_rows_padded, x.kv_rows_padded = q8.shape[1], k8.shape[1]
     with torch.cuda.device(q.device):
-        if qk_int8 is None:
-            check(lib.jenga_carved_attn_fwd(C.byref(a), _stream_ptr(q.device)), "carved_attn_fwd")
-        else:
-            q8, q_scale, k8, k_scale = qk_int8
-            x = _lib.JengaQkInt8Args()
-            x.q_i8, x.q_scale, x.k_i8, x.k_scale = q8.data_ptr(), q_scale.data_ptr(), k8.data_ptr(), k_scale.data_ptr()
-            x.q_rows_padded, x.kv_rows_padded = q8.shape[1], k8.shape[1]
-            check(lib.jenga_carved_attn_fwd_qk_int8(C.byref(a), C.byref(x), _stream_ptr(q.device)),
-                  "carved_attn_fwd_qk_int8")
+        # the work order of this launch (jenga_carved_attn_fwd_sched): stream-ordered from the caching
+        # allocator, so launches on other streams each get their own
+        sched = _lib.JengaAttnSched()
+        sched.workspace_bytes = lib.jenga_carved_attn_sched_workspace_bytes(B, H, nq_sparse, nq_dense)
+        ws = torch.empty(max(sched.workspace_bytes, 1), dtype=torch.uint8, device=q.device)
+        sched.workspace = ws.data_ptr()
+        check(lib.jenga_carved_attn_fwd_sched(C.byref(a), C.byref(x) if x is not None else None, C.byref(sched),
+                                              _stream_ptr(q.device)), "carved_attn_fwd_sched")
     return out
 
 

@@ -161,6 +161,17 @@ extern "C" int jenga_carved_attn_fwd_qk_int8(const JengaAttnArgs* args, const Je
   return carved_attn_fwd_impl(args, static_cast<cudaStream_t>(stream), qk);
 }
 
+extern "C" int jenga_carved_attn_fwd_sched(const JengaAttnArgs* args, const JengaQkInt8Args* qk,
+                                           const JengaAttnSched* sched, void* stream) {
+  if (!sched) return set_error(JENGA_E_INVALID, "sched: null pointer");
+  return carved_attn_fwd_impl(args, static_cast<cudaStream_t>(stream), qk, sched);
+}
+
+extern "C" int64_t jenga_carved_attn_sched_workspace_bytes(int32_t batch, int32_t heads, int32_t nq_sparse,
+                                                           int32_t nq_dense) {
+  return carved_attn_sched_workspace_bytes(batch, heads, nq_sparse, nq_dense);
+}
+
 extern "C" int jenga_gather_rows(const void* src, void* dst, const int64_t* index, int64_t n_index,
                                  int64_t n_src_rows, int64_t row_bytes, int batch,
                                  int64_t src_batch_stride, int64_t dst_batch_stride, void* stream) {

@@ -29,6 +29,10 @@
 // HBM/L2 layout: q,k,v stay in the caller's [B,S,H,D] layout; TMA boxes are {64 d, 128 rows}
 // with 128-byte swizzle.  K boxes are K-major wgmma operands, V boxes MN-major (no transpose).
 // CTAs are numbered head-major so that all CTAs in flight read the same head's K/V out of L2.
+// With a schedule (jenga_carved_attn_fwd_sched) a small pass first orders the work: every dense
+// block first (the longest), then each head's sparse blocks by live-tile count, longest first.  The
+// CTAs that run side by side then walk rows of nearly equal length, finish together and start the
+// next rows together, so they sweep the keys in step and share each K/V tile through L2.
 #include <cfloat>
 
 #include "carved_attn_common.cuh"
@@ -107,10 +111,12 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // ---- which tile is this CTA?  head-major; within a head the (long) dense blocks first ----
+  // ---- which tile is this CTA?  Items are numbered head-major, within a head the dense blocks
+  // first; p.order (when given) says which item each CTA runs ----
+  const int item = p.order ? __ldg(p.order + blockIdx.x) : static_cast<int>(blockIdx.x);
   const int per_bh = p.nq_sparse + p.nq_dense;
-  const int bh = blockIdx.x / per_bh;
-  const int local = blockIdx.x - bh * per_bh;
+  const int bh = item / per_bh;
+  const int local = item - bh * per_bh;
   const bool dense = local < p.nq_dense;
   const int qb = dense ? p.nq_sparse + local : local - p.nq_dense;
   const int b = bh / p.heads;
@@ -519,6 +525,66 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
   }
 }
 
+// live tiles of sparse row r of head bh: what the attention kernel's mask staging keeps
+__device__ int sparse_row_tiles(const KernelParams& p, int bh, int r, long long q_limit) {
+  if (static_cast<long long>(r) * kBlock >= q_limit) return 0;
+  const uint32_t* m = p.mask_bits + (static_cast<size_t>(bh) * p.nq_sparse + r) * p.mask_words;
+  int n = 0;
+  for (int w = 0; w < p.mask_words; ++w) {
+    uint32_t bits = __ldg(m + w);
+    const int rem = p.nb_kv - w * 32;
+    if (rem < 32) bits &= rem > 0 ? ((1u << rem) - 1u) : 0u;
+    n += __popc(bits);
+  }
+  return n;
+}
+
+constexpr int kOrderThreads = 256;
+
+// One CTA per batch*head.  order[0, B*H*nq_dense) = the dense items (head-major); then, head after
+// head, the head's sparse items by live-tile count, longest first, ties in row order (a stable
+// counting sort: the schedule is deterministic).  Items are numbered as the attention kernel decodes
+// them.  Dynamic shared memory: (nb_kv + 1 + kOrderThreads) ints.
+__global__ void __launch_bounds__(kOrderThreads) carved_attn_order_kernel(const KernelParams p, int* order) {
+  extern __shared__ int s_order[];
+  int* start = s_order;                   // [nb_kv + 1]: count histogram, then first slot per count
+  int* chunk = s_order + p.nb_kv + 1;     // [kOrderThreads]: counts of the current chunk of rows
+  const int bh = blockIdx.x;
+  const int per_bh = p.nq_sparse + p.nq_dense;
+  for (int i = threadIdx.x; i < p.nq_dense; i += kOrderThreads) order[bh * p.nq_dense + i] = bh * per_bh + i;
+  if (p.nq_sparse == 0) return;
+  const long long seqlen_over = p.seqlen_dev ? static_cast<long long>(__ldg(p.seqlen_dev)) : -1;
+  const long long q_limit = seqlen_over >= 0 ? seqlen_over : p.q_limit_sparse;
+  for (int c = threadIdx.x; c <= p.nb_kv; c += kOrderThreads) start[c] = 0;
+  __syncthreads();
+  for (int r = threadIdx.x; r < p.nq_sparse; r += kOrderThreads) atomicAdd(&start[sparse_row_tiles(p, bh, r, q_limit)], 1);
+  __syncthreads();
+  if (threadIdx.x == 0) {   // descending exclusive scan; O(nb_kv) against the kernel's O(nq * nb_kv)
+    int run = 0;
+    for (int c = p.nb_kv; c >= 0; --c) {
+      const int t = start[c];
+      start[c] = run;
+      run += t;
+    }
+  }
+  __syncthreads();
+  int* dst = order + static_cast<size_t>(gridDim.x) * p.nq_dense + static_cast<size_t>(bh) * p.nq_sparse;
+  for (int base = 0; base < p.nq_sparse; base += kOrderThreads) {
+    const int r = base + threadIdx.x;
+    const int c = r < p.nq_sparse ? sparse_row_tiles(p, bh, r, q_limit) : -1;
+    chunk[threadIdx.x] = c;
+    __syncthreads();
+    if (c >= 0) {
+      int rank = 0;   // rows of this chunk before r with the same count
+      for (int t = 0; t < static_cast<int>(threadIdx.x); ++t) rank += chunk[t] == c;
+      dst[start[c] + rank] = bh * per_bh + p.nq_dense + r;
+    }
+    __syncthreads();
+    if (c >= 0) atomicAdd(&start[c], 1);
+    __syncthreads();
+  }
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
@@ -557,7 +623,13 @@ static int make_bytes_map(CUtensorMap* map, const void* base, long long rows, in
 
 static bool stride_ok(long long s) { return s > 0 && (s * 2) % 16 == 0; }
 
-int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const JengaQkInt8Args* qk) {
+int64_t carved_attn_sched_workspace_bytes(long long batch, long long heads, long long nq_sparse, long long nq_dense) {
+  if (batch <= 0 || heads <= 0 || nq_sparse < 0 || nq_dense < 0) return 0;
+  return batch * heads * (nq_sparse + nq_dense) * static_cast<int64_t>(sizeof(int));
+}
+
+int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const JengaQkInt8Args* qk,
+                         const JengaAttnSched* sched) {
   if (!a || !a->q || !a->k || !a->v || (!a->out && a->sp_world <= 0)) return set_error(JENGA_E_INVALID, "null pointer");
   if (a->dtype != JENGA_BF16 && a->dtype != JENGA_F16)
     return set_error(JENGA_E_INVALID, "dtype must be bf16 or f16");
@@ -622,6 +694,17 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
       return set_error(JENGA_E_UNSUPPORTED, "fp8 P.V: needs v_fp8_amax and bf16 q/k");
     if (reinterpret_cast<uintptr_t>(a->v_fp8) % 16) return set_error(JENGA_E_INVALID, "v_fp8 must be 16-byte aligned");
   }
+  const long long grid = static_cast<long long>(a->batch) * a->heads * (a->nq_sparse + a->nq_dense);
+  if (grid > 0x7fffffffll) return set_error(JENGA_E_UNSUPPORTED, "grid too large");
+  if (sched) {
+    const int64_t need = carved_attn_sched_workspace_bytes(a->batch, a->heads, a->nq_sparse, a->nq_dense);
+    if (!sched->workspace) return set_error(JENGA_E_INVALID, "sched: null workspace");
+    if (reinterpret_cast<uintptr_t>(sched->workspace) % alignof(int))
+      return set_error(JENGA_E_INVALID, "sched: workspace must be 4-byte aligned");
+    if (sched->workspace_bytes < need)
+      return set_error(JENGA_E_WORKSPACE, "sched: workspace %lld < %lld bytes",
+                       static_cast<long long>(sched->workspace_bytes), static_cast<long long>(need));
+  }
   CUtensorMap tm_q, tm_k, tm_v;
   int rc;
   if (qk) {
@@ -679,14 +762,21 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
     p.k_groups = qk->kv_rows_padded / kBlock;
   }
 
-  const long long grid = static_cast<long long>(a->batch) * a->heads * (a->nq_sparse + a->nq_dense);
-  if (grid > 0x7fffffffll) return set_error(JENGA_E_UNSUPPORTED, "grid too large");
+  cudaError_t ce;
+  if (sched) {
+    p.order = static_cast<const int*>(sched->workspace);
+    const int bhs = a->batch * a->heads;
+    carved_attn_order_kernel<<<bhs, kOrderThreads, (p.nb_kv + 1 + kOrderThreads) * sizeof(int), stream>>>(
+        p, static_cast<int*>(sched->workspace));
+    ce = cudaGetLastError();
+    if (ce != cudaSuccess) return set_cuda_error(ce, "carved_attn order launch");
+  }
   const bool bf16 = a->dtype == JENGA_BF16;
   auto kern = qk ? (pv_fp8 ? carved_attn_fwd_kernel<true, true, true>
                            : (bf16 ? carved_attn_fwd_kernel<true, false, true> : carved_attn_fwd_kernel<false, false, true>))
                  : (pv_fp8 ? carved_attn_fwd_kernel<true, true>
                            : (bf16 ? carved_attn_fwd_kernel<true> : carved_attn_fwd_kernel<false>));
-  cudaError_t ce = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+  ce = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
   if (ce != cudaSuccess) return set_cuda_error(ce, "cudaFuncSetAttribute(carved_attn)");
   kern<<<static_cast<unsigned>(grid), kThreads, kSmemBytes, stream>>>(tm_q, tm_k, tm_v, p);
   ce = cudaGetLastError();

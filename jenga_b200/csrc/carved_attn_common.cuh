@@ -37,6 +37,8 @@ struct KernelParams {
   const float* k_scale;
   long long q_groups, k_groups;   // scales per (batch, head): q_rows_padded / 64, kv_rows_padded / 128
   int* err_flag;
+  // optional [grid] item of each CTA (carved_attn_order_kernel); NULL: CTA i runs item i
+  const int* order;
 };
 
 // Walks the set bits of the row mask in ascending key-block order.
