@@ -5,14 +5,16 @@
 // and its text-row flash_attn_func call (:371-380) with ONE launch.
 //
 // Work decomposition: one CTA per (batch*head, 128-row query block); 384 threads, three warpgroups:
-//   warpgroups 0, 1  consumers, 64 query rows each: S = Q~ K^T by wgmma (Q and K from shared
-//                    memory, S in registers), online softmax in base 2 on the registers, then
-//                    O += P V by wgmma with P as the register A operand; final O / l -> global
+//   warpgroups 0, 1  consumers, 64 query rows each: S = Q~ K^T by wgmma (Q~ in registers, loaded
+//                    once per CTA with ldmatrix; K from shared memory; S in registers), online
+//                    softmax in base 2 on the registers, then O += P V by wgmma with P as the
+//                    register A operand; final O / l -> global
 //   warpgroup 2      producer: warp 8 issues TMA — Q once, then one K tile and one V tile per live
 //                    key block into a two-stage ring (K and V slots are released separately);
 //                    with FP8 P.V, warps 9..11 transpose each V tile (see kPvFp8)
 // setmaxnreg moves registers from the producer (24, or 40 with the FP8 transpose) to the consumers
-// (240, or 232): S, O and the packed P of the previous tile are all live in a consumer at once.
+// (240, or 232): Q~, S, O and the packed P of the previous tile are all live in a consumer at once.
+// Keeping Q~ in registers takes a third of the shared-memory reads off Q.K^T: only K is read per tile.
 //
 // Consumer schedule (FlashAttention-3's):
 //   - in-warpgroup pipelining: iteration j issues S_j = Q~ K_j^T, then O += P_{j-1} V_{j-1}; it
@@ -53,7 +55,6 @@ constexpr int kStages = 2;                       // K/V ring depth
 constexpr int kBoxBytes = kBlock * 64 * 2;       // 16 KB: 128 rows x 64 d (one TMA box)
 constexpr int kTileBytes = 2 * kBoxBytes;        // 32 KB: 128 rows x 128 d (two d halves)
 constexpr int kMaxMaskWords = 256;               // up to 8192 key blocks (1M tokens)
-constexpr uint32_t kBarQScaled = 1;              // named barrier: Q~ written by both consumer warpgroups
 constexpr uint32_t kBarTurn = 3;                 // named barriers 3, 4: consumer warpgroup 0's, 1's turn
 
 // shared-memory carve-up (offsets from the 1024-aligned base)
@@ -90,7 +91,8 @@ __device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t col) {
 // kQkInt8 (opt-in, SageAttention's recipe): Q and K enter Q.K^T as int8 made by jenga_quantize_int8 —
 // Q per 64-row group (one scale per consumer warpgroup), K per 128-key block after subtracting its
 // per-head channel mean (a constant per score row: every softmax is unchanged) — through wgmma
-// m64n128k32 s8 x s8 -> s32 (half the Q.K^T tensor cycles).  Q and K tiles are one 16 KB box each.
+// m64n128k32 s8 x s8 -> s32 (half the Q.K^T tensor cycles).  Q and K tiles are one 16 KB box each;
+// Q stays in shared memory (the s32 accumulator already takes the registers Q would need).
 // The s32 scores become fp32 exactly (|S| < 2^22) and both classes scale them inside the exponent by
 // c = q_scale * k_scale[blk] * qk_scale, so the sparse class skips its Q~ pre-scaling.  text_amp,
 // the masks, the lazy rescale and P.V (bf16/f16, or e4m3 with kPvFp8) are unchanged.
@@ -256,24 +258,25 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
 
   if (n_tiles > 0) {
     mbar_wait(&bars[Q_FULL], 0, p.err_flag);
-    if (!dense && !kQkInt8) {
-      // ref :87-88  q = (q * qk_scale).to(dtype) — elementwise, so swizzle-agnostic
-      uint4* q4 = reinterpret_cast<uint4*>(sQ);
-#pragma unroll 4
-      for (int i = 0; i < kTileBytes / 16 / kConsumerThreads; ++i) {
-        uint4 v = q4[threadIdx.x + i * kConsumerThreads];
-        uint32_t* e = reinterpret_cast<uint32_t*>(&v);
+    const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128;   // kQkInt8: this warpgroup's 64 rows
+    // 16-bit Q: the warpgroup's 64 rows stay in registers as the A operand of all its Q.K^T wgmmas
+    // (16 k per step: matrices {rows 0-7, 8-15} x {k 0-7, 8-15} of the warp's 16 rows)
+    uint32_t qa[kQkInt8 ? 1 : 8][4];
+    if constexpr (!kQkInt8) {
+      const int q_row = wg * 64 + (warp & 3) * 16 + (lane & 7) + 8 * ((lane >> 3) & 1);
 #pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float2 f = unpack2<kBF16>(e[t]);
-          e[t] = pack2<kBF16>(f.x * p.qk_scale, f.y * p.qk_scale);
-        }
-        q4[threadIdx.x + i * kConsumerThreads] = v;
+      for (int kk = 0; kk < kHeadDim / 16; ++kk)
+        ldmatrix_x4(qa[kk], sQ + (kk >> 2) * kBoxBytes + sw128(q_row, (kk & 3) * 32 + (lane >> 4) * 16));
+      if (!dense) {   // ref :87-88  q = (q * qk_scale).to(dtype)
+#pragma unroll
+        for (int kk = 0; kk < kHeadDim / 16; ++kk)
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {
+            const float2 f = unpack2<kBF16>(qa[kk][t]);
+            qa[kk][t] = pack2<kBF16>(f.x * p.qk_scale, f.y * p.qk_scale);
+          }
       }
-      fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core proxy
-      named_bar_sync(kBarQScaled, kConsumerThreads);
     }
-    const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128;   // this warpgroup's 64 rows of each d half
 
     float sc[64];                      // S_j, then P_j in fp32
     int32_t si[kQkInt8 ? 64 : 1];      // kQkInt8: integer S_j while its wgmma runs
@@ -304,8 +307,7 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
 #pragma unroll
         for (int kk = 0; kk < kHeadDim / 16; ++kk) {
           const uint32_t off = (kk & 3) * 32 + (kk >> 2) * kBoxBytes;
-          wgmma_128_ss<kBF16>(sc, gmma_desc_sw128(q_addr + off, 16, 1024),
-                              gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
+          wgmma_128_rs<kBF16>(sc, qa[kk], gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
         }
       }
       wgmma_commit();

@@ -477,11 +477,6 @@ pooled_scores_kernel(const uint16_t* __restrict__ q_pool, const uint16_t* __rest
 // rounding points on the way out.  Legacy warp-level MMA on purpose: the whole problem is
 // 5 GFLOP (24 heads x 900 x 900 x 128) — a wgmma pipeline would cost more to set up than
 // the math takes.  64x64 outputs per CTA, 4 warps of 32x32.
-__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_ptr) {
-  const uint32_t a = static_cast<uint32_t>(__cvta_generic_to_shared(smem_ptr));
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
 template <int kDtype>
 __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   if constexpr (kDtype == JENGA_BF16) {

@@ -128,22 +128,17 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t
 // the 64 fp32 accumulator registers of an m64n128 wgmma: operands %0..%63
 #define JENGA_WGMMA_D64 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
 #define JENGA_WGMMA_OUT64 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-#define JENGA_WGMMA_SS(TY)                                                                              \
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                        \
-               "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " " JENGA_WGMMA_D64             \
-               ", %64, %65, p, 1, 1, 0, 0;\n\t}\n"                                                     \
-               : JENGA_WGMMA_OUT64 : "l"(a_desc), "l"(b_desc), "r"(scale_d))
 #define JENGA_WGMMA_RS(SHAPE, TY, TAIL)                                                                 \
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"                                        \
                "wgmma.mma_async.sync.aligned." SHAPE ".f32." TY "." TY " " JENGA_WGMMA_D64              \
                ", {%64, %65, %66, %67}, %68, p, 1, 1" TAIL ";\n\t}\n"                                  \
                : JENGA_WGMMA_OUT64 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d))
 
-// D[64x128 f32, registers] (+)= A[smem, K-major] * B[smem, K-major], K = 16 (16-bit operands)
+// D[64x128 f32, registers] (+)= A[registers] * B[smem, K-major], K = 16 (16-bit operands)
 template <bool kBF16>
-__device__ __forceinline__ void wgmma_128_ss(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
-  if constexpr (kBF16) JENGA_WGMMA_SS("bf16");
-  else JENGA_WGMMA_SS("f16");
+__device__ __forceinline__ void wgmma_128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  if constexpr (kBF16) JENGA_WGMMA_RS("m64n128k16", "bf16", ", 0");
+  else JENGA_WGMMA_RS("m64n128k16", "f16", ", 0");
 }
 // D[64x128 f32] (+)= A[registers] * B[smem, MN-major], K = 16 (16-bit operands)
 template <bool kBF16>
@@ -182,6 +177,13 @@ __device__ __forceinline__ uint32_t pack4_e4m3(float a, float b, float c, float 
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(b), "f"(a));
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
   return static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+}
+
+// four 8x8 b16 matrices from shared memory; lanes 8m..8m+7 give the row addresses of matrix m, and
+// register m of lane l holds elements (l / 4, 2 (l % 4) + {0, 1}) of matrix m
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_ptr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(smem_ptr)));
 }
 
 // sub-CTA barrier among `count` threads (ids 1..15; 0 is __syncthreads)
