@@ -127,7 +127,8 @@ typedef struct JengaAttnArgs {
    * text rows).  out_peers_host[r] (HOST array of sp_world device pointers, peer-mapped) is the
    * base of rank r's result buffer [sp_rows + dense rows, sp_heads_total, D]; each output row is
    * stored directly into its owner's buffer (image row t -> rank t / sp_rows; dense rows ->
-   * every rank), at heads [sp_rank*heads, (sp_rank+1)*heads).  `out` is ignored.  The caller
+   * every rank, sp_world == 1 included), at heads [sp_rank*heads, (sp_rank+1)*heads).  Every
+   * entry must be non-NULL and 16-byte aligned.  `out` is ignored and may be NULL.  The caller
    * synchronises the ranks before reading (jenga_b200.ulysses.UlyssesFusedAttention). */
   int32_t sp_world, sp_rank, sp_heads_total;
   int64_t sp_rows;
@@ -217,7 +218,7 @@ int64_t jenga_select_blocks_workspace_bytes(int32_t batch_heads, int32_t nq, int
  * buffer at [w, rank*n_loc + i, 0:heads/world, :] <- heads [p*heads/world, (p+1)*heads/world),
  * and the replicated text rows joint[w] into the LOCAL buffer at rows [world*n_loc, +n_text).
  * peer_qkv_host[p] (HOST array) = peer-mapped base of rank p's [3, world*n_loc + n_text,
- * heads/world, head_dim] buffer.  Element size 2 bytes.
+ * heads/world, head_dim] buffer; every entry non-NULL and 16-byte aligned.  Element size 2 bytes.
  * ---------------------------------------------------------------------------------------- */
 typedef struct JengaUlyssesScatterArgs {
   const void* x[3];

@@ -248,6 +248,9 @@ extern "C" int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* a, void* str
     return set_error(JENGA_E_INVALID, "ulysses_scatter: bad shape");
   if (a->n_text > 0 && (!a->joint[0] || !a->joint[1] || !a->joint[2]))
     return set_error(JENGA_E_INVALID, "ulysses_scatter: joint tensors missing");
+  for (int r = 0; r < a->world; ++r)
+    if (!a->peer_qkv_host[r] || a->peer_qkv_host[r] % 16)
+      return set_error(JENGA_E_INVALID, "ulysses_scatter: peer_qkv_host[%d] is null or not 16-byte aligned", r);
   ScatterParams p{};
   for (int w = 0; w < 3; ++w) {
     p.x[w] = static_cast<const uint4*>(a->x[w]);

@@ -506,6 +506,8 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
         obase = reinterpret_cast<uint16_t*>(p.peer_out[owner]);
         o_off = ((q_row - owner * p.sp_rows) * p.sp_heads_total + gh) * kHeadDim;
       } else {
+        // every rank's buffer; with one rank that is peer_out[0] through the single-store path
+        obase = reinterpret_cast<uint16_t*>(p.peer_out[0]);
         n_dst = p.sp_world;
         o_off = ((p.sp_rows + (q_row - n_img)) * p.sp_heads_total + gh) * kHeadDim;
       }
@@ -689,6 +691,9 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
       ((!a->sp_head_base_valid && a->sp_heads_total != a->heads * a->sp_world) || sp_head_base < 0 ||
        sp_head_base + a->heads > a->sp_heads_total))
     return set_error(JENGA_E_INVALID, "bad Ulysses head range");
+  for (int r = 0; r < a->sp_world; ++r)
+    if (!a->out_peers_host[r] || a->out_peers_host[r] % 16)
+      return set_error(JENGA_E_INVALID, "Ulysses out_peers_host[%d] is null or not 16-byte aligned", r);
 
   const bool pv_fp8 = a->v_fp8 != nullptr;
   if (pv_fp8) {

@@ -193,6 +193,62 @@ def test_fp8_and_head_group_arguments_of_the_attention_entry_point():
     assert lib.jenga_carved_attn_fwd(C.byref(a), None) == E_INVALID and "head range" in _err()
 
 
+def _peer_array(world, bad_rank, bad):
+    """Host array of `world` plausible device addresses; entry `bad_rank` is NULL or 8 bytes off."""
+    vals = [0x100000 * (r + 1) for r in range(world)]
+    if bad_rank is not None:
+        vals[bad_rank] = 0 if bad == "null" else vals[bad_rank] + 8
+    return (C.c_uint64 * world)(*vals)
+
+
+@pytest.mark.parametrize("world,bad_rank", [(1, 0), (2, 1), (8, 0), (8, 7)])
+@pytest.mark.parametrize("bad", ["null", "misaligned"])
+def test_ulysses_epilogue_rejects_bad_peer_entries(world, bad_rank, bad):
+    """Every out_peers_host[0..sp_world) entry is checked before any CUDA call, with a NULL `out`
+    as the fused Ulysses path passes it."""
+    peers = _peer_array(world, bad_rank, bad)
+    a = _attn_args(out=None, sp_world=world, sp_rank=world - 1, sp_heads_total=2 * world, sp_rows=128,
+                   out_peers_host=C.addressof(peers))
+    assert lib.jenga_carved_attn_fwd(C.byref(a), None) == E_INVALID, _err()
+    assert f"out_peers_host[{bad_rank}]" in _err(), _err()
+    sched = _lib.JengaAttnSched(0x20000, 1 << 20)
+    assert lib.jenga_carved_attn_fwd_sched(C.byref(a), None, C.byref(sched), None) == E_INVALID, _err()
+    assert f"out_peers_host[{bad_rank}]" in _err(), _err()
+
+
+@pytest.mark.parametrize("world,bad_rank", [(1, 0), (2, 1), (8, 0), (8, 7)])
+@pytest.mark.parametrize("bad", ["null", "misaligned"])
+def test_ulysses_scatter_rejects_bad_peer_entries(world, bad_rank, bad):
+    a = _lib.JengaUlyssesScatterArgs()
+    P = 0x10000
+    a.x = (C.c_void_p * 3)(P, P, P)
+    a.x_stride_s = 24 * 128
+    a.world, a.rank, a.heads, a.head_dim, a.n_loc, a.n_text = world, 0, 24, 128, 144, 0
+    peers = _peer_array(world, bad_rank, bad)
+    a.peer_qkv_host = C.addressof(peers)
+    assert lib.jenga_ulysses_scatter(C.byref(a), None) == E_INVALID, _err()
+    assert f"peer_qkv_host[{bad_rank}]" in _err(), _err()
+
+
+def test_good_peer_entries_pass_validation_without_a_device():
+    """Control for the two tests above: the same arguments with every entry good get past the
+    validation and fail only at the first CUDA call."""
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("GPU present: the addresses are not real allocations")
+    for world in (1, 8):
+        peers = _peer_array(world, None, None)
+        a = _attn_args(out=None, sp_world=world, sp_rank=0, sp_heads_total=2 * world, sp_rows=128,
+                       out_peers_host=C.addressof(peers))
+        assert lib.jenga_carved_attn_fwd(C.byref(a), None) == E_CUDA, _err()
+        s = _lib.JengaUlyssesScatterArgs()
+        s.x = (C.c_void_p * 3)(0x10000, 0x10000, 0x10000)
+        s.x_stride_s = 24 * 128
+        s.world, s.rank, s.heads, s.head_dim, s.n_loc, s.n_text = world, 0, 24, 128, 144, 0
+        s.peer_qkv_host = C.addressof(peers)
+        assert lib.jenga_ulysses_scatter(C.byref(s), None) == E_CUDA, _err()
+
+
 def test_scatter_head_group_validation():
     a = _lib.JengaUlyssesScatterArgs()
     P = 0x10000

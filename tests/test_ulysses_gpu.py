@@ -1,5 +1,7 @@
-"""2-GPU NCCL run of the Ulysses wrapper; skipped on boxes with one GPU (run with
-`gpurun --gpus 2`).  The SP result must equal the single-GPU operator bit for bit."""
+"""2-GPU NCCL run of the Ulysses wrapper; skipped on boxes with one GPU.  The SP result must equal
+the single-GPU operator bit for bit.  This is the only test whose peer stores cross NVLink; the
+fused exchange at world sizes 1-8, ragged per-rank slices, head sub-groups and HostPipelinedUlysses
+are covered on one GPU by tests/test_ulysses_emulated_gpu.py."""
 import os
 import subprocess
 import sys
