@@ -377,6 +377,31 @@ int jenga_gate_residual_tr(const void* x, int64_t x_stride, const void* y, int64
                            const void* tr_gate, const uint8_t* row_is_tr, void* out, int64_t out_stride,
                            int64_t rows, int32_t channels, void* stream);
 
+/* Wan2.1 forms (wan/modules/model_mul.py:303-346 WanAttentionBlock.forward under
+ * torch.autocast(bf16)).  The residual stream is fp32 after block 0; parameter vectors (scale, shift,
+ * gate, weight, bias) are fp32 [channels]; x is bf16 or fp32 (x_dtype JENGA_BF16 / JENGA_F32), y is
+ * bf16.  LN(v) = layer_norm(v) in fp32 without affine, rstd * (v - mean); every other step is one fp32
+ * rounding; bf16(.) is round-to-nearest-even.  Rows are `channels` contiguous elements, strides in
+ * elements (multiples of 8, >= channels), pointers 16-byte aligned, channels % 8 == 0 and <= 6144.
+ * Outputs never alias inputs.
+ * wan_ln_modulate:   n = LN(float(x)), rounded to bf16 when x is bf16 (WanLayerNorm's .type_as(x),
+ *                    :98-103); out = bf16( n * (1 + scale) + shift )                  (norm1, :331-333)
+ * wan_residual_ln:   r = x + y * gate (gate NULL: r = x + y), written to `res` as fp32; then
+ *                    affine != 0: out = bf16( fma(vec_a, LN(r), vec_b) )  weight / bias of norm3, the
+ *                                 form ATen's layer_norm kernel computes        (gate 1 + norm3, :334-339)
+ *                    affine == 0: out = bf16( LN(r) * (1 + vec_a) + vec_b )  scale / shift
+ *                                                                   (cross residual + norm2, :339-340)
+ * wan_gate_residual: out = x + y * gate, fp32                                    (gate 2, :341-342) */
+int jenga_wan_ln_modulate(const void* x, int32_t x_dtype, int64_t x_stride, const float* scale, const float* shift,
+                          void* out, int64_t out_stride, int64_t rows, int32_t channels, float eps, void* stream);
+int jenga_wan_residual_ln(const void* x, int32_t x_dtype, int64_t x_stride, const void* y, int64_t y_stride,
+                          const float* gate, float* res, int64_t res_stride, const float* vec_a, const float* vec_b,
+                          int32_t affine, void* out, int64_t out_stride, int64_t rows, int32_t channels, float eps,
+                          void* stream);
+int jenga_wan_gate_residual(const void* x, int32_t x_dtype, int64_t x_stride, const void* y, int64_t y_stride,
+                            const float* gate, float* out, int64_t out_stride, int64_t rows, int32_t channels,
+                            void* stream);
+
 /* (f-2) ProRes stage switch in one kernel: out = trilinear_up(latents + noise_pred*d_sigma) *
  * (1 - sigma_next) + noise * sigma_next, fp32, NCDHW contiguous.
  * ref: pipeline_hunyuan_video_prores.py:721-731; scheduling_flow_match_discrete.py:258-299.

@@ -177,6 +177,16 @@ def _load() -> C.CDLL:
     lib.jenga_gate_residual_tr.restype = C.c_int
     lib.jenga_gelu_tanh.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]
     lib.jenga_gelu_tanh.restype = C.c_int
+    lib.jenga_wan_ln_modulate.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]
+    lib.jenga_wan_ln_modulate.restype = C.c_int
+    lib.jenga_wan_residual_ln.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                          C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                          C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_void_p]
+    lib.jenga_wan_residual_ln.restype = C.c_int
+    lib.jenga_wan_gate_residual.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                            C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]
+    lib.jenga_wan_gate_residual.restype = C.c_int
     lib.jenga_prores_switch.argtypes = [C.c_void_p] * 4 + [C.c_int32] * 7 + [C.c_float, C.c_float, C.c_void_p]
     lib.jenga_prores_switch.restype = C.c_int
     lib.jenga_gilbert_mapping_device.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -10,6 +10,8 @@ reference module is executed,
   MMDoubleStreamBlock.forward / MMSingleStreamBlock.forward of HunyuanVideo-I2V
       (hyvideo_i2v/modules/models_mul.py:136-319, :393-505)
   WanSelfAttention.forward            (wan/modules/model_mul.py:134-180)
+  WanT2VCrossAttention.forward        (wan/modules/model_mul.py:183-205)
+  WanAttentionBlock.forward           (wan/modules/model_mul.py:303-346)
 
 with versions whose attention section is `jenga_hy_prologue` / `jenga_wan_prologue` (RMSNorm +
 RoPE + img||txt concatenation + block pooling in one pass over the QKV projection output)
@@ -25,6 +27,12 @@ token-replace modulation (rows of the first frame take the `tr_` shift / scale /
 reference does it with boolean-mask index_put, modulate_layers.py:51-56,84-95, here it is a per-row
 parameter select inside the ln_modulate / gate_residual kernels), a ragged S = L + 400 that the
 operator zero-pads to whole blocks, and the operator's default text_blocks=4.
+
+The Wan block forward runs its elementwise chains as the wan_* dense kernels (fp32 residual stream,
+one pass per chain, bf16 handed to the Linears as autocast would cast it) and leaves the Linears, the
+attention modules and the FFN to the block's own sub-modules.  Its T2V cross-attention runs the
+norm-only prologue and the dense class of the attention kernel, without flash_attention's segment
+table and host syncs.  WanI2VCrossAttention is left as it is.
 
 A second hook routes `x[:, long_index]` / `x[long_index]` on contiguous CUDA activations — the
 token reorder of jenga_hyvideo.py:116-118,226 and jenga_wan.py:559,655 — to `jenga_gather_rows`.
@@ -45,7 +53,7 @@ _HY_MODULES = ("hyvideo.modules.models_mul_block_gc_ha_multigpu",)
 _I2V_MODULES = ("hyvideo_i2v.modules.models_mul",)
 _WAN_MODULES = ("wan.modules.model_mul",)
 STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "wan_self": 0, "fallback": 0,
-         "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0}
+         "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0}
 # the HunyuanVideo-I2V operator's text_blocks default (hyvideo_i2v/…/attention_block_triton_diffres.py:409);
 # models_mul.py never passes text_blocks, so it holds whatever the text length
 _I2V_TEXT_BLOCKS = 4
@@ -365,6 +373,67 @@ def _make_wan_forward(orig, mod):
     return forward
 
 
+def _make_wan_cross_forward(orig, mod):
+    def forward(self, x, context, context_lens):
+        wq = getattr(self.norm_q, "weight", None)
+        wk = getattr(self.norm_k, "weight", None)
+        # context_lens: the reference's varlen form (wan/modules/attention.py:69-80); teacache_forward
+        # passes None (jenga_wan.py:569)
+        if (context_lens is not None or not x.is_cuda or x.dim() != 3 or x.shape[0] != 1 or context.dim() != 3
+                or context.shape[0] != 1 or self.head_dim != 128 or wq is None or wk is None
+                or type(self.norm_q).__name__ != "WanRMSNorm" or type(self.norm_k).__name__ != "WanRMSNorm"
+                or not DN._autocast_bf16()):
+            STATS["fallback"] += 1
+            return orig(self, x, context, context_lens)
+        q_lin, k_lin, v = self.q(x), self.k(context), self.v(context)
+        if (q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype not in (torch.bfloat16, torch.float32)
+                or v.dtype != torch.bfloat16):
+            STATS["fallback"] += 1
+            return orig(self, x, context, context_lens)
+        out = WAN.cross_attention(q_lin, k_lin, v.view(1, -1, self.num_heads, self.head_dim), wq, wk,
+                                  self.num_heads, eps=float(self.norm_q.eps))
+        STATS["wan_cross"] += 1
+        return self.o(out.flatten(2))
+    forward.__jenga_b200__ = True
+    forward.__wrapped__ = orig
+    return forward
+
+
+def _make_wan_block_forward(orig, mod):
+    def forward(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=0.0, freq_remap=None,
+                block_neighbor_list=None, p_remain_rates=0.0):
+        args = (x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate, freq_remap,
+                block_neighbor_list, p_remain_rates)
+        ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
+              and type(self.cross_attn).__name__ == "WanT2VCrossAttention"
+              and self.modulation.dtype == torch.float32)
+        if ok:
+            with torch.autocast("cuda", dtype=torch.float32):                      # :326-327
+                e6 = self.modulation + e
+            ok = (DN.wan_ln_modulate_supported(x, self.norm1, e6)
+                  and DN.wan_residual_ln_supported(x, self.norm3, e6, affine=True)
+                  and DN.wan_residual_ln_supported(x, self.norm2, e6, affine=False)
+                  and DN.wan_gate_residual_supported(x, e6))
+        if not ok:
+            # no autocast, batch > 1, cross_attn_norm=False (norm3 is Identity), I2V cross-attention, …
+            STATS["fallback"] += 1
+            return orig(self, *args)
+        e = e6.chunk(6, dim=1)
+        # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to
+        y = self.self_attn(DN.wan_ln_modulate(x, e[0], e[1], eps=self.norm1.eps), seq_lens, grid_sizes, freqs,
+                           sa_drop_rate=sa_drop_rate, freq_remap=freq_remap, block_neighbor_list=block_neighbor_list,
+                           p_remain_rates=p_remain_rates)                          # :331-333
+        x, h = DN.wan_residual_ln(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight,
+                                  bias=self.norm3.bias)                            # :334-335, :339
+        x, h = DN.wan_residual_ln(x, self.cross_attn(h, context, context_lens), None, eps=self.norm2.eps,
+                                  shift=e[3], scale=e[4])                          # :339-340
+        STATS["wan_block"] += 1
+        return DN.wan_gate_residual(x, self.ffn(h), e[5])                          # :340-342
+    forward.__jenga_b200__ = True
+    forward.__wrapped__ = orig
+    return forward
+
+
 def patch_module(mod) -> list[str]:
     """Patches the block classes of an already imported reference module; returns what it did."""
     done = []
@@ -384,8 +453,12 @@ def patch_module(mod) -> list[str]:
     if hasattr(mod, "WanSelfAttention") and not getattr(mod.WanSelfAttention.forward, "__jenga_b200__", False):
         orig = mod.WanSelfAttention.forward
         mod.WanSelfAttention.forward = _make_wan_forward(orig, mod)
-        # WanT2VCrossAttention / WanI2VCrossAttention override forward themselves: untouched
         done.append(f"{name}.WanSelfAttention.forward")
+    # WanI2VCrossAttention overrides forward itself and is left as it is
+    for cls, make in (("WanT2VCrossAttention", _make_wan_cross_forward), ("WanAttentionBlock", _make_wan_block_forward)):
+        if hasattr(mod, cls) and not getattr(getattr(mod, cls).forward, "__jenga_b200__", False):
+            getattr(mod, cls).forward = make(getattr(mod, cls).forward, mod)
+            done.append(f"{name}.{cls}.forward")
     return done
 
 

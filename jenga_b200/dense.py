@@ -7,13 +7,18 @@ callers (jenga_b200/blocks.py) fall back to the reference's own ops for anything
 
 `ln_modulate` and `gate_residual` also take the token-replace form of HunyuanVideo-I2V
 (hyvideo_i2v/modules/modulate_layers.py:51-56,84-95): `tr=(tr_shift, tr_scale, row_mask)` /
-`tr=(tr_gate, row_mask)`, where rows whose mask entry is true take the tr_ parameters."""
+`tr=(tr_gate, row_mask)`, where rows whose mask entry is true take the tr_ parameters.
+
+The `wan_*` functions are the chains of Wan2.1's WanAttentionBlock.forward
+(wan/modules/model_mul.py:326-346), whose residual stream is fp32 and whose modulation vectors are
+the fp32 rows of `e` [1, 6, C]."""
 from __future__ import annotations
 
 import weakref
 
 import torch
 
+from . import _lib
 from ._lib import check, lib
 from .attention import _require_cuda, _stream_ptr
 
@@ -156,4 +161,123 @@ def gelu_tanh_into(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     with torch.cuda.device(x.device):
         check(lib.jenga_gelu_tanh(x.data_ptr(), xs, out.data_ptr(), os_, rows, x.shape[-1], _stream_ptr(x.device)),
               "gelu_tanh")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Wan2.1 (wan/modules/model_mul.py:303-346)
+# ------------------------------------------------------------------------------------------------
+def _autocast_bf16() -> bool:
+    return torch.is_autocast_enabled() and torch.get_autocast_dtype("cuda") == torch.bfloat16
+
+
+def _wan_rows_ok(x: torch.Tensor, e: torch.Tensor) -> bool:
+    """x [1, L, C] bf16 or fp32 on a GPU with 8-aligned rows, e the fp32 [1, 6, C] modulation sum"""
+    return (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype in (torch.bfloat16, torch.float32)
+            and x.dim() == 3 and x.shape[0] == 1 and x.shape[-1] % 8 == 0 and x.shape[-1] <= 6144
+            and x.stride(-1) == 1 and x.stride(-2) % 8 == 0
+            and isinstance(e, torch.Tensor) and e.is_cuda and e.dtype == torch.float32
+            and tuple(e.shape) == (1, 6, x.shape[-1]) and _autocast_bf16())
+
+
+def _wan_layer_norm(norm, affine: bool) -> bool:
+    """WanLayerNorm (model_mul.py:93-103), with fp32 weight and bias when `affine`"""
+    if type(norm).__name__ != "WanLayerNorm" or not isinstance(norm, torch.nn.LayerNorm):
+        return False
+    if not affine:
+        return norm.weight is None and norm.bias is None
+    return (norm.weight is not None and norm.bias is not None and norm.weight.dtype == torch.float32
+            and norm.bias.dtype == torch.float32)
+
+
+def wan_ln_modulate_supported(x: torch.Tensor, norm: torch.nn.Module, e: torch.Tensor) -> bool:
+    """norm1 + modulate of a Wan block: x the block input (bf16 in block 0, fp32 after)"""
+    return _wan_rows_ok(x, e) and _wan_layer_norm(norm, affine=False)
+
+
+def wan_residual_ln_supported(x: torch.Tensor, norm: torch.nn.Module, e: torch.Tensor, affine: bool) -> bool:
+    """gate 1 + norm3 (affine) or cross residual + norm2 (not affine) of a Wan block"""
+    return _wan_rows_ok(x, e) and _wan_layer_norm(norm, affine=affine)
+
+
+def wan_gate_residual_supported(x: torch.Tensor, e: torch.Tensor) -> bool:
+    """gate 2 of a Wan block"""
+    return _wan_rows_ok(x, e)
+
+
+def _wan_vec(v: torch.Tensor, C: int, what: str) -> torch.Tensor:
+    _require_cuda(v)
+    if v.dtype != torch.float32:
+        raise ValueError(f"{what} must be fp32")
+    return _per_channel(v, C, what)
+
+
+def _wan_y(x: torch.Tensor, y: torch.Tensor):
+    _require_cuda(y)
+    if y.dtype != torch.bfloat16 or y.shape != x.shape:
+        raise ValueError("y must be a bf16 tensor shaped like x")
+    return _rows2d(y)[1]
+
+
+def _x_code(x: torch.Tensor) -> int:
+    codes = {torch.bfloat16: _lib.JENGA_BF16, torch.float32: _lib.JENGA_F32}
+    if x.dtype not in codes:
+        raise ValueError("x must be bf16 or fp32")
+    return codes[x.dtype]
+
+
+def wan_ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6) -> torch.Tensor:
+    """`norm1(x).float() * (1 + scale) + shift` (model_mul.py:331-333, WanLayerNorm :98-103) followed by
+    the bf16 cast the q / k / v Linears apply under autocast.  x [1, L, C] bf16 or fp32, shift / scale
+    fp32 with C values (e[0] / e[1]) -> [1, L, C] bf16."""
+    _require_cuda(x)
+    rows, xs = _rows2d(x)
+    C = x.shape[-1]
+    sc, sh = _wan_vec(scale, C, "scale"), _wan_vec(shift, C, "shift")
+    out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.jenga_wan_ln_modulate(x.data_ptr(), _x_code(x), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(),
+                                        C, rows, C, float(eps), _stream_ptr(x.device)), "wan_ln_modulate")
+    return out
+
+
+def wan_residual_ln(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor | None, eps: float = 1e-6, *,
+                    weight: torch.Tensor | None = None, bias: torch.Tensor | None = None,
+                    shift: torch.Tensor | None = None, scale: torch.Tensor | None = None):
+    """r = x + y * gate (gate None: x + y), then the next LayerNorm of r as the following Linear sees it.
+    weight / bias: `norm3(r)`, the affine WanLayerNorm (gate 1 + norm3, model_mul.py:334-339).
+    shift / scale: `norm2(r).float() * (1 + scale) + shift` (cross residual + norm2, :339-340).
+    x [1, L, C] bf16 or fp32, y bf16 like x -> (r fp32 [1, L, C], normed bf16 [1, L, C])."""
+    _require_cuda(x)
+    rows, xs = _rows2d(x)
+    ys = _wan_y(x, y)
+    C = x.shape[-1]
+    affine = weight is not None
+    if affine == (scale is not None) or (bias is None) != (weight is None) or (shift is None) != (scale is None):
+        raise ValueError("pass either weight and bias or shift and scale")
+    va = _wan_vec(weight if affine else scale, C, "weight" if affine else "scale")
+    vb = _wan_vec(bias if affine else shift, C, "bias" if affine else "shift")
+    g = _wan_vec(gate, C, "gate") if gate is not None else None
+    res = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.jenga_wan_residual_ln(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys,
+                                        g.data_ptr() if g is not None else None, res.data_ptr(), C, va.data_ptr(),
+                                        vb.data_ptr(), int(affine), out.data_ptr(), C, rows, C, float(eps),
+                                        _stream_ptr(x.device)), "wan_residual_ln")
+    return res, out
+
+
+def wan_gate_residual(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
+    """`x + y * gate` under autocast(float32) (gate 2, model_mul.py:341-342): x [1, L, C] bf16 or fp32,
+    y bf16 like x, gate fp32 with C values (e[5]) -> fp32 [1, L, C]."""
+    _require_cuda(x)
+    rows, xs = _rows2d(x)
+    ys = _wan_y(x, y)
+    C = x.shape[-1]
+    g = _wan_vec(gate, C, "gate")
+    out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.jenga_wan_gate_residual(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys, g.data_ptr(), out.data_ptr(),
+                                          C, rows, C, _stream_ptr(x.device)), "wan_gate_residual")
     return out

@@ -1,5 +1,6 @@
-"""Wan2.1-side glue of the hot path (wan/modules/model_mul.py:134-180 WanSelfAttention.forward):
-fused WanRMSNorm + RoPE prologue, the block-count rules and the operator call."""
+"""Wan2.1-side glue of the hot path (wan/modules/model_mul.py:134-180 WanSelfAttention.forward,
+:183-205 WanT2VCrossAttention.forward): fused WanRMSNorm + RoPE prologue, the block-count rules, the
+operator call and the dense text cross-attention."""
 from __future__ import annotations
 
 import ctypes as C
@@ -9,7 +10,7 @@ import torch
 
 from . import _lib
 from ._lib import check, lib
-from .attention import _require_cuda, _stream_ptr, block_sparse_attention_variant
+from .attention import BLOCK, _launch, _require_cuda, _stream_ptr, block_sparse_attention_variant
 
 
 def rope_freqs(head_dim: int = 128, max_len: int = 1024, theta: float = 10000.0) -> torch.Tensor:
@@ -44,10 +45,11 @@ def _device_freqs(freqs: torch.Tensor, dev) -> torch.Tensor:
     return fr
 
 
-def norm_rope(x: torch.Tensor, weight: torch.Tensor | None, heads: int, grid_size, freqs: torch.Tensor,
+def norm_rope(x: torch.Tensor, weight: torch.Tensor | None, heads: int, grid_size, freqs: torch.Tensor | None,
               freq_remap: torch.Tensor | None = None, eps: float = 1e-6) -> torch.Tensor:
     """rope_apply(norm(x).view(b, s, n, d), grid_sizes, freqs, freq_remap) as the carved
-    attention consumes it: [B, L, H, 128] bf16.  x: [B, L, H*128] bf16 or fp32."""
+    attention consumes it: [B, L, H, 128] bf16.  x: [B, L, H*128] bf16 or fp32.
+    freqs=None: the norm alone, `bf16(norm(x))` with no rotation (grid_size and freq_remap unused)."""
     _require_cuda(x)
     B, L, Cc = x.shape
     if Cc != heads * 128 or x.stride(2) != 1:
@@ -69,9 +71,14 @@ def norm_rope(x: torch.Tensor, weight: torch.Tensor | None, heads: int, grid_siz
         a.w, a.w_dtype = None, _lib.JENGA_F32
     a.batch, a.heads, a.head_dim, a.tokens = B, heads, 128, L
     a.stride_b, a.stride_s, a.eps = x.stride(0), x.stride(1), eps
-    fr = _device_freqs(freqs, dev)
-    a.freqs, a.freq_rows = fr.data_ptr(), fr.shape[0]
-    a.grid_f, a.grid_h, a.grid_w = (int(v) for v in grid_size)
+    if freqs is None:
+        a.freqs, a.freq_rows = None, 0
+        a.grid_f = a.grid_h = a.grid_w = 0
+        freq_remap = None
+    else:
+        fr = _device_freqs(freqs, dev)
+        a.freqs, a.freq_rows = fr.data_ptr(), fr.shape[0]
+        a.grid_f, a.grid_h, a.grid_w = (int(v) for v in grid_size)
     if freq_remap is not None:
         freq_remap = freq_remap.to(device=dev, dtype=torch.int64).contiguous()
         a.freq_remap = freq_remap.data_ptr()
@@ -94,3 +101,24 @@ def self_attention(q_lin, k_lin, v, norm_q_w, norm_k_w, heads, grid_size, freqs,
                                           block_neighbor_list=block_neighbor_list,
                                           p_remain_rates=p_remain_rates, first_frame_blocks=ff,
                                           shape_xfuse=True)
+
+
+def cross_attention(q_lin, k_lin, v, norm_q_w, norm_k_w, heads, eps=1e-6):
+    """WanT2VCrossAttention.forward's attention part (model_mul.py:195-200) for one sample with every
+    context row valid (context_lens=None): q_lin [1, L, C] = self.q(x), k_lin [1, Lc, C] = self.k(context),
+    v [1, Lc, H, 128] = self.v(context) bf16.  Returns [1, L, H, 128] bf16.
+
+    q and k go through the norm-only prologue, `bf16(bf16(norm(x)) * w)` — what flash_attention's
+    half() makes of norm_q(self.q(x)) (wan/modules/attention.py:59-83) — and the dense class of the
+    attention kernel runs over all Lc keys with softmax_scale D^-1/2.  flash_attention returns the
+    result as fp32 (`x.type(out_dtype)`, :130), which self.o casts straight back to bf16 under
+    autocast: the bf16 result here is what self.o sees.  No segment table, no host sync."""
+    q = norm_rope(q_lin, norm_q_w, heads, None, None, eps=eps)
+    k = norm_rope(k_lin, norm_k_w, heads, None, None, eps=eps)
+    if v.dtype != torch.bfloat16 or v.shape != k.shape or v.stride(3) != 1:
+        raise ValueError("v must be bf16 [1, Lc, heads, 128] with contiguous channels")
+    _, L, _, D = q.shape
+    Lc = k.shape[1]
+    out = torch.empty_like(q)
+    _launch(q, k, v, None, 0, (L + BLOCK - 1) // BLOCK, D ** -0.5, 0.0, 1 << 30, Lc, L, Lc, out, None, torch.bfloat16)
+    return out
