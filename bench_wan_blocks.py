@@ -1,22 +1,26 @@
 #!/usr/bin/env python
-"""Wan2.1 DiT block stack on one GPU: unmodified wan/modules/model_mul.py WanAttentionBlocks (T2V
-cross-attention, cross_attn_norm=True, random init, fp32 parameters, bf16 autocast as jenga_wan.py
+"""Wan2.1 DiT block stack on one GPU: unmodified wan/modules/model_mul.py WanAttentionBlocks (T2V or
+I2V cross-attention, cross_attn_norm=True, random init, fp32 parameters, bf16 autocast as jenga_wan.py
 runs them) timed three ways on the same weights and inputs:
 
   A  the reference operator (Triton + FlashAttention-2), if both import
-  B  the original WanAttentionBlock and WanT2VCrossAttention forwards on the jenga_b200 operator
-     (WanSelfAttention patched): what `python -m jenga_b200.install jenga_wan.py` ran before the
-     fused Wan forwards existed
+  B  the original WanAttentionBlock and WanT2VCrossAttention / WanI2VCrossAttention forwards on the
+     jenga_b200 operator (WanSelfAttention patched): what `python -m jenga_b200.install jenga_wan.py`
+     ran before the fused Wan forwards existed
   C  the fused forwards that install() patches in (jenga_b200/blocks.py)
 
 Block 0 receives a bf16 x (patch_embedding runs under bf16 autocast) and returns the fp32 residual
 stream the following blocks carry.  Default shape: Wan-14B (scripts/wan_14B_jenga_base.sh), grid
 21x45x80, dim 5120, 40 heads, ffn 13824, 512 context tokens, sa_drop_rate 0.7, p_remain_rates 0.8,
 4 blocks.  --model 1.3b: grid 21x30x52, dim 1536, 12 heads, ffn 8960, 0.75 / 0.9, 8 blocks.
+--model i2v-14b (jenga_wan.py --task i2v-14B): the 14B shape with "i2v_cross_attn" blocks, the context
+cat(fp32 [1, 257, C] CLIP tokens, bf16 [1, 512, C] text) = fp32 as jenga_wan.py:577-579 builds it,
+sa_drop_rate 0.0 (the I2V path never passes one), 4 blocks; it also times the I2V cross-attention
+kernel alone at L = 75 600, H = 40 against the two dense launches + fp32 add + bf16 cast it replaces.
 Legs alternate after a warm-up; CUDA events time each stack.  One JSON line on stdout; nothing is
 written to the tree.
 
-    python bench_wan_blocks.py [--model 14b|1.3b] [--blocks N] [--reps 3]
+    python bench_wan_blocks.py [--model 14b|1.3b|i2v-14b] [--blocks N] [--reps 3]
 """
 from __future__ import annotations
 
@@ -37,10 +41,12 @@ MODELS = {
     # grid, dim, heads, ffn, sa_drop_rate, p_remain_rates, blocks
     "14b": ((21, 45, 80), 5120, 40, 13824, 0.7, 0.8, 4),
     "1.3b": ((21, 30, 52), 1536, 12, 8960, 0.75, 0.9, 8),
+    "i2v-14b": ((21, 45, 80), 5120, 40, 13824, 0.0, 0.8, 4),
 }
+I2V_IMG_TOKENS = 257
 
 
-def modelled_bytes(L: int, C: int) -> dict:
+def modelled_bytes(L: int, C: int, i2v: bool = False) -> dict:
     """HBM bytes per block of the elementwise chains around the Linears and attentions, eager (one
     read and one write per ATen kernel, L2 ignored) and fused, from the activation shape alone"""
     lc = L * C
@@ -54,15 +60,70 @@ def modelled_bytes(L: int, C: int) -> dict:
         # q: .float() 2+4, pow 4+4, mean 4, * rsqrt 4+4, type_as 4+2, * w 2+4, half() 4+2,
         # fp32 output 2+4, cast at o 4+2 -> prologue read 2, write 2
         "cross_q_rmsnorm": (56, 4),
+        # I2V instead of cross_q_rmsnorm: q as above up to the first half() (44), a second half() 4+2, two
+        # fp32 outputs 2 x (2+4), x + img_x 4+4+4, cast at o 4+2 -> prologue read 2, write 2
+        "i2v_cross": (80, 4),
         # x + y 4+2+4, layer_norm 4+4, * (1+e) 4+4, + e 4+4, cast at ffn 4+2 -> read 4+2, write 4+2
         "cross_residual_norm2": (40, 12),
         # y*e 2+4, x + . 4+4+4 -> read 4+2, write 4
         "gate2": (18, 10),
     }
+    chains.pop("cross_q_rmsnorm" if i2v else "i2v_cross")
     out = {k: {"eager_gb": e * lc / 1e9, "fused_gb": f * lc / 1e9} for k, (e, f) in chains.items()}
     out["total"] = {"eager_gb": sum(e for e, _ in chains.values()) * lc / 1e9,
                     "fused_gb": sum(f for _, f in chains.values()) * lc / 1e9}
     return out
+
+
+def i2v_cross_kernel(dev, L: int, H: int, Li: int, Lt: int, launches: int = 20, rounds: int = 3) -> dict:
+    """jenga_wan_i2v_cross_attn alone against the composition it replaces — two dense-class launches of
+    the attention kernel (as wan.cross_attention issues them), an fp32 add and the bf16 cast — on the same
+    seeded bf16 inputs.  The two alternate, `launches` back-to-back calls per CUDA-event window; the best
+    window of `rounds` is reported per call."""
+    from jenga_b200 import wan
+    from jenga_b200.attention import BLOCK, _launch
+    g = torch.Generator(device=dev).manual_seed(7)
+    r = lambda n: torch.randn(1, n, H, 128, generator=g, device=dev).bfloat16()  # noqa: E731
+    q, ki, vi, kt, vt = r(L), r(Li), r(Li), r(Lt), r(Lt)
+    nq = (L + BLOCK - 1) // BLOCK
+    out = torch.empty_like(q)
+    a_img, a_txt = torch.empty_like(q), torch.empty_like(q)
+
+    def fused():
+        return wan.i2v_cross_attn(q, ki, vi, kt, vt, out=out)
+
+    def composed():
+        for k, v, o in ((ki, vi, a_img), (kt, vt, a_txt)):
+            _launch(q, k, v, None, 0, nq, 128 ** -0.5, 0.0, 1 << 30, k.shape[1], L, k.shape[1], o, None,
+                    torch.bfloat16)
+        return (a_txt.float() + a_img.float()).bfloat16()
+
+    def window(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(launches):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / launches
+
+    got, want = fused().clone(), composed()
+    torch.cuda.synchronize()
+    ms = {"fused": [], "composed": []}
+    for _ in range(rounds):
+        ms["fused"].append(window(fused))
+        ms["composed"].append(window(composed))
+    flop = 4.0 * L * H * 128 * (Li + Lt)          # Q K^T and P V over both segments
+    best = {k: min(v) for k, v in ms.items()}
+    d = (got.float() - want.float()).abs()
+    return {
+        "L": L, "heads": H, "img_keys": Li, "txt_keys": Lt, "launches_per_window": launches,
+        "ms_per_call": best, "ms_all": ms, "composed_over_fused": best["composed"] / best["fused"],
+        "algorithmic_tflop_per_call": flop / 1e12,
+        "tflops": {k: flop / (v * 1e-3) / 1e12 for k, v in best.items()},
+        "bit_identical": bool(torch.equal(got, want)), "max_abs_diff": d.max().item(),
+        "elements_differing": int((d > 0).sum().item()),
+    }
 
 
 def main(argv=None):
@@ -78,6 +139,7 @@ def main(argv=None):
         raise SystemExit("oracle/_ref/ is not staged: run __graft_entry__.build() first")
     (f, h, w), dim, heads, ffn, drop, p_remain, n_blocks = MODELS[args.model]
     n_blocks = args.blocks or n_blocks
+    i2v = args.model.startswith("i2v")
     Lc = 512
     dev = torch.device("cuda")
 
@@ -106,8 +168,10 @@ def main(argv=None):
                 else:
                     p_.copy_(torch.randn(p_.shape, generator=g, device=dev).mul_(0.02))
 
+    cross_type = "i2v_cross_attn" if i2v else "t2v_cross_attn"
+
     def stack(mod, meta=False):
-        mk = lambda: mod.WanAttentionBlock("t2v_cross_attn", dim, ffn, heads, (-1, -1), True, True, 1e-6)  # noqa: E731
+        mk = lambda: mod.WanAttentionBlock(cross_type, dim, ffn, heads, (-1, -1), True, True, 1e-6)  # noqa: E731
         if meta:
             with torch.device("meta"):
                 return [mk() for _ in range(n_blocks)]
@@ -134,6 +198,9 @@ def main(argv=None):
     x0 = torch.randn(1, L, dim, generator=g, device=dev).bfloat16()
     e0 = 0.1 * torch.randn(1, 6, dim, generator=g, device=dev)
     ctx = torch.randn(1, Lc, dim, generator=g, device=dev).bfloat16()
+    if i2v:
+        # img_emb's final LayerNorm runs in fp32 (model_mul.py:379-391); the concat promotes the text
+        ctx = torch.concat([torch.randn(1, I2V_IMG_TOKENS, dim, generator=g, device=dev), ctx], dim=1)
     kw = dict(sa_drop_rate=drop, freq_remap=h2l.to(dev), block_neighbor_list=nbr, p_remain_rates=p_remain)
 
     def forward(blks):
@@ -204,10 +271,13 @@ def main(argv=None):
         "C_vs_B": err(outs["B"], outs["C"]),
         "C_vs_A": err(outs["A"], outs["C"]) if "A" in outs else None,
         "B_vs_A": err(outs["A"], outs["B"]) if "A" in outs else None,
-        "modelled_bytes_per_block": modelled_bytes(L, dim),
+        "modelled_bytes_per_block": modelled_bytes(L, dim, i2v=i2v),
         "reference_leg": "ran" if ref is not None else f"unavailable ({ref_err})",
         "card": info, "card_after": info_after,
     }
+    if i2v:
+        res["context_tokens"] = I2V_IMG_TOKENS + Lc
+        res["i2v_cross_kernel"] = i2v_cross_kernel(dev, L, heads, I2V_IMG_TOKENS, Lc)
     print(json.dumps(res))
 
 

@@ -402,6 +402,36 @@ int jenga_wan_gate_residual(const void* x, int32_t x_dtype, int64_t x_stride, co
                             const float* gate, float* out, int64_t out_stride, int64_t rows, int32_t channels,
                             void* stream);
 
+/* Wan2.1-I2V cross-attention in one launch (wan/modules/model_mul.py:223-249 WanI2VCrossAttention.forward,
+ * the part between the norms and self.o, under bf16 autocast):
+ *   out[b,r,h,:] = bf16( f32(A_img) + f32(A_txt) ),  A_seg = bf16( softmax(q k_seg^T sm_scale) v_seg )
+ * Each segment is normalised by its own softmax sum with the arithmetic of the dense class of
+ * jenga_carved_attn_fwd, so A_img and A_txt are bit for bit what a dense launch over that segment alone
+ * returns.  q / out are [B, q_rows, H, 128], k_img / v_img [B, img_rows, H, 128], k_txt / v_txt
+ * [B, txt_rows, H, 128]; all bf16 with head_dim contiguous and element strides (b, s, h) that are
+ * positive multiples of 8; pointers 16-byte aligned; img_rows, txt_rows >= 1.  Rows >= q_rows are not
+ * stored. */
+typedef struct JengaWanCrossArgs {
+  const void* q;
+  const void* k_img;
+  const void* v_img;
+  const void* k_txt;
+  const void* v_txt;
+  void* out;
+  int32_t dtype; /* JENGA_BF16 */
+  int32_t batch, heads, head_dim;
+  int64_t q_rows, img_rows, txt_rows;
+  int64_t q_stride_b, q_stride_s, q_stride_h;
+  int64_t ki_stride_b, ki_stride_s, ki_stride_h;
+  int64_t vi_stride_b, vi_stride_s, vi_stride_h;
+  int64_t kt_stride_b, kt_stride_s, kt_stride_h;
+  int64_t vt_stride_b, vt_stride_s, vt_stride_h;
+  int64_t o_stride_b, o_stride_s, o_stride_h;
+  float sm_scale;
+  int32_t* err_flag; /* device int, may be NULL: set non-zero by in-kernel watchdogs */
+} JengaWanCrossArgs;
+int jenga_wan_i2v_cross_attn(const JengaWanCrossArgs* args, void* stream);
+
 /* (f-2) ProRes stage switch in one kernel: out = trilinear_up(latents + noise_pred*d_sigma) *
  * (1 - sigma_next) + noise * sigma_next, fp32, NCDHW contiguous.
  * ref: pipeline_hunyuan_video_prores.py:721-731; scheduling_flow_match_discrete.py:258-299.

@@ -103,6 +103,22 @@ class JengaWanPrologueArgs(C.Structure):
     ]
 
 
+class JengaWanCrossArgs(C.Structure):
+    _fields_ = [
+        ("q", C.c_void_p), ("k_img", C.c_void_p), ("v_img", C.c_void_p), ("k_txt", C.c_void_p),
+        ("v_txt", C.c_void_p), ("out", C.c_void_p),
+        ("dtype", C.c_int32), ("batch", C.c_int32), ("heads", C.c_int32), ("head_dim", C.c_int32),
+        ("q_rows", C.c_int64), ("img_rows", C.c_int64), ("txt_rows", C.c_int64),
+        ("q_stride_b", C.c_int64), ("q_stride_s", C.c_int64), ("q_stride_h", C.c_int64),
+        ("ki_stride_b", C.c_int64), ("ki_stride_s", C.c_int64), ("ki_stride_h", C.c_int64),
+        ("vi_stride_b", C.c_int64), ("vi_stride_s", C.c_int64), ("vi_stride_h", C.c_int64),
+        ("kt_stride_b", C.c_int64), ("kt_stride_s", C.c_int64), ("kt_stride_h", C.c_int64),
+        ("vt_stride_b", C.c_int64), ("vt_stride_s", C.c_int64), ("vt_stride_h", C.c_int64),
+        ("o_stride_b", C.c_int64), ("o_stride_s", C.c_int64), ("o_stride_h", C.c_int64),
+        ("sm_scale", C.c_float), ("err_flag", C.c_void_p),
+    ]
+
+
 class JengaTeaCacheArgs(C.Structure):
     _fields_ = [
         ("cur", C.c_void_p), ("prev", C.c_void_p), ("dtype", C.c_int32), ("n", C.c_int64),
@@ -208,6 +224,8 @@ def _load() -> C.CDLL:
     lib.jenga_carved_attn_fwd_sched.restype = C.c_int
     lib.jenga_carved_attn_sched_workspace_bytes.argtypes = [C.c_int32] * 4
     lib.jenga_carved_attn_sched_workspace_bytes.restype = C.c_int64
+    lib.jenga_wan_i2v_cross_attn.argtypes = [C.POINTER(JengaWanCrossArgs), C.c_void_p]
+    lib.jenga_wan_i2v_cross_attn.restype = C.c_int
     lib.jenga_gilbert_xyz2d.argtypes = [C.c_int] * 6
     lib.jenga_gilbert_xyz2d.restype = C.c_int64
     if lib.jenga_abi_version() != 3:

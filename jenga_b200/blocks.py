@@ -32,7 +32,10 @@ The Wan block forward runs its elementwise chains as the wan_* dense kernels (fp
 one pass per chain, bf16 handed to the Linears as autocast would cast it) and leaves the Linears, the
 attention modules and the FFN to the block's own sub-modules.  Its T2V cross-attention runs the
 norm-only prologue and the dense class of the attention kernel, without flash_attention's segment
-table and host syncs.  WanI2VCrossAttention is left as it is.
+table and host syncs.  Its I2V cross-attention (WanI2VCrossAttention, model_mul.py:223-249) runs the
+module's own Linears around the norm-only prologue and ONE jenga_wan_i2v_cross_attn launch that
+attends the 257 image and the text keys and adds the two results as the reference does; the block
+calls it directly, and WanI2VCrossAttention.forward itself is left as it is.
 
 A second hook routes `x[:, long_index]` / `x[long_index]` on contiguous CUDA activations — the
 token reorder of jenga_hyvideo.py:116-118,226 and jenga_wan.py:559,655 — to `jenga_gather_rows`.
@@ -53,7 +56,10 @@ _HY_MODULES = ("hyvideo.modules.models_mul_block_gc_ha_multigpu",)
 _I2V_MODULES = ("hyvideo_i2v.modules.models_mul",)
 _WAN_MODULES = ("wan.modules.model_mul",)
 STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "wan_self": 0, "fallback": 0,
-         "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0}
+         "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0,
+         "wan_i2v_cross": 0}
+# the CLIP image tokens at the head of the Wan2.1-I2V context (model_mul.py:230-231)
+_WAN_I2V_IMG_TOKENS = 257
 # the HunyuanVideo-I2V operator's text_blocks default (hyvideo_i2v/…/attention_block_triton_diffres.py:409);
 # models_mul.py never passes text_blocks, so it holds whatever the text length
 _I2V_TEXT_BLOCKS = 4
@@ -399,13 +405,53 @@ def _make_wan_cross_forward(orig, mod):
     return forward
 
 
+def _wan_i2v_cross_shape_ok(ca, x, context, context_lens):
+    """the I2V cross-attention configuration the fused kernel takes, device and autocast aside: one
+    sample, every context row valid (teacache_forward passes context_lens=None, jenga_wan.py:569),
+    head_dim 128, WanRMSNorm q / k / k_img norms with weights and one eps, and text rows after the
+    image rows"""
+    norms = [getattr(ca, n, None) for n in ("norm_q", "norm_k", "norm_k_img")]
+    return (context_lens is None and isinstance(x, torch.Tensor) and isinstance(context, torch.Tensor)
+            and x.dim() == 3 and x.shape[0] == 1 and context.dim() == 3 and context.shape[0] == 1
+            and context.shape[1] > _WAN_I2V_IMG_TOKENS and getattr(ca, "head_dim", None) == 128
+            and all(type(n).__name__ == "WanRMSNorm" and getattr(n, "weight", None) is not None for n in norms)
+            and len({float(n.eps) for n in norms}) == 1)
+
+
+def wan_i2v_cross_eligible(ca, x, context, context_lens):
+    """True when the fused block runs WanI2VCrossAttention `ca` as i2v_cross_attention: the shape rules
+    above, CUDA tensors and bf16 autocast"""
+    return _wan_i2v_cross_shape_ok(ca, x, context, context_lens) and x.is_cuda and DN._autocast_bf16()
+
+
+def _wan_i2v_cross(ca, x, context, context_lens):
+    """WanI2VCrossAttention.forward (model_mul.py:223-249) with its attention part as one
+    jenga_wan_i2v_cross_attn launch; the module's own q / k / v / k_img / v_img / o Linears run around
+    it.  Anything else runs the module's own forward."""
+    if wan_i2v_cross_eligible(ca, x, context, context_lens):
+        ctx_img, ctx = context[:, :_WAN_I2V_IMG_TOKENS], context[:, _WAN_I2V_IMG_TOKENS:]   # :230-231
+        q_lin, k_lin, v = ca.q(x), ca.k(ctx), ca.v(ctx)
+        kimg_lin, vimg = ca.k_img(ctx_img), ca.v_img(ctx_img)
+        lin_ok = all(t.dtype in (torch.bfloat16, torch.float32) for t in (q_lin, k_lin, kimg_lin))
+        if lin_ok and v.dtype == vimg.dtype == torch.bfloat16:
+            n = ca.num_heads
+            out = WAN.i2v_cross_attention(q_lin, k_lin, v.view(1, -1, n, 128), kimg_lin, vimg.view(1, -1, n, 128),
+                                          ca.norm_q.weight, ca.norm_k.weight, ca.norm_k_img.weight, n,
+                                          eps=float(ca.norm_q.eps))
+            STATS["wan_i2v_cross"] += 1
+            return ca.o(out.flatten(2))
+    STATS["fallback"] += 1
+    return ca(x, context, context_lens)
+
+
 def _make_wan_block_forward(orig, mod):
     def forward(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=0.0, freq_remap=None,
                 block_neighbor_list=None, p_remain_rates=0.0):
         args = (x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate, freq_remap,
                 block_neighbor_list, p_remain_rates)
+        i2v = type(self.cross_attn).__name__ == "WanI2VCrossAttention"
         ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
-              and type(self.cross_attn).__name__ == "WanT2VCrossAttention"
+              and (i2v or type(self.cross_attn).__name__ == "WanT2VCrossAttention")
               and self.modulation.dtype == torch.float32)
         if ok:
             with torch.autocast("cuda", dtype=torch.float32):                      # :326-327
@@ -415,7 +461,7 @@ def _make_wan_block_forward(orig, mod):
                   and DN.wan_residual_ln_supported(x, self.norm2, e6, affine=False)
                   and DN.wan_gate_residual_supported(x, e6))
         if not ok:
-            # no autocast, batch > 1, cross_attn_norm=False (norm3 is Identity), I2V cross-attention, …
+            # no autocast, batch > 1, cross_attn_norm=False (norm3 is Identity), …
             STATS["fallback"] += 1
             return orig(self, *args)
         e = e6.chunk(6, dim=1)
@@ -425,8 +471,10 @@ def _make_wan_block_forward(orig, mod):
                            p_remain_rates=p_remain_rates)                          # :331-333
         x, h = DN.wan_residual_ln(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight,
                                   bias=self.norm3.bias)                            # :334-335, :339
-        x, h = DN.wan_residual_ln(x, self.cross_attn(h, context, context_lens), None, eps=self.norm2.eps,
-                                  shift=e[3], scale=e[4])                          # :339-340
+        # WanI2VCrossAttention.forward itself stays unpatched: the block routes it here
+        cross = _wan_i2v_cross(self.cross_attn, h, context, context_lens) if i2v else \
+            self.cross_attn(h, context, context_lens)
+        x, h = DN.wan_residual_ln(x, cross, None, eps=self.norm2.eps, shift=e[3], scale=e[4])   # :339-340
         STATS["wan_block"] += 1
         return DN.wan_gate_residual(x, self.ffn(h), e[5])                          # :340-342
     forward.__jenga_b200__ = True
@@ -454,7 +502,8 @@ def patch_module(mod) -> list[str]:
         orig = mod.WanSelfAttention.forward
         mod.WanSelfAttention.forward = _make_wan_forward(orig, mod)
         done.append(f"{name}.WanSelfAttention.forward")
-    # WanI2VCrossAttention overrides forward itself and is left as it is
+    # WanI2VCrossAttention overrides forward itself and is left as it is; the fused block forward runs
+    # its fused form (_wan_i2v_cross)
     for cls, make in (("WanT2VCrossAttention", _make_wan_cross_forward), ("WanAttentionBlock", _make_wan_block_forward)):
         if hasattr(mod, cls) and not getattr(getattr(mod, cls).forward, "__jenga_b200__", False):
             getattr(mod, cls).forward = make(getattr(mod, cls).forward, mod)

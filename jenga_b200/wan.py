@@ -1,6 +1,7 @@
 """Wan2.1-side glue of the hot path (wan/modules/model_mul.py:134-180 WanSelfAttention.forward,
-:183-205 WanT2VCrossAttention.forward): fused WanRMSNorm + RoPE prologue, the block-count rules, the
-operator call and the dense text cross-attention."""
+:183-205 WanT2VCrossAttention.forward, :223-249 WanI2VCrossAttention.forward): fused WanRMSNorm + RoPE
+prologue, the block-count rules, the operator call, the dense text cross-attention and the I2V
+image + text cross-attention."""
 from __future__ import annotations
 
 import ctypes as C
@@ -122,3 +123,51 @@ def cross_attention(q_lin, k_lin, v, norm_q_w, norm_k_w, heads, eps=1e-6):
     out = torch.empty_like(q)
     _launch(q, k, v, None, 0, (L + BLOCK - 1) // BLOCK, D ** -0.5, 0.0, 1 << 30, Lc, L, Lc, out, None, torch.bfloat16)
     return out
+
+
+def i2v_cross_attn(q, k_img, v_img, k_txt, v_txt, sm_scale=None, out=None):
+    """One launch of jenga_wan_i2v_cross_attn: out = bf16(f32(A_img) + f32(A_txt)), each A the bf16 result
+    of a dense softmax(q k^T sm_scale) v over its own keys.  All [B, S, H, 128] bf16 with contiguous
+    channels; sm_scale defaults to 128^-1/2.  Returns `out` (allocated like q when None)."""
+    _require_cuda(q, k_img, v_img, k_txt, v_txt)
+    ts = (q, k_img, v_img, k_txt, v_txt) + (() if out is None else (out,))
+    if any(t.dim() != 4 or t.dtype != torch.bfloat16 or t.stride(3) != 1 for t in ts):
+        raise ValueError("q, k_img, v_img, k_txt, v_txt and out must be bf16 [B, S, H, 128] with contiguous channels")
+    B, L, H, D = q.shape
+    if (k_img.shape != v_img.shape or k_txt.shape != v_txt.shape or k_img.shape[::2] != (B, H)
+            or k_txt.shape[::2] != (B, H) or k_img.shape[3] != D or k_txt.shape[3] != D):
+        raise ValueError("k_img / v_img and k_txt / v_txt must be [B, S, H, D] with q's B, H and D")
+    if out is None:
+        out = torch.empty_like(q)
+    elif out.shape != q.shape:
+        raise ValueError("out must have q's shape")
+    a = _lib.JengaWanCrossArgs()
+    a.q, a.k_img, a.v_img, a.k_txt, a.v_txt, a.out = (t.data_ptr() for t in (q, k_img, v_img, k_txt, v_txt, out))
+    a.dtype, a.batch, a.heads, a.head_dim = _lib.JENGA_BF16, B, H, D
+    a.q_rows, a.img_rows, a.txt_rows = L, k_img.shape[1], k_txt.shape[1]
+    for name, t in (("q", q), ("ki", k_img), ("vi", v_img), ("kt", k_txt), ("vt", v_txt), ("o", out)):
+        setattr(a, f"{name}_stride_b", t.stride(0))
+        setattr(a, f"{name}_stride_s", t.stride(1))
+        setattr(a, f"{name}_stride_h", t.stride(2))
+    a.sm_scale = D ** -0.5 if sm_scale is None else float(sm_scale)
+    a.err_flag = None
+    with torch.cuda.device(q.device):
+        check(lib.jenga_wan_i2v_cross_attn(C.byref(a), _stream_ptr(q.device)), "wan_i2v_cross_attn")
+    return out
+
+
+def i2v_cross_attention(q_lin, k_lin, v, kimg_lin, vimg, wq, wk, wk_img, heads, eps=1e-6):
+    """WanI2VCrossAttention.forward's attention part (model_mul.py:230-247) for one sample with every
+    context row valid: q_lin [1, L, C] = self.q(x); k_lin [1, Lt, C] = self.k(context[:, 257:]) and
+    v [1, Lt, H, 128] = self.v(…) bf16; kimg_lin [1, Li, C] = self.k_img(context[:, :257]) and
+    vimg [1, Li, H, 128] = self.v_img(…) bf16.  Returns [1, L, H, 128] bf16: what self.o receives.
+
+    q, k and k_img go through the norm-only prologue, as in cross_attention; one launch then computes
+    both attentions and their sum, `x + img_x` in fp32 (:247) of the two fp32-typed flash_attention
+    results, rounded to bf16 as self.o's autocast cast does."""
+    q = norm_rope(q_lin, wq, heads, None, None, eps=eps)
+    k = norm_rope(k_lin, wk, heads, None, None, eps=eps)
+    ki = norm_rope(kimg_lin, wk_img, heads, None, None, eps=eps)
+    if v.dtype != torch.bfloat16 or v.shape != k.shape or vimg.dtype != torch.bfloat16 or vimg.shape != ki.shape:
+        raise ValueError("v / vimg must be bf16 [1, Lt / Li, heads, 128] like the projected keys")
+    return i2v_cross_attn(q, ki, vimg, k, v)
