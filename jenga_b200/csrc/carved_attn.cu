@@ -4,29 +4,12 @@
 //   hyvideo/modules/attention_block_triton_diffres.py:38-136 (+ launcher :139-196)
 // and its text-row flash_attn_func call (:371-380) with ONE launch.
 //
-// Work decomposition: one CTA per (batch*head, 128-row query block); 384 threads, three warpgroups:
-//   warpgroups 0, 1  consumers, 64 query rows each: S = Q~ K^T by wgmma (Q~ in registers, loaded
-//                    once per CTA with ldmatrix; K from shared memory; S in registers), online
-//                    softmax in base 2 on the registers, then O += P V by wgmma with P as the
-//                    register A operand; final O / l -> global
-//   warpgroup 2      producer: warp 8 issues TMA — Q once, then one K tile and one V tile per live
-//                    key block into a two-stage ring (K and V slots are released separately);
-//                    with FP8 P.V, warps 9..11 transpose each V tile (see kPvFp8)
-// setmaxnreg moves registers from the producer (24, or 40 with the FP8 transpose) to the consumers
-// (240, or 232): Q~, S, O and the packed P of the previous tile are all live in a consumer at once.
-// Keeping Q~ in registers takes a third of the shared-memory reads off Q.K^T: only K is read per tile.
-//
-// Consumer schedule (FlashAttention-3's):
-//   - in-warpgroup pipelining: iteration j issues S_j = Q~ K_j^T, then O += P_{j-1} V_{j-1}; it
-//     waits for S_j alone, runs softmax_j while P_{j-1} V_{j-1} is still on the tensor cores, then
-//     waits for that and applies the lazy rescale O *= alpha_j.  The prologue computes S_0 and its
-//     softmax, the epilogue issues the last P V.  O and l see the same operations in the same
-//     order as a plain S, softmax, P V loop, so the result is the same bit for bit.
-//   - ping-pong: the two warpgroups take turns to issue their GEMMs (named barriers kBarTurn and
-//     kBarTurn + 1), so one warpgroup's softmax runs while the other's GEMMs occupy the tensor
-//     cores.  Warpgroup 0 goes first.
-// S and O are fp32 register accumulators (64 + 64 registers per thread); one CTA per SM with
-// ~164 KB of shared memory.
+// Work decomposition: one CTA per (batch*head, 128-row query block), running the pipeline of
+// carved_attn_common.cuh over the live key blocks of its row; final O / l -> global.  With FP8 P.V,
+// producer warps 9..11 also transpose each V tile (see kPvFp8), so setmaxnreg leaves the producer 40
+// registers instead of 24 and gives the consumers 232 instead of 240.  Keeping Q~ in registers takes a
+// third of the shared-memory reads off Q.K^T: only K is read per tile.  One CTA per SM, ~164 KB of
+// shared memory.
 //
 // HBM/L2 layout: q,k,v stay in the caller's [B,S,H,D] layout; TMA boxes are {64 d, 128 rows}
 // with 128-byte swizzle.  K boxes are K-major wgmma operands, V boxes MN-major (no transpose).
@@ -43,41 +26,11 @@ namespace jenga {
 
 namespace {
 
-using attn::BlockWalker;
-using attn::KernelParams;
+using namespace attn;
 
-constexpr int kBlock = 128;           // rows per q block == keys per kv block
-constexpr int kHeadDim = 128;
-constexpr int kConsumerThreads = 256;
-constexpr int kThreads = kConsumerThreads + 128;  // + the producer warpgroup
 constexpr int kTransposeWarps = 3;               // producer warps 9..11 (FP8 P.V only)
-constexpr int kStages = 2;                       // K/V ring depth
-constexpr int kBoxBytes = kBlock * 64 * 2;       // 16 KB: 128 rows x 64 d (one TMA box)
-constexpr int kTileBytes = 2 * kBoxBytes;        // 32 KB: 128 rows x 128 d (two d halves)
 constexpr int kMaxMaskWords = 256;               // up to 8192 key blocks (1M tokens)
-constexpr uint32_t kBarTurn = 3;                 // named barriers 3, 4: consumer warpgroup 0's, 1's turn
-
-// shared-memory carve-up (offsets from the 1024-aligned base)
-constexpr int kOffQ = 0;
-constexpr int kOffK = kOffQ + kTileBytes;
-constexpr int kOffV = kOffK + kStages * kTileBytes;
-constexpr int kOffBars = kOffV + kStages * kTileBytes;
-constexpr int kOffMask = kOffBars + 128;
-constexpr int kSmemBytes = 1024 /*align slack*/ + kOffMask + kMaxMaskWords * 4;
-
-enum BarId {
-  Q_FULL = 0,
-  K_FULL = 1, V_FULL = K_FULL + kStages,
-  K_EMPTY = V_FULL + kStages, V_EMPTY = K_EMPTY + kStages,   // one arrival per consumer warp
-  VT_FULL = V_EMPTY + kStages,                                // FP8: one arrival per transpose warp
-  NUM_BARS = VT_FULL + kStages
-};
-static_assert(NUM_BARS * 8 <= 128, "barrier block overflow");
-
-// byte offset of (row, col) inside a 128-byte-swizzled tile of 128-byte rows (1024-B aligned)
-__device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t col) {
-  return row * 128u + ((((col >> 4) ^ row) & 7u) << 4) + (col & 15u);
-}
+constexpr int kSmemBytes = 1024 /*align slack*/ + kOffEnd + kMaxMaskWords * 4;   // + the row mask
 
 // kPvFp8 (opt-in): P and V enter the P.V product as FP8 e4m3 — V quantised per head by
 // jenga_quantize_v_fp8 (scale = absmax/448), P converted with cvt.rn.satfinite.e4m3x2 (p <= 2^8 by
@@ -104,11 +57,9 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint8_t* sQ = smem + kOffQ;
-  uint8_t* sK = smem + kOffK;  // + stage * kTileBytes
-  uint8_t* sV = smem + kOffV;
+  uint8_t* sV = smem + kOffV;  // + stage * kTileBytes
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
-  uint32_t* s_mask = reinterpret_cast<uint32_t*>(smem + kOffMask);
+  uint32_t* s_mask = reinterpret_cast<uint32_t*>(smem + kOffEnd);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -167,42 +118,13 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     // =============================== producer warpgroup ===============================
     setmaxnreg_dec<kPvFp8 ? 40 : 24>();
     if (warp == kConsumerThreads / 32) {
-      if (n_tiles > 0 && lane == 0) {   // TMA
-        if constexpr (kQkInt8) {   // 128 rows x 128 one-byte channels = one 16 KB box
-          mbar_arrive_expect_tx(&bars[Q_FULL], kBoxBytes);
-          tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
-        } else {
-          mbar_arrive_expect_tx(&bars[Q_FULL], kTileBytes);
-          tma_load_4d(sQ, &tm_q, &bars[Q_FULL], 0, static_cast<int>(q_row0), h, b);
-          tma_load_4d(sQ + kBoxBytes, &tm_q, &bars[Q_FULL], 64, static_cast<int>(q_row0), h, b);
-        }
+      if (n_tiles > 0 && lane == 0) {   // TMA: the live key blocks in mask order
         BlockWalker it(s_mask, nwords);
-        int j = 0;
-        for (int blk = it.next(); blk >= 0; blk = it.next(), ++j) {
-          const int s = j % kStages;
-          const uint32_t par = ((j / kStages) & 1) ^ 1;   // slot-free parity (a fresh barrier passes)
-          const int row0 = blk * kBlock;
-          uint8_t* k_dst = sK + s * kTileBytes;
-          uint8_t* v_dst = sV + s * kTileBytes;
-          mbar_wait(&bars[K_EMPTY + s], par, p.err_flag);
-          if constexpr (kQkInt8) {
-            mbar_arrive_expect_tx(&bars[K_FULL + s], kBoxBytes);
-            tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
-          } else {
-            mbar_arrive_expect_tx(&bars[K_FULL + s], kTileBytes);
-            tma_load_4d(k_dst, &tm_k, &bars[K_FULL + s], 0, row0, h, b);
-            tma_load_4d(k_dst + kBoxBytes, &tm_k, &bars[K_FULL + s], 64, row0, h, b);
-          }
-          mbar_wait(&bars[V_EMPTY + s], par, p.err_flag);
-          if constexpr (kPvFp8) {   // 128 keys x 128 one-byte channels = one 16 KB box
-            mbar_arrive_expect_tx(&bars[V_FULL + s], kBoxBytes);
-            tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
-          } else {
-            mbar_arrive_expect_tx(&bars[V_FULL + s], kTileBytes);
-            tma_load_4d(v_dst, &tm_v, &bars[V_FULL + s], 0, row0, h, b);
-            tma_load_4d(v_dst + kBoxBytes, &tm_v, &bars[V_FULL + s], 64, row0, h, b);
-          }
-        }
+        produce<kPvFp8, kQkInt8>(smem, bars, p.err_flag, &tm_q, static_cast<int>(q_row0), h, b,
+                                 [&](int, KvMaps& m) {
+                                   m = {&tm_k, &tm_v};
+                                   return it.next() * kBlock;   // < 0 past the last live block
+                                 });
       }
     } else if constexpr (kPvFp8) {
       // V^T[d][32 g + L] = V[32 g + perm(L)][d], perm(4 t + u) = {2t, 2t+1, 2t+8, 2t+9}[u] (+16 for
@@ -240,256 +162,55 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
 
   // =============================== consumers ===============================
   setmaxnreg_inc<kPvFp8 ? 232 : 240>();
-  const int wg = warp >> 2;                       // warpgroup: query rows [64 wg, 64 wg + 64)
-  const int g = lane >> 2, qd = lane & 3;
-  // accumulator fragment: element i of a thread is row g + 8 ((i >> 1) & 1) of the warp's 16 rows,
-  // column 8 (i >> 2) + 2 qd + (i & 1)
-  const int row_lo = wg * 64 + (warp & 3) * 16 + g;
-  float m_used[2] = {-INFINITY, -INFINITY};  // running (possibly stale) max, in scaled log2 units
-  float l_sum[2] = {0.f, 0.f};               // this thread's partial sums (its 32 columns)
-  float o[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  Consumer<kBF16, kPvFp8, kQkInt8> cons(smem, bars, p.err_flag);
   // sparse class: Q~ = round(Q * qk_scale) and raw S is already in log2 units (c = 1)
   // dense class : raw S, scaled inside the exponent (c = qk_scale), like FlashAttention
   // kQkInt8     : integer S, scaled inside the exponent by c = q_scale * k_scale[blk] * qk_scale
   const float c = dense ? p.qk_scale : 1.0f;
-  const float qs = kQkInt8 && n_tiles > 0 ? __ldg(p.q_scale + bh * p.q_groups + 2 * qb + wg) * p.qk_scale : 0.f;
+  const float qs = kQkInt8 && n_tiles > 0 ? __ldg(p.q_scale + bh * p.q_groups + 2 * qb + cons.wg) * p.qk_scale : 0.f;
 
   if (n_tiles > 0) {
-    mbar_wait(&bars[Q_FULL], 0, p.err_flag);
-    const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128;   // kQkInt8: this warpgroup's 64 rows
-    // 16-bit Q: the warpgroup's 64 rows stay in registers as the A operand of all its Q.K^T wgmmas
-    // (16 k per step: matrices {rows 0-7, 8-15} x {k 0-7, 8-15} of the warp's 16 rows)
-    uint32_t qa[kQkInt8 ? 1 : 8][4];
+    cons.load_q();
     if constexpr (!kQkInt8) {
-      const int q_row = wg * 64 + (warp & 3) * 16 + (lane & 7) + 8 * ((lane >> 3) & 1);
-#pragma unroll
-      for (int kk = 0; kk < kHeadDim / 16; ++kk)
-        ldmatrix_x4(qa[kk], sQ + (kk >> 2) * kBoxBytes + sw128(q_row, (kk & 3) * 32 + (lane >> 4) * 16));
       if (!dense) {   // ref :87-88  q = (q * qk_scale).to(dtype)
 #pragma unroll
         for (int kk = 0; kk < kHeadDim / 16; ++kk)
 #pragma unroll
           for (int t = 0; t < 4; ++t) {
-            const float2 f = unpack2<kBF16>(qa[kk][t]);
-            qa[kk][t] = pack2<kBF16>(f.x * p.qk_scale, f.y * p.qk_scale);
+            const float2 f = unpack2<kBF16>(cons.qa[kk][t]);
+            cons.qa[kk][t] = pack2<kBF16>(f.x * p.qk_scale, f.y * p.qk_scale);
           }
       }
     }
-
-    float sc[64];                      // S_j, then P_j in fp32
-    int32_t si[kQkInt8 ? 64 : 1];      // kQkInt8: integer S_j while its wgmma runs
-    uint32_t pa[kPvFp8 ? 4 : 8][4];    // P_{j-1}: A operand of the P.V wgmma; untouched while it runs
-    float alpha[2];
-
-    // Turns: a warpgroup waits on its own barrier before it issues GEMMs and arrives on the
-    // other's once they are issued.  Warpgroup 1 arrives ahead for warpgroup 0's first turn and
-    // skips the hand-over after its own last turn: both take the same number of turns, so every
-    // barrier sees as many arrivals as waits.
-    auto turn_begin = [&] { named_bar_sync(kBarTurn + wg, kConsumerThreads); };
-    auto turn_end = [&](bool last) {
-      if (!(last && wg == 1)) named_bar_arrive(kBarTurn + (wg ^ 1), kConsumerThreads);
-    };
-    auto release = [&](int bar) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[bar]);
-    };
-    // ---- S = Q~ K^T (64 x 128 per warpgroup, K = 128 in 8 steps) ----
-    auto issue_qk = [&](int s) {
-      const uint32_t k_addr = smem_u32(sK + s * kTileBytes);
-      if constexpr (kQkInt8) {   // K = 128 in 4 steps of 32 one-byte channels inside the swizzled row
-#pragma unroll
-        for (int kc = 0; kc < kHeadDim / 32; ++kc)
-          wgmma_128_ss_s8(si, gmma_desc_sw128(q_addr + kc * 32, 16, 1024),
-                          gmma_desc_sw128(k_addr + kc * 32, 16, 1024), kc > 0 ? 1u : 0u);
-      } else {
-#pragma unroll
-        for (int kk = 0; kk < kHeadDim / 16; ++kk) {
-          const uint32_t off = (kk & 3) * 32 + (kk >> 2) * kBoxBytes;
-          wgmma_128_rs<kBF16>(sc, qa[kk], gmma_desc_sw128(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
-        }
-      }
-      wgmma_commit();
-    };
-    // S_j has retired: make it visible (and, for kQkInt8, exact fp32: |S| <= 128 * 127^2 < 2^22, so
-    // the s32 value lands in the mantissa of 1.5 * 2^23 — two ALU ops, no 16/clk I2F)
-    auto scores_ready = [&] {
-      if constexpr (kQkInt8) {
-        fence_regs(si);
-#pragma unroll
-        for (int i = 0; i < 64; ++i) sc[i] = __int_as_float(si[i] + 0x4B400000) - 12582912.f;
-      } else {
-        fence_regs(sc);
-      }
-    };
-    // exponent factor of key block blk (kQkInt8: read before the tile's waits, so the softmax
-    // never stalls on it; never 0, which would turn the -inf of masked columns into NaN)
-    auto tile_c = [&](int blk) -> float {
-      if constexpr (kQkInt8) return fmaxf(qs * __ldg(p.k_scale + bh * p.k_groups + blk), FLT_MIN);
-      else return c;
-    };
-    // ---- O += P V ----
-    auto issue_pv = [&](int s) {
-      if constexpr (kPvFp8) {
-        const uint32_t vt_addr = smem_u32(sV + s * kTileBytes + kBoxBytes);
-#pragma unroll
-        for (int kc = 0; kc < 4; ++kc)
-          wgmma_128_rs_e4m3(o, pa[kc], gmma_desc_sw128(vt_addr + kc * 32, 16, 1024), 1u);
-      } else {
-        const uint32_t v_addr = smem_u32(sV + s * kTileBytes);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)   // 16 keys = 16 rows x 128 B inside each V box
-          wgmma_128_rs_bmn<kBF16>(o, pa[kk], gmma_desc_sw128(v_addr + kk * 16 * 128, kBoxBytes, 1024), 1u);
-      }
-      wgmma_commit();
-    };
-    // ---- online softmax of key block blk on sc; true when O must be rescaled by alpha ----
-    auto softmax = [&](int blk, float ct) -> bool {
-      // ref :113-114 — text_amp is a constant added to every score of a text key block, in
-      // log2 units (sparse class only, where c == 1): fold it into the exponent offset.
-      const float amp = (!dense && blk >= p.text_block_start) ? p.text_amp : 0.f;
-      const long long col0 = static_cast<long long>(blk) * kBlock;
-      if (col0 + kBlock > kv_limit) {  // rare: only the tile that straddles seqlen
-#pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (col0 + (i >> 2) * 8 + qd * 2 + (i & 1) >= kv_limit) sc[i] = -INFINITY;  // ref :117-118
-      }
-      float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 64; i += 4) {
-        mx[0] = fmaxf(mx[0], fmaxf(sc[i], sc[i + 1]));
-        mx[1] = fmaxf(mx[1], fmaxf(sc[i + 2], sc[i + 3]));
-      }
-      float m_cand[2];
-      bool need = false;
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        m_cand[r] = fmaxf(m_used[r], fmaf(mx[r], ct, amp));
-        // Lazy rescale: the reference rescales acc by exp2(m_old - m_new) every tile
-        // (:121-132).  O/l is invariant to the reference point, so it only moves when the
-        // max grew by more than 2^8 — the final O/l is the same up to fp32 rounding.
-        need = need || (m_cand[r] - m_used[r]) > 8.0f;   // false for NaN (-inf - -inf)
-      }
-      const bool rescale = __any_sync(0xffffffffu, need);
-      if (rescale) {
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          alpha[r] = (m_cand[r] == -INFINITY) ? 1.0f : fast_exp2(m_used[r] - m_cand[r]);
-          l_sum[r] *= alpha[r];
-          m_used[r] = m_cand[r];
-        }
-      }
-      // p = exp2(s*c + off); l accumulates the unrounded p (ref :131), P is rounded to the
-      // input dtype for the PV product (ref :128)
-      float off[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) off[r] = amp - ((m_used[r] == -INFINITY) ? 0.f : m_used[r]);
-#pragma unroll
-      for (int i = 0; i < 64; ++i) {
-        const int r = (i >> 1) & 1;
-        sc[i] = fast_exp2(fmaf(sc[i], ct, off[r]));
-        l_sum[r] += sc[i];
-      }
-      return rescale;
-    };
-    auto rescale_o = [&] {
-#pragma unroll
-      for (int r = 0; r < 2; ++r)
-#pragma unroll
-        for (int i = 2 * r; i < 64; i += 4) {
-          o[i] *= alpha[r];
-          o[i + 1] *= alpha[r];
-        }
-    };
-    auto pack_p = [&] {
-      if constexpr (kPvFp8) {
-#pragma unroll
-        for (int kc = 0; kc < 4; ++kc) {
-          const float* x = sc + 16 * kc;
-          pa[kc][0] = pack4_e4m3(x[0], x[1], x[4], x[5]);
-          pa[kc][1] = pack4_e4m3(x[2], x[3], x[6], x[7]);
-          pa[kc][2] = pack4_e4m3(x[8], x[9], x[12], x[13]);
-          pa[kc][3] = pack4_e4m3(x[10], x[11], x[14], x[15]);
-        }
-      } else {
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)
-#pragma unroll
-          for (int t = 0; t < 4; ++t) pa[kk][t] = pack2<kBF16>(sc[8 * kk + 2 * t], sc[8 * kk + 2 * t + 1]);
-      }
-    };
-    constexpr int kVReady = kPvFp8 ? VT_FULL : V_FULL;
-
-    if (wg == 1) named_bar_arrive(kBarTurn, kConsumerThreads);
     BlockWalker it(s_mask, nwords);
-    // prologue: S_0 and its softmax
-    int blk = it.next();
-    float ct = tile_c(blk);
-    mbar_wait(&bars[K_FULL], 0, p.err_flag);
-    turn_begin();
-    wgmma_fence();
-    issue_qk(0);
-    turn_end(false);
-    wgmma_wait<0>();
-    scores_ready();
-    release(K_EMPTY);
-    if (softmax(blk, ct)) rescale_o();
-    pack_p();
-    int j = 1;
-    for (blk = it.next(); blk >= 0; blk = it.next(), ++j) {   // S_j and P_{j-1} V_{j-1}
-      const int s = j % kStages, sv = (j - 1) % kStages;
-      ct = tile_c(blk);
-      mbar_wait(&bars[kVReady + sv], ((j - 1) / kStages) & 1, p.err_flag);
-      mbar_wait(&bars[K_FULL + s], (j / kStages) & 1, p.err_flag);
-      turn_begin();
-      fence_regs(o);
-      wgmma_fence();
-      issue_qk(s);
-      issue_pv(sv);
-      turn_end(false);
-      wgmma_wait<1>();
-      scores_ready();
-      release(K_EMPTY + s);
-      const bool rescale = softmax(blk, ct);
-      wgmma_wait<0>();
-      fence_regs(o);
-      release(V_EMPTY + sv);
-      if (rescale) rescale_o();
-      pack_p();
-    }
-    // epilogue: P V of the last tile
-    const int sv = (j - 1) % kStages;
-    mbar_wait(&bars[kVReady + sv], ((j - 1) / kStages) & 1, p.err_flag);
-    turn_begin();
-    fence_regs(o);
-    wgmma_fence();
-    issue_pv(sv);
-    turn_end(true);
-    wgmma_wait<0>();
-    fence_regs(o);
-    release(V_EMPTY + sv);
+    cons.run(
+        n_tiles,
+        [&](int, Tile& t) {
+          const int blk = it.next();
+          // exponent factor: kQkInt8's is never 0, which would turn the -inf of masked columns into
+          // NaN.  ref :113-114 — text_amp is a constant added to every score of a text key block, in
+          // log2 units (sparse class only, where c == 1)
+          t = {static_cast<long long>(blk) * kBlock, kv_limit,
+               kQkInt8 ? fmaxf(qs * __ldg(p.k_scale + bh * p.k_groups + blk), FLT_MIN) : c,
+               (!dense && blk >= p.text_block_start) ? p.text_amp : 0.f, false};
+        },
+        [](const float (&)[2]) {});   // one segment
   }
 
   // ---- epilogue: O / l -> global (ref :135-136); rows past the limit are zeros (:156) ----
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    l_sum[r] += __shfl_xor_sync(0xffffffffu, l_sum[r], 1);
-    l_sum[r] += __shfl_xor_sync(0xffffffffu, l_sum[r], 2);
-  }
+  for (int r = 0; r < 2; ++r) cons.l_sum[r] = row_sum(cons.l_sum[r]);
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    const long long q_row = q_row0 + row_lo + 8 * r;
+    const long long q_row = q_row0 + cons.row_lo + 8 * r;
     const bool in_tensor = q_row < p.q_rows;
     const bool zero_row = (n_tiles == 0) || (!dense && q_row >= q_limit_sparse);
-    float inv_l = zero_row ? 0.f : 1.0f / l_sum[r];
+    float inv_l = zero_row ? 0.f : 1.0f / cons.l_sum[r];
     if constexpr (kPvFp8) inv_l *= __ldg(p.v_fp8_amax + b * p.heads + h) * (1.0f / 448.0f);   // undo the V scale
-    if (p.lse_out && dense && in_tensor && qd == 0) {
+    if (p.lse_out && dense && in_tensor && cons.qd == 0) {
       // softmax_lse of flash_attn (natural log): ln sum_j exp(s_j * sm_scale) = (m + log2 l) * ln 2
       p.lse_out[(static_cast<long long>(b) * p.heads + h) * p.q_rows + q_row] =
-          zero_row ? -INFINITY : (m_used[r] + log2f(l_sum[r])) * 0.6931471805599453f;
+          zero_row ? -INFINITY : (cons.m_used[r] + log2f(cons.l_sum[r])) * 0.6931471805599453f;
     }
     if (!in_tensor) continue;
     // destination(s) of this row
@@ -515,8 +236,8 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
 #pragma unroll
     for (int n8 = 0; n8 < 16; ++n8) {
       const int i = 4 * n8 + 2 * r;
-      const int col = 8 * n8 + 2 * qd;
-      const uint32_t v = pack2<kBF16>(zero_row ? 0.f : o[i] * inv_l, zero_row ? 0.f : o[i + 1] * inv_l);
+      const int col = 8 * n8 + 2 * cons.qd;
+      const uint32_t v = pack2<kBF16>(zero_row ? 0.f : cons.o[i] * inv_l, zero_row ? 0.f : cons.o[i + 1] * inv_l);
       if (n_dst > 1) {
         for (int rr = 0; rr < n_dst; ++rr)
           *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.peer_out[rr]) + o_off + col) = v;
@@ -594,24 +315,6 @@ __global__ void __launch_bounds__(kOrderThreads) carved_attn_order_kernel(const 
 // ------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------
-static int make_tile_map(CUtensorMap* map, const void* base, int dtype, long long rows, int heads,
-                         int batch, long long stride_b, long long stride_s, long long stride_h,
-                         int box_rows) {
-  // dims (fastest first): d, row, head, batch.  Box {64, box_rows, 1, 1}, 128-B swizzle.
-  const cuuint64_t dims[4] = {static_cast<cuuint64_t>(kHeadDim), static_cast<cuuint64_t>(rows),
-                              static_cast<cuuint64_t>(heads), static_cast<cuuint64_t>(batch)};
-  const cuuint64_t strides[3] = {static_cast<cuuint64_t>(stride_s) * 2,
-                                 static_cast<cuuint64_t>(stride_h) * 2,
-                                 static_cast<cuuint64_t>(stride_b) * 2};
-  const cuuint32_t box[4] = {64, static_cast<cuuint32_t>(box_rows), 1, 1};
-  const cuuint32_t elem_strides[4] = {1, 1, 1, 1};
-  const CUtensorMapDataType dt =
-      dtype == JENGA_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  return encode_tensor_map(map, dt, 4, const_cast<void*>(base), dims, strides, box, elem_strides,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-}
-
 // one-byte operands (FP8 V, int8 Q / K): contiguous [B, S, H, 128] bytes; box {128 channels, 128 rows}
 static int make_bytes_map(CUtensorMap* map, const void* base, long long rows, int heads, int batch) {
   const cuuint64_t dims[4] = {static_cast<cuuint64_t>(kHeadDim), static_cast<cuuint64_t>(rows),
@@ -624,8 +327,6 @@ static int make_bytes_map(CUtensorMap* map, const void* base, long long rows, in
                            elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
-
-static bool stride_ok(long long s) { return s > 0 && (s * 2) % 16 == 0; }
 
 int64_t carved_attn_sched_workspace_bytes(long long batch, long long heads, long long nq_sparse, long long nq_dense) {
   if (batch <= 0 || heads <= 0 || nq_sparse < 0 || nq_dense < 0) return 0;
@@ -719,16 +420,16 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
     if ((rc = make_bytes_map(&tm_k, qk->k_i8, qk->kv_rows_padded, a->heads, a->batch))) return rc;
   } else {
     if ((rc = make_tile_map(&tm_q, a->q, a->dtype, a->q_rows, a->heads, a->batch, a->q_stride_b,
-                            a->q_stride_s, a->q_stride_h, kBlock)))
+                            a->q_stride_s, a->q_stride_h)))
       return rc;
     if ((rc = make_tile_map(&tm_k, a->k, a->dtype, a->kv_rows, a->heads, a->batch, a->k_stride_b,
-                            a->k_stride_s, a->k_stride_h, kBlock)))
+                            a->k_stride_s, a->k_stride_h)))
       return rc;
   }
   if (pv_fp8) {
     if ((rc = make_bytes_map(&tm_v, a->v_fp8, a->kv_rows, a->heads, a->batch))) return rc;
   } else if ((rc = make_tile_map(&tm_v, a->v, a->dtype, a->kv_rows, a->heads, a->batch, a->v_stride_b,
-                                 a->v_stride_s, a->v_stride_h, kBlock)))
+                                 a->v_stride_s, a->v_stride_h)))
     return rc;
 
   KernelParams p{};
