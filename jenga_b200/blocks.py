@@ -20,13 +20,15 @@ section (modulation, linear layers, gates, MLP) is executed by the block's own s
 the reference module's own helper functions (`modulate`, `apply_gate`), so those numerics are the
 reference's by construction.  Whenever a call is not the carved configuration (sa_drop_rate == 0,
 no RMS qk-norm, unusual dtype, batch > 1 for Wan, sequence parallel for I2V, …) the ORIGINAL forward
-runs.
+runs, with the caller's own arguments (`_patched`).
 
 The I2V blocks differ from the HunyuanVideo ones in three ways the fused forwards follow: the
 token-replace modulation (rows of the first frame take the `tr_` shift / scale / gate; the
 reference does it with boolean-mask index_put, modulate_layers.py:51-56,84-95, here it is a per-row
 parameter select inside the ln_modulate / gate_residual kernels), a ragged S = L + 400 that the
-operator zero-pads to whole blocks, and the operator's default text_blocks=4.
+operator zero-pads to whole blocks, and the operator's default text_blocks=4.  Both variants run one
+fused body per stream kind (`_double_stream`, `_single_stream`); each keeps a thin entry point with
+its reference signature that hands the body these differences.
 
 The Wan block forward runs its elementwise chains as the wan_* dense kernels (fp32 residual stream,
 one pass per chain, bf16 handed to the Linears as autocast would cast it) and leaves the Linears, the
@@ -42,6 +44,7 @@ token reorder of jenga_hyvideo.py:116-118,226 and jenga_wan.py:559,655 — to `j
 """
 from __future__ import annotations
 
+import functools
 import importlib.abc
 import importlib.machinery
 import sys
@@ -76,9 +79,12 @@ def _rms_params(norm):
     return norm.weight, float(norm.eps)
 
 
-def _carved_call(x, sa_drop_rate, curve_sel):
+def _carved_call(self, x, norms, sa_drop_rate, curve_sel, cu_seqlens_q, per_block_token):
+    """the carved configuration the fused forwards of both HunyuanVideo variants take: a bf16 / fp16
+    CUDA input, a sparse call with a curve, RMS qk-norms, 128-token blocks and head_dim 128"""
     return (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and sa_drop_rate != 0.0
-            and curve_sel is not None and not isinstance(curve_sel, int))
+            and curve_sel is not None and not isinstance(curve_sel, int) and None not in norms
+            and per_block_token == HY.BLOCK and cu_seqlens_q is not None and x.shape[-1] // self.heads_num == 128)
 
 
 def _ln_mod(mod, norm, x, shift, scale, tr=None):
@@ -104,305 +110,226 @@ def _gate_res(mod, x, y, gate, tr=None):
     return x + mod.apply_gate(y, gate=gate, condition_type="token_replace", tr_gate=tr[0], first_frame_mask=tr[1])
 
 
-def _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis, cu_seqlens_q, cu_seqlens_kv,
-                       sa_drop_rate, txt_amp, curve_sel, p_remain_rates, txt_block_num, per_block_token,
-                       text_blocks_default, out=None, pad_ragged=False):
+def _modulation(layer, vec, n, tr):
+    """layer(vec).chunk(n): the block's (shift, scale, gate) triples.  Also returns, per triple, the
+    token-replace arguments of _ln_mod and _gate_res — (tr_shift, tr_scale, first_frame_mask) and
+    (tr_gate, first_frame_mask) — or None each without token replace (I2V models_mul.py:156-179,
+    :413-424).  tr: (token_replace_vec, first_frame_mask) or None."""
+    if tr is None:
+        return layer(vec).chunk(n, dim=-1), [None] * (n // 3 * 2)
+    token_replace_vec, mask = tr
+    mods, tr_mods = layer(vec, condition_type="token_replace", token_replace_vec=token_replace_vec)
+    r = tr_mods.chunk(n, dim=-1)
+    args = []
+    for i in range(0, n, 3):
+        args += [(r[i], r[i + 1], mask), (r[i + 2], mask)]
+    return mods.chunk(n, dim=-1), args
+
+
+def _attention_section(self, mod, img_qkv, txt_qkv, norms, *, freqs_cis, cu_seqlens_q, cu_seqlens_kv,
+                       sa_drop_rate, txt_amp, curve_sel, p_remain_rates, text_blocks, pad_ragged, out=None):
     """prologue -> (SP exchange | select + carved attention).  Returns attn [B, L+T, H*D]
     (written into `out`, a [B, L+T, H, D] view, when given and not under SP).
     pad_ragged: S = L+T need not be a multiple of 128 (the I2V operator zero-pads it)."""
     (wq_i, eps), (wk_i, _), (wq_t, _), (wk_t, _) = norms
-    heads = self.heads_num
     L = img_qkv.shape[1]
     _, _, block_neighbor_list = mod.random.choice(curve_sel)                       # :232 / :438
-    top_k = int((1 - sa_drop_rate) * (L // per_block_token))                       # models_mul…:242
     sp = getattr(self, "hybrid_seq_parallel_attn", None)
-    want_pool = not sp
-    S = L + (0 if txt_qkv is None else txt_qkv.shape[1])
-    if want_pool and S % HY.BLOCK and not pad_ragged:
-        return None
-    q, k, v, pools = HY.attention_prologue(img_qkv, txt_qkv, heads, wq_i, wk_i, wq_t, wk_t, eps, freqs_cis,
-                                           want_pool=want_pool)
+    top_k = HY.select_block_num(sa_drop_rate, L, mod.get_sequence_parallel_world_size() if sp else 1)  # :242, :249-251
+    q, k, v, pools = HY.attention_prologue(img_qkv, txt_qkv, self.heads_num, wq_i, wk_i, wq_t, wk_t, eps, freqs_cis,
+                                           want_pool=not sp)
     if sp:
-        top_k = mod.get_sequence_parallel_world_size() * top_k                      # :249-251
         return mod.my_parallel_attention(sp, q, k, v, img_q_len=L, img_kv_len=L, cu_seqlens_q=cu_seqlens_q,
                                          cu_seqlens_kv=cu_seqlens_kv, top_k=top_k, text_amp=txt_amp,
                                          block_neighbor_list=block_neighbor_list,
                                          p_remain_rates=p_remain_rates)
-    return HY.carved_attention_from_pools(q, k, v, pools, top_k=top_k, text_blocks=txt_block_num,
+    return HY.carved_attention_from_pools(q, k, v, pools, top_k=top_k, text_blocks=text_blocks,
                                           text_amp=txt_amp, block_neighbor_list=block_neighbor_list,
                                           p_remain_rates=p_remain_rates, cu_seqlens_q=cu_seqlens_q, out=out,
                                           pad_ragged=pad_ragged)
 
 
 # ------------------------------------------------------------------------------------------------
-# HunyuanVideo blocks
+# HunyuanVideo and HunyuanVideo-I2V blocks: one body per stream kind
 # ------------------------------------------------------------------------------------------------
-def _make_double_forward(orig, mod, text_blocks_default):
-    def forward(self, img, txt, vec, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
-                max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, txt_amp=1.0, curve_sel=None,
-                p_remain_rates=0.5, txt_block_num=text_blocks_default, per_block_token=128):
-        norms = [_rms_params(n) for n in (self.img_attn_q_norm, self.img_attn_k_norm,
-                                          self.txt_attn_q_norm, self.txt_attn_k_norm)]
-        if (not _carved_call(img, sa_drop_rate, curve_sel) or None in norms or per_block_token != HY.BLOCK
-                or cu_seqlens_q is None or img.shape[-1] // self.heads_num != 128):
-            STATS["fallback"] += 1
-            return orig(self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv,
-                        freqs_cis, sa_drop_rate, txt_amp, curve_sel, p_remain_rates, txt_block_num,
-                        per_block_token)
-        i_shift1, i_scale1, i_gate1, i_shift2, i_scale2, i_gate2 = self.img_mod(vec).chunk(6, dim=-1)
-        t_shift1, t_scale1, t_gate1, t_shift2, t_scale2, t_gate2 = self.txt_mod(vec).chunk(6, dim=-1)
-        img_qkv = self.img_attn_qkv(_ln_mod(mod, self.img_norm1, img, i_shift1, i_scale1))
-        txt_qkv = self.txt_attn_qkv(_ln_mod(mod, self.txt_norm1, txt, t_shift1, t_scale1))
-        assert cu_seqlens_q.shape[0] == 2 * img.shape[0] + 1                         # :244-246
-        attn = _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis, cu_seqlens_q, cu_seqlens_kv,
-                                  sa_drop_rate, txt_amp, curve_sel, p_remain_rates, txt_block_num,
-                                  per_block_token, text_blocks_default)
-        if attn is None:
-            STATS["fallback"] += 1
-            return orig(self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv,
-                        freqs_cis, sa_drop_rate, txt_amp, curve_sel, p_remain_rates, txt_block_num,
-                        per_block_token)
-        STATS["hy_double"] += 1
-        L = img.shape[1]
-        img_attn, txt_attn = attn[:, :L], attn[:, L:]
-        img = _gate_res(mod, img, self.img_attn_proj(img_attn), i_gate1)
-        img = _gate_res(mod, img, self.img_mlp(_ln_mod(mod, self.img_norm2, img, i_shift2, i_scale2)), i_gate2)
-        txt = _gate_res(mod, txt, self.txt_attn_proj(txt_attn), t_gate1)
-        txt = _gate_res(mod, txt, self.txt_mlp(_ln_mod(mod, self.txt_norm2, txt, t_shift2, t_scale2)), t_gate2)
-        return img, txt
-    forward.__jenga_b200__ = True
-    forward.__wrapped__ = orig
-    return forward
+# The bodies return None when the call is not the carved configuration; _patched then runs the
+# original forward.  The variants hand them what differs:
+#   stat          the STATS key of the fused forward
+#   tr            (token_replace_vec, first_frame_mask) for I2V token replace, else None
+#   text_blocks   the operator's text_blocks: txt_block_num for HunyuanVideo, always 4 for I2V
+#   pad_ragged    the I2V operator zero-pads S = L + T to whole blocks
+#   ok            the variant's own eligibility rules
+def _double_stream(mod, self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp, curve_sel,
+                   p_remain_rates, per_block_token, *, stat, tr, text_blocks, pad_ragged, ok):
+    norms = [_rms_params(n) for n in (self.img_attn_q_norm, self.img_attn_k_norm,
+                                      self.txt_attn_q_norm, self.txt_attn_k_norm)]
+    if not (ok and _carved_call(self, img, norms, sa_drop_rate, curve_sel, cu_seqlens_q, per_block_token)):
+        return None
+    (i_shift1, i_scale1, i_gate1, i_shift2, i_scale2, i_gate2), (tr_mod1, tr_gate1, tr_mod2, tr_gate2) = \
+        _modulation(self.img_mod, vec, 6, tr)
+    t_shift1, t_scale1, t_gate1, t_shift2, t_scale2, t_gate2 = self.txt_mod(vec).chunk(6, dim=-1)
+    img_qkv = self.img_attn_qkv(_ln_mod(mod, self.img_norm1, img, i_shift1, i_scale1, tr=tr_mod1))
+    txt_qkv = self.txt_attn_qkv(_ln_mod(mod, self.txt_norm1, txt, t_shift1, t_scale1))
+    assert cu_seqlens_q.shape[0] == 2 * img.shape[0] + 1                         # :244-246
+    attn = _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis=freqs_cis, cu_seqlens_q=cu_seqlens_q,
+                              cu_seqlens_kv=cu_seqlens_kv, sa_drop_rate=sa_drop_rate, txt_amp=txt_amp,
+                              curve_sel=curve_sel, p_remain_rates=p_remain_rates, text_blocks=text_blocks,
+                              pad_ragged=pad_ragged)
+    STATS[stat] += 1
+    L = img.shape[1]
+    img_attn, txt_attn = attn[:, :L], attn[:, L:]
+    img = _gate_res(mod, img, self.img_attn_proj(img_attn), i_gate1, tr=tr_gate1)   # :297-305
+    img = _gate_res(mod, img, self.img_mlp(_ln_mod(mod, self.img_norm2, img, i_shift2, i_scale2, tr=tr_mod2)),
+                    i_gate2, tr=tr_gate2)
+    txt = _gate_res(mod, txt, self.txt_attn_proj(txt_attn), t_gate1)                 # :307-315
+    txt = _gate_res(mod, txt, self.txt_mlp(_ln_mod(mod, self.txt_norm2, txt, t_shift2, t_scale2)), t_gate2)
+    return img, txt
 
 
-def _make_single_forward(orig, mod, text_blocks_default):
-    def forward(self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
-                max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, txt_amp=1.0, curve_sel=None,
-                p_remain_rates=0.5, txt_block_num=text_blocks_default, per_block_token=128):
-        norms = [_rms_params(n) for n in (self.q_norm, self.k_norm)]
-        if (not _carved_call(x, sa_drop_rate, curve_sel) or None in norms or per_block_token != HY.BLOCK
-                or cu_seqlens_q is None or freqs_cis is None or self.hidden_size // self.heads_num != 128):
-            STATS["fallback"] += 1
-            return orig(self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv,
-                        freqs_cis, sa_drop_rate, txt_amp, curve_sel, p_remain_rates, txt_block_num,
-                        per_block_token)
-        shift, scale, gate = self.modulation(vec).chunk(3, dim=-1)
-        lin1 = self.linear1(_ln_mod(mod, self.pre_norm, x, shift, scale))
-        C3 = 3 * self.hidden_size
-        L = x.shape[1] - txt_len
-        # strided views into linear1's output: no split / rearrange / cat copies (:413-441)
-        img_qkv, txt_qkv = lin1[:, :L, :C3], lin1[:, L:, :C3]
-        mlp = lin1[:, :, C3:]
-        assert cu_seqlens_q.shape[0] == 2 * x.shape[0] + 1                           # :444-446
-        # `torch.cat((attn, self.mlp_act(mlp)), 2)` (:499) without the concatenation copy: the attention
-        # kernel writes its rows into the first `hidden` columns of linear2's input buffer and the
-        # GELU kernel writes the rest
-        act = self.mlp_act
-        fuse_cat = (isinstance(act, torch.nn.GELU) and getattr(act, "approximate", "none") == "tanh"
-                    and lin1.dtype == torch.bfloat16 and x.shape[0] == 1
-                    and not getattr(self, "hybrid_seq_parallel_attn", None))
-        cat = attn_view = None
-        if fuse_cat:
-            cat = torch.empty((x.shape[0], x.shape[1], C3 // 3 + mlp.shape[-1]), dtype=lin1.dtype, device=lin1.device)
-            attn_view = cat[:, :, :C3 // 3].unflatten(2, (self.heads_num, -1))
-        attn = _attention_section(self, mod, img_qkv, txt_qkv, [norms[0], norms[1], norms[0], norms[1]],
-                                  freqs_cis, cu_seqlens_q, cu_seqlens_kv, sa_drop_rate, txt_amp, curve_sel,
-                                  p_remain_rates, txt_block_num, per_block_token, text_blocks_default, out=attn_view)
-        if attn is None:
-            STATS["fallback"] += 1
-            return orig(self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv,
-                        freqs_cis, sa_drop_rate, txt_amp, curve_sel, p_remain_rates, txt_block_num,
-                        per_block_token)
-        STATS["hy_single"] += 1
-        if fuse_cat:
-            STATS["gelu_cat"] += 1
-            DN.gelu_tanh_into(mlp, cat[:, :, C3 // 3:])
-            out = self.linear2(cat)
-        else:
-            out = self.linear2(torch.cat((attn, act(mlp)), 2))
-        return _gate_res(mod, x, out, gate)
-    forward.__jenga_b200__ = True
-    forward.__wrapped__ = orig
-    return forward
+def _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp,
+                   curve_sel, p_remain_rates, per_block_token, *, stat, tr, text_blocks, pad_ragged, ok):
+    norms = [_rms_params(n) for n in (self.q_norm, self.k_norm)]
+    if not (ok and freqs_cis is not None
+            and _carved_call(self, x, norms, sa_drop_rate, curve_sel, cu_seqlens_q, per_block_token)):
+        return None
+    (shift, scale, gate), (tr_mod, tr_gate) = _modulation(self.modulation, vec, 3, tr)
+    lin1 = self.linear1(_ln_mod(mod, self.pre_norm, x, shift, scale, tr=tr_mod))
+    C3 = 3 * self.hidden_size
+    L = x.shape[1] - txt_len
+    # strided views into linear1's output: no split / rearrange / cat copies (:413-441)
+    img_qkv, txt_qkv = lin1[:, :L, :C3], lin1[:, L:, :C3]
+    mlp = lin1[:, :, C3:]
+    assert cu_seqlens_q.shape[0] == 2 * x.shape[0] + 1                           # :444-446
+    # `torch.cat((attn, self.mlp_act(mlp)), 2)` (:499) without the concatenation copy: the attention
+    # kernel writes its rows into the first `hidden` columns of linear2's input buffer and the
+    # GELU kernel writes the rest
+    act = self.mlp_act
+    fuse_cat = (isinstance(act, torch.nn.GELU) and getattr(act, "approximate", "none") == "tanh"
+                and lin1.dtype == torch.bfloat16 and x.shape[0] == 1
+                and not getattr(self, "hybrid_seq_parallel_attn", None))
+    cat = attn_view = None
+    if fuse_cat:
+        cat = torch.empty((x.shape[0], x.shape[1], C3 // 3 + mlp.shape[-1]), dtype=lin1.dtype, device=lin1.device)
+        attn_view = cat[:, :, :C3 // 3].unflatten(2, (self.heads_num, -1))
+    attn = _attention_section(self, mod, img_qkv, txt_qkv, norms * 2, freqs_cis=freqs_cis, cu_seqlens_q=cu_seqlens_q,
+                              cu_seqlens_kv=cu_seqlens_kv, sa_drop_rate=sa_drop_rate, txt_amp=txt_amp,
+                              curve_sel=curve_sel, p_remain_rates=p_remain_rates, text_blocks=text_blocks,
+                              pad_ragged=pad_ragged, out=attn_view)
+    STATS[stat] += 1
+    if fuse_cat:
+        STATS["gelu_cat"] += 1
+        DN.gelu_tanh_into(mlp, cat[:, :, C3 // 3:])
+        out = self.linear2(cat)
+    else:
+        out = self.linear2(torch.cat((attn, act(mlp)), 2))
+    return _gate_res(mod, x, out, gate, tr=tr_gate)                              # :500
 
 
-# ------------------------------------------------------------------------------------------------
-# HunyuanVideo-I2V blocks
-# ------------------------------------------------------------------------------------------------
-def _i2v_eligible(self, x, sa_drop_rate, curve_sel, norms, per_block_token, cu_seqlens_q, S, tr, mask):
-    """the carved configuration the fused I2V forwards take; anything else runs the original"""
-    return (_carved_call(x, sa_drop_rate, curve_sel) and None not in norms and per_block_token == HY.BLOCK
-            and cu_seqlens_q is not None and x.shape[-1] // self.heads_num == 128
-            # sequence parallel: the reference runs the dense parallel_attention (:264-274, :483-493)
-            and not getattr(self, "hybrid_seq_parallel_attn", None)
-            # the prefix form (frist_frame_token_num) is only reached outside the Jenga forward
-            and not (tr and mask is None)
+def _hy_ok(self, S):
+    # the HunyuanVideo operator needs whole blocks; under sequence parallel the exchange takes any S
+    return bool(getattr(self, "hybrid_seq_parallel_attn", None)) or S % HY.BLOCK == 0
+
+
+def _hy_double(mod, self, img, txt, vec, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
+               max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, txt_amp=1.0, curve_sel=None,
+               p_remain_rates=0.5, txt_block_num=2, per_block_token=128):
+    return _double_stream(mod, self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp,
+                          curve_sel, p_remain_rates, per_block_token, stat="hy_double", tr=None,
+                          text_blocks=txt_block_num, pad_ragged=False,
+                          ok=_hy_ok(self, img.shape[1] + txt.shape[1]))
+
+
+def _hy_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
+               max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, txt_amp=1.0, curve_sel=None,
+               p_remain_rates=0.5, txt_block_num=2, per_block_token=128):
+    return _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp,
+                          curve_sel, p_remain_rates, per_block_token, stat="hy_single", tr=None,
+                          text_blocks=txt_block_num, pad_ragged=False, ok=_hy_ok(self, x.shape[1]))
+
+
+def _i2v_ok(self, S, condition_type, first_frame_mask):
+    # sequence parallel: the reference runs the dense parallel_attention (:264-274, :483-493); the
+    # prefix form of token replace (frist_frame_token_num) is only reached outside the Jenga forward;
+    # with text_blocks=4 the operator needs at least one image block
+    return (not getattr(self, "hybrid_seq_parallel_attn", None)
+            and not (condition_type == "token_replace" and first_frame_mask is None)
             and (S + HY.BLOCK - 1) // HY.BLOCK > _I2V_TEXT_BLOCKS)
 
 
-def _make_i2v_double_forward(orig, mod):
-    def forward(self, img, txt, vec, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
+def _i2v_tr(condition_type, token_replace_vec, first_frame_mask):
+    return (token_replace_vec, first_frame_mask) if condition_type == "token_replace" else None
+
+
+def _i2v_double(mod, self, img, txt, vec, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
                 max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, first_frame_mask=None,
                 condition_type=None, token_replace_vec=None, frist_frame_token_num=None, txt_amp=0.0,
                 curve_sel=None, p_remain_rates=0.5, per_block_token=128):
-        args = (img, txt, vec, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv, freqs_cis, sa_drop_rate,
-                first_frame_mask, condition_type, token_replace_vec, frist_frame_token_num, txt_amp, curve_sel,
-                p_remain_rates, per_block_token)
-        tr = condition_type == "token_replace"
-        norms = [_rms_params(n) for n in (self.img_attn_q_norm, self.img_attn_k_norm,
-                                          self.txt_attn_q_norm, self.txt_attn_k_norm)]
-        L = img.shape[1]
-        if not _i2v_eligible(self, img, sa_drop_rate, curve_sel, norms, per_block_token, cu_seqlens_q,
-                             L + txt.shape[1], tr, first_frame_mask):
-            STATS["fallback"] += 1
-            return orig(self, *args)
-        if tr:                                                                         # :156-179
-            img_mods, tr_mods = self.img_mod(vec, condition_type=condition_type, token_replace_vec=token_replace_vec)
-            i_shift1, i_scale1, i_gate1, i_shift2, i_scale2, i_gate2 = img_mods.chunk(6, dim=-1)
-            r_shift1, r_scale1, r_gate1, r_shift2, r_scale2, r_gate2 = tr_mods.chunk(6, dim=-1)
-            tr_mod1 = (r_shift1, r_scale1, first_frame_mask)
-            tr_mod2 = (r_shift2, r_scale2, first_frame_mask)
-            tr_gate1, tr_gate2 = (r_gate1, first_frame_mask), (r_gate2, first_frame_mask)
-        else:
-            i_shift1, i_scale1, i_gate1, i_shift2, i_scale2, i_gate2 = self.img_mod(vec).chunk(6, dim=-1)
-            tr_mod1 = tr_mod2 = tr_gate1 = tr_gate2 = None
-        t_shift1, t_scale1, t_gate1, t_shift2, t_scale2, t_gate2 = self.txt_mod(vec).chunk(6, dim=-1)
-        img_qkv = self.img_attn_qkv(_ln_mod(mod, self.img_norm1, img, i_shift1, i_scale1, tr=tr_mod1))
-        txt_qkv = self.txt_attn_qkv(_ln_mod(mod, self.txt_norm1, txt, t_shift1, t_scale1))
-        assert cu_seqlens_q.shape[0] == 2 * img.shape[0] + 1                         # :235-237
-        attn = _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis, cu_seqlens_q, cu_seqlens_kv,
-                                  sa_drop_rate, txt_amp, curve_sel, p_remain_rates, _I2V_TEXT_BLOCKS,
-                                  per_block_token, _I2V_TEXT_BLOCKS, pad_ragged=True)
-        STATS["i2v_double"] += 1
-        img_attn, txt_attn = attn[:, :L], attn[:, L:]
-        img = _gate_res(mod, img, self.img_attn_proj(img_attn), i_gate1, tr=tr_gate1)   # :281-306
-        img = _gate_res(mod, img, self.img_mlp(_ln_mod(mod, self.img_norm2, img, i_shift2, i_scale2, tr=tr_mod2)),
-                        i_gate2, tr=tr_gate2)
-        txt = _gate_res(mod, txt, self.txt_attn_proj(txt_attn), t_gate1)                 # :309-317
-        txt = _gate_res(mod, txt, self.txt_mlp(_ln_mod(mod, self.txt_norm2, txt, t_shift2, t_scale2)), t_gate2)
-        return img, txt
-    forward.__jenga_b200__ = True
-    forward.__wrapped__ = orig
-    return forward
+    return _double_stream(mod, self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp,
+                          curve_sel, p_remain_rates, per_block_token, stat="i2v_double",
+                          tr=_i2v_tr(condition_type, token_replace_vec, first_frame_mask),
+                          text_blocks=_I2V_TEXT_BLOCKS, pad_ragged=True,
+                          ok=_i2v_ok(self, img.shape[1] + txt.shape[1], condition_type, first_frame_mask))
 
 
-def _make_i2v_single_forward(orig, mod):
-    def forward(self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
+def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
                 max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, first_frame_mask=None,
                 condition_type=None, token_replace_vec=None, frist_frame_token_num=None, txt_amp=0.0,
                 curve_sel=None, p_remain_rates=0.5, per_block_token=128):
-        args = (x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, max_seqlen_q, max_seqlen_kv, freqs_cis, sa_drop_rate,
-                first_frame_mask, condition_type, token_replace_vec, frist_frame_token_num, txt_amp, curve_sel,
-                p_remain_rates, per_block_token)
-        tr = condition_type == "token_replace"
-        norms = [_rms_params(n) for n in (self.q_norm, self.k_norm)]
-        if (not _i2v_eligible(self, x, sa_drop_rate, curve_sel, norms, per_block_token, cu_seqlens_q, x.shape[1],
-                              tr, first_frame_mask)
-                or freqs_cis is None or not 0 < txt_len < x.shape[1]):
-            STATS["fallback"] += 1
-            return orig(self, *args)
-        if tr:                                                                         # :413-424
-            mods, tr_mods = self.modulation(vec, condition_type=condition_type, token_replace_vec=token_replace_vec)
-            shift, scale, gate = mods.chunk(3, dim=-1)
-            r_shift, r_scale, r_gate = tr_mods.chunk(3, dim=-1)
-            # full_first_frame_mask (jenga_hyi2v.py:129-130): a CPU bool over L+T rows
-            tr_mod, tr_gate = (r_shift, r_scale, first_frame_mask), (r_gate, first_frame_mask)
-        else:
-            shift, scale, gate = self.modulation(vec).chunk(3, dim=-1)
-            tr_mod = tr_gate = None
-        lin1 = self.linear1(_ln_mod(mod, self.pre_norm, x, shift, scale, tr=tr_mod))
-        C3 = 3 * self.hidden_size
-        L = x.shape[1] - txt_len
-        # strided views into linear1's output: no split / rearrange / cat copies (:431-451)
-        img_qkv, txt_qkv = lin1[:, :L, :C3], lin1[:, L:, :C3]
-        mlp = lin1[:, :, C3:]
-        assert cu_seqlens_q.shape[0] == 2 * x.shape[0] + 1                           # :464-466
-        # `torch.cat((attn, self.mlp_act(mlp)), 2)` (:497) without the concatenation copy, as in the
-        # HunyuanVideo single-stream forward above
-        act = self.mlp_act
-        fuse_cat = (isinstance(act, torch.nn.GELU) and getattr(act, "approximate", "none") == "tanh"
-                    and lin1.dtype == torch.bfloat16 and x.shape[0] == 1)
-        cat = attn_view = None
-        if fuse_cat:
-            cat = torch.empty((x.shape[0], x.shape[1], C3 // 3 + mlp.shape[-1]), dtype=lin1.dtype, device=lin1.device)
-            attn_view = cat[:, :, :C3 // 3].unflatten(2, (self.heads_num, -1))
-        attn = _attention_section(self, mod, img_qkv, txt_qkv, [norms[0], norms[1], norms[0], norms[1]],
-                                  freqs_cis, cu_seqlens_q, cu_seqlens_kv, sa_drop_rate, txt_amp, curve_sel,
-                                  p_remain_rates, _I2V_TEXT_BLOCKS, per_block_token, _I2V_TEXT_BLOCKS,
-                                  out=attn_view, pad_ragged=True)
-        STATS["i2v_single"] += 1
-        if fuse_cat:
-            STATS["gelu_cat"] += 1
-            DN.gelu_tanh_into(mlp, cat[:, :, C3 // 3:])
-            out = self.linear2(cat)
-        else:
-            out = self.linear2(torch.cat((attn, act(mlp)), 2))
-        return _gate_res(mod, x, out, gate, tr=tr_gate)                              # :499-505
-    forward.__jenga_b200__ = True
-    forward.__wrapped__ = orig
-    return forward
+    # first_frame_mask here is full_first_frame_mask (jenga_hyi2v.py:129-130): a CPU bool over L+T rows
+    return _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp,
+                          curve_sel, p_remain_rates, per_block_token, stat="i2v_single",
+                          tr=_i2v_tr(condition_type, token_replace_vec, first_frame_mask),
+                          text_blocks=_I2V_TEXT_BLOCKS, pad_ragged=True,
+                          ok=(_i2v_ok(self, x.shape[1], condition_type, first_frame_mask)
+                              and 0 < txt_len < x.shape[1]))
 
 
 # ------------------------------------------------------------------------------------------------
-# Wan self-attention
+# Wan blocks
 # ------------------------------------------------------------------------------------------------
-def _make_wan_forward(orig, mod):
-    def forward(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128,
-                p_remain_rates=0.8, freq_remap=None, block_neighbor_list=None):
-        b, s = x.shape[:2]
-        wq = getattr(self.norm_q, "weight", None)
-        wk = getattr(self.norm_k, "weight", None)
-        if (sa_drop_rate <= 0.25 or not x.is_cuda or b != 1 or self.head_dim != 128 or per_block_tokens != 128
-                or wq is None or wk is None or type(self.norm_q).__name__ != "WanRMSNorm"):
-            STATS["fallback"] += 1
-            return orig(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
-                        freq_remap, block_neighbor_list)
-        q_lin, k_lin = self.q(x), self.k(x)
-        if q_lin.dtype not in (torch.bfloat16, torch.float32):
-            STATS["fallback"] += 1
-            return orig(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
-                        freq_remap, block_neighbor_list)
-        v = self.v(x).view(b, s, self.num_heads, self.head_dim)
-        grid = [int(g) for g in grid_sizes[0].tolist()]
-        out = WAN.self_attention(q_lin, k_lin, v, wq, wk, self.num_heads, grid, freqs, sa_drop_rate,
-                                 p_remain_rates=p_remain_rates, freq_remap=freq_remap,
-                                 block_neighbor_list=block_neighbor_list, eps=float(self.norm_q.eps))
-        STATS["wan_self"] += 1
-        out = out.flatten(2)
-        if not torch.is_autocast_enabled():
-            # the reference returns the query dtype, fp32 (rope_apply -> .float(), model_mul.py:71;
-            # operator :530-532); under autocast the following Linear casts back to bf16 anyway
-            out = out.float()
-        return self.o(out)
-    forward.__jenga_b200__ = True
-    forward.__wrapped__ = orig
-    return forward
+def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128, p_remain_rates=0.8,
+              freq_remap=None, block_neighbor_list=None):
+    b, s = x.shape[:2]
+    wq = getattr(self.norm_q, "weight", None)
+    wk = getattr(self.norm_k, "weight", None)
+    if (sa_drop_rate <= 0.25 or not x.is_cuda or b != 1 or self.head_dim != 128 or per_block_tokens != 128
+            or wq is None or wk is None or type(self.norm_q).__name__ != "WanRMSNorm"):
+        return None
+    q_lin, k_lin = self.q(x), self.k(x)
+    if q_lin.dtype not in (torch.bfloat16, torch.float32):
+        return None
+    v = self.v(x).view(b, s, self.num_heads, self.head_dim)
+    grid = [int(g) for g in grid_sizes[0].tolist()]
+    out = WAN.self_attention(q_lin, k_lin, v, wq, wk, self.num_heads, grid, freqs, sa_drop_rate,
+                             p_remain_rates=p_remain_rates, freq_remap=freq_remap,
+                             block_neighbor_list=block_neighbor_list, eps=float(self.norm_q.eps))
+    STATS["wan_self"] += 1
+    out = out.flatten(2)
+    if not torch.is_autocast_enabled():
+        # the reference returns the query dtype, fp32 (rope_apply -> .float(), model_mul.py:71;
+        # operator :530-532); under autocast the following Linear casts back to bf16 anyway
+        out = out.float()
+    return self.o(out)
 
 
-def _make_wan_cross_forward(orig, mod):
-    def forward(self, x, context, context_lens):
-        wq = getattr(self.norm_q, "weight", None)
-        wk = getattr(self.norm_k, "weight", None)
-        # context_lens: the reference's varlen form (wan/modules/attention.py:69-80); teacache_forward
-        # passes None (jenga_wan.py:569)
-        if (context_lens is not None or not x.is_cuda or x.dim() != 3 or x.shape[0] != 1 or context.dim() != 3
-                or context.shape[0] != 1 or self.head_dim != 128 or wq is None or wk is None
-                or type(self.norm_q).__name__ != "WanRMSNorm" or type(self.norm_k).__name__ != "WanRMSNorm"
-                or not DN._autocast_bf16()):
-            STATS["fallback"] += 1
-            return orig(self, x, context, context_lens)
-        q_lin, k_lin, v = self.q(x), self.k(context), self.v(context)
-        if (q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype not in (torch.bfloat16, torch.float32)
-                or v.dtype != torch.bfloat16):
-            STATS["fallback"] += 1
-            return orig(self, x, context, context_lens)
-        out = WAN.cross_attention(q_lin, k_lin, v.view(1, -1, self.num_heads, self.head_dim), wq, wk,
-                                  self.num_heads, eps=float(self.norm_q.eps))
-        STATS["wan_cross"] += 1
-        return self.o(out.flatten(2))
-    forward.__jenga_b200__ = True
-    forward.__wrapped__ = orig
-    return forward
+def _wan_cross(self, x, context, context_lens):
+    wq = getattr(self.norm_q, "weight", None)
+    wk = getattr(self.norm_k, "weight", None)
+    # context_lens: the reference's varlen form (wan/modules/attention.py:69-80); teacache_forward
+    # passes None (jenga_wan.py:569)
+    if (context_lens is not None or not x.is_cuda or x.dim() != 3 or x.shape[0] != 1 or context.dim() != 3
+            or context.shape[0] != 1 or self.head_dim != 128 or wq is None or wk is None
+            or type(self.norm_q).__name__ != "WanRMSNorm" or type(self.norm_k).__name__ != "WanRMSNorm"
+            or not DN._autocast_bf16()):
+        return None
+    q_lin, k_lin, v = self.q(x), self.k(context), self.v(context)
+    if (q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype not in (torch.bfloat16, torch.float32)
+            or v.dtype != torch.bfloat16):
+        return None
+    out = WAN.cross_attention(q_lin, k_lin, v.view(1, -1, self.num_heads, self.head_dim), wq, wk,
+                              self.num_heads, eps=float(self.norm_q.eps))
+    STATS["wan_cross"] += 1
+    return self.o(out.flatten(2))
 
 
 def _wan_i2v_cross_shape_ok(ca, x, context, context_lens):
@@ -444,39 +371,48 @@ def _wan_i2v_cross(ca, x, context, context_lens):
     return ca(x, context, context_lens)
 
 
-def _make_wan_block_forward(orig, mod):
-    def forward(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=0.0, freq_remap=None,
-                block_neighbor_list=None, p_remain_rates=0.0):
-        args = (x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate, freq_remap,
-                block_neighbor_list, p_remain_rates)
-        i2v = type(self.cross_attn).__name__ == "WanI2VCrossAttention"
-        ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
-              and (i2v or type(self.cross_attn).__name__ == "WanT2VCrossAttention")
-              and self.modulation.dtype == torch.float32)
-        if ok:
-            with torch.autocast("cuda", dtype=torch.float32):                      # :326-327
-                e6 = self.modulation + e
-            ok = (DN.wan_ln_modulate_supported(x, self.norm1, e6)
-                  and DN.wan_residual_ln_supported(x, self.norm3, e6, affine=True)
-                  and DN.wan_residual_ln_supported(x, self.norm2, e6, affine=False)
-                  and DN.wan_gate_residual_supported(x, e6))
-        if not ok:
-            # no autocast, batch > 1, cross_attn_norm=False (norm3 is Identity), …
+def _wan_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=0.0, freq_remap=None,
+               block_neighbor_list=None, p_remain_rates=0.0):
+    i2v = type(self.cross_attn).__name__ == "WanI2VCrossAttention"
+    ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
+          and (i2v or type(self.cross_attn).__name__ == "WanT2VCrossAttention")
+          and self.modulation.dtype == torch.float32)
+    if ok:
+        with torch.autocast("cuda", dtype=torch.float32):                      # :326-327
+            e6 = self.modulation + e
+        ok = (DN.wan_ln_modulate_supported(x, self.norm1, e6)
+              and DN.wan_residual_ln_supported(x, self.norm3, e6, affine=True)
+              and DN.wan_residual_ln_supported(x, self.norm2, e6, affine=False)
+              and DN.wan_gate_residual_supported(x, e6))
+    if not ok:
+        return None                     # no autocast, batch > 1, cross_attn_norm=False (norm3 is Identity), …
+    e = e6.chunk(6, dim=1)
+    # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to
+    y = self.self_attn(DN.wan_ln_modulate(x, e[0], e[1], eps=self.norm1.eps), seq_lens, grid_sizes, freqs,
+                       sa_drop_rate=sa_drop_rate, freq_remap=freq_remap, block_neighbor_list=block_neighbor_list,
+                       p_remain_rates=p_remain_rates)                          # :331-333
+    x, h = DN.wan_residual_ln(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight,
+                              bias=self.norm3.bias)                            # :334-335, :339
+    # WanI2VCrossAttention.forward itself stays unpatched: the block routes it here
+    cross = _wan_i2v_cross(self.cross_attn, h, context, context_lens) if i2v else \
+        self.cross_attn(h, context, context_lens)
+    x, h = DN.wan_residual_ln(x, cross, None, eps=self.norm2.eps, shift=e[3], scale=e[4])   # :339-340
+    STATS["wan_block"] += 1
+    return DN.wan_gate_residual(x, self.ffn(h), e[5])                          # :340-342
+
+
+# ------------------------------------------------------------------------------------------------
+# patching
+# ------------------------------------------------------------------------------------------------
+def _patched(orig, fused):
+    """The patched forward: `fused` takes the reference arguments and returns None for a call it does
+    not take; that call then runs `orig` with exactly the caller's arguments."""
+    def forward(self, *args, **kwargs):
+        out = fused(self, *args, **kwargs)
+        if out is None:
             STATS["fallback"] += 1
-            return orig(self, *args)
-        e = e6.chunk(6, dim=1)
-        # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to
-        y = self.self_attn(DN.wan_ln_modulate(x, e[0], e[1], eps=self.norm1.eps), seq_lens, grid_sizes, freqs,
-                           sa_drop_rate=sa_drop_rate, freq_remap=freq_remap, block_neighbor_list=block_neighbor_list,
-                           p_remain_rates=p_remain_rates)                          # :331-333
-        x, h = DN.wan_residual_ln(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight,
-                                  bias=self.norm3.bias)                            # :334-335, :339
-        # WanI2VCrossAttention.forward itself stays unpatched: the block routes it here
-        cross = _wan_i2v_cross(self.cross_attn, h, context, context_lens) if i2v else \
-            self.cross_attn(h, context, context_lens)
-        x, h = DN.wan_residual_ln(x, cross, None, eps=self.norm2.eps, shift=e[3], scale=e[4])   # :339-340
-        STATS["wan_block"] += 1
-        return DN.wan_gate_residual(x, self.ffn(h), e[5])                          # :340-342
+            out = orig(self, *args, **kwargs)
+        return out
     forward.__jenga_b200__ = True
     forward.__wrapped__ = orig
     return forward
@@ -484,29 +420,21 @@ def _make_wan_block_forward(orig, mod):
 
 def patch_module(mod) -> list[str]:
     """Patches the block classes of an already imported reference module; returns what it did."""
-    done = []
     name = mod.__name__
-    # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
-    # a ragged S with four text blocks: its own pair of forwards
-    i2v = name.startswith("hyvideo_i2v.")
-    if ((name.startswith("hyvideo.") or i2v) and hasattr(mod, "MMDoubleStreamBlock")
-            and not getattr(mod.MMDoubleStreamBlock.forward, "__jenga_b200__", False)):
-        if i2v:
-            mod.MMDoubleStreamBlock.forward = _make_i2v_double_forward(mod.MMDoubleStreamBlock.forward, mod)
-            mod.MMSingleStreamBlock.forward = _make_i2v_single_forward(mod.MMSingleStreamBlock.forward, mod)
-        else:
-            mod.MMDoubleStreamBlock.forward = _make_double_forward(mod.MMDoubleStreamBlock.forward, mod, 2)
-            mod.MMSingleStreamBlock.forward = _make_single_forward(mod.MMSingleStreamBlock.forward, mod, 2)
-        done += [f"{name}.MMDoubleStreamBlock.forward", f"{name}.MMSingleStreamBlock.forward"]
-    if hasattr(mod, "WanSelfAttention") and not getattr(mod.WanSelfAttention.forward, "__jenga_b200__", False):
-        orig = mod.WanSelfAttention.forward
-        mod.WanSelfAttention.forward = _make_wan_forward(orig, mod)
-        done.append(f"{name}.WanSelfAttention.forward")
+    fused = {}
+    if name.startswith(("hyvideo.", "hyvideo_i2v.")):
+        # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
+        # a ragged S with four text blocks: its own pair of entry points
+        i2v = name.startswith("hyvideo_i2v.")
+        fused["MMDoubleStreamBlock"] = functools.partial(_i2v_double if i2v else _hy_double, mod)
+        fused["MMSingleStreamBlock"] = functools.partial(_i2v_single if i2v else _hy_single, mod)
     # WanI2VCrossAttention overrides forward itself and is left as it is; the fused block forward runs
     # its fused form (_wan_i2v_cross)
-    for cls, make in (("WanT2VCrossAttention", _make_wan_cross_forward), ("WanAttentionBlock", _make_wan_block_forward)):
+    fused.update(WanSelfAttention=_wan_self, WanT2VCrossAttention=_wan_cross, WanAttentionBlock=_wan_block)
+    done = []
+    for cls, body in fused.items():
         if hasattr(mod, cls) and not getattr(getattr(mod, cls).forward, "__jenga_b200__", False):
-            getattr(mod, cls).forward = make(getattr(mod, cls).forward, mod)
+            getattr(mod, cls).forward = _patched(getattr(mod, cls).forward, body)
             done.append(f"{name}.{cls}.forward")
     return done
 
