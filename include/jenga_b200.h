@@ -25,6 +25,8 @@
 extern "C" {
 #endif
 
+/* The version changes when an existing struct layout or signature changes; entry points that are only
+ * added (the FP8 Linear ones below, jenga_wan_i2v_cross_attn) keep it, so older callers stay valid. */
 #define JENGA_B200_ABI_VERSION 3
 
 enum {
@@ -376,6 +378,51 @@ int jenga_ln_modulate_tr(const void* x, int64_t x_stride, const void* scale, con
 int jenga_gate_residual_tr(const void* x, int64_t x_stride, const void* y, int64_t y_stride, const void* gate,
                            const void* tr_gate, const uint8_t* row_is_tr, void* out, int64_t out_stride,
                            int64_t rows, int32_t channels, void* stream);
+
+/* ----------------------------------------------------------------------------------------
+ * (f-1, opt-in) W8A8 FP8 Linear: e4m3 activations with one scale per row, e4m3 weights with one
+ * scale per output channel or per tensor, fp32 accumulation promoted every 128 channels of K.
+ *
+ * jenga_quantize_rows_fp8: scale[m] = amax(|x[m, :]|) / 448 (1 for an all-zero row),
+ *   out[m, k] = e4m3_rn_satfinite(x[m, k] / scale[m]).  x bf16 rows of `cols` elements, `x_stride`
+ *   elements apart (multiple of 8); out rows `out_stride` bytes apart (multiple of 16); cols % 16 == 0
+ *   (JENGA_E_UNSUPPORTED otherwise).  Also quantises bf16 nn.Linear weights per output channel.
+ * jenga_ln_modulate_fp8 / jenga_ln_modulate_tr_fp8: jenga_ln_modulate / _tr followed by
+ *   jenga_quantize_rows_fp8 of its bf16 rows, in one pass (bit-identical to the two calls); out8 rows
+ *   `out_stride` bytes apart (multiple of 16), a_scale [rows] f32.  Same validation as the bf16 forms,
+ *   plus channels % 16 == 0.
+ * jenga_linear_fp8: out[m, n] = bf16( sum_k a[m, k] w[n, k] * a_scale[m] * w_scale[n * w_scale_stride]
+ *   + bias[n] ).  a: e4m3 [m, k], rows `a_stride` bytes apart (multiple of 16); w: contiguous e4m3
+ *   [n, k] (the nn.Linear layout); w_scale_stride 1 (per channel) or 0 (per tensor); bias bf16 or f32
+ *   (bias_dtype) or NULL; out bf16 rows `out_stride` elements apart (multiple of 8).  k % 16 == 0 and
+ *   n % 8 == 0, JENGA_E_UNSUPPORTED otherwise; any m.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct JengaLinearFp8Args {
+  const void* a;
+  int64_t a_stride;       /* bytes */
+  const float* a_scale;   /* [m] */
+  const void* w;
+  const float* w_scale;
+  int32_t w_scale_stride; /* 1: [n] per output channel; 0: one value */
+  const void* bias;       /* [n] or NULL */
+  int32_t bias_dtype;     /* JENGA_BF16 or JENGA_F32 */
+  void* out;
+  int64_t out_stride;     /* elements */
+  int64_t m;
+  int32_t n;
+  int32_t k;
+} JengaLinearFp8Args;
+
+int jenga_quantize_rows_fp8(const void* x, int64_t x_stride, int64_t rows, int32_t cols, void* out,
+                            int64_t out_stride, float* scale, void* stream);
+int jenga_ln_modulate_fp8(const void* x, int64_t x_stride, const void* scale, const void* shift, void* out8,
+                          int64_t out_stride, float* a_scale, int64_t rows, int32_t channels, float eps,
+                          void* stream);
+int jenga_ln_modulate_tr_fp8(const void* x, int64_t x_stride, const void* scale, const void* shift,
+                             const void* tr_scale, const void* tr_shift, const uint8_t* row_is_tr, void* out8,
+                             int64_t out_stride, float* a_scale, int64_t rows, int32_t channels, float eps,
+                             void* stream);
+int jenga_linear_fp8(const JengaLinearFp8Args* args, void* stream);
 
 /* Wan2.1 forms (wan/modules/model_mul.py:303-346 WanAttentionBlock.forward under
  * torch.autocast(bf16)).  The residual stream is fp32 after block 0; parameter vectors (scale, shift,

@@ -119,6 +119,14 @@ class JengaWanCrossArgs(C.Structure):
     ]
 
 
+class JengaLinearFp8Args(C.Structure):
+    _fields_ = [
+        ("a", C.c_void_p), ("a_stride", C.c_int64), ("a_scale", C.c_void_p), ("w", C.c_void_p),
+        ("w_scale", C.c_void_p), ("w_scale_stride", C.c_int32), ("bias", C.c_void_p), ("bias_dtype", C.c_int32),
+        ("out", C.c_void_p), ("out_stride", C.c_int64), ("m", C.c_int64), ("n", C.c_int32), ("k", C.c_int32),
+    ]
+
+
 class JengaTeaCacheArgs(C.Structure):
     _fields_ = [
         ("cur", C.c_void_p), ("prev", C.c_void_p), ("dtype", C.c_int32), ("n", C.c_int64),
@@ -226,6 +234,18 @@ def _load() -> C.CDLL:
     lib.jenga_carved_attn_sched_workspace_bytes.restype = C.c_int64
     lib.jenga_wan_i2v_cross_attn.argtypes = [C.POINTER(JengaWanCrossArgs), C.c_void_p]
     lib.jenga_wan_i2v_cross_attn.restype = C.c_int
+    lib.jenga_quantize_rows_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
+                                            C.c_void_p, C.c_void_p]
+    lib.jenga_quantize_rows_fp8.restype = C.c_int
+    lib.jenga_ln_modulate_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_void_p]
+    lib.jenga_ln_modulate_fp8.restype = C.c_int
+    lib.jenga_ln_modulate_tr_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32,
+                                             C.c_float, C.c_void_p]
+    lib.jenga_ln_modulate_tr_fp8.restype = C.c_int
+    lib.jenga_linear_fp8.argtypes = [C.POINTER(JengaLinearFp8Args), C.c_void_p]
+    lib.jenga_linear_fp8.restype = C.c_int
     lib.jenga_gilbert_xyz2d.argtypes = [C.c_int] * 6
     lib.jenga_gilbert_xyz2d.restype = C.c_int64
     if lib.jenga_abi_version() != 3:

@@ -60,7 +60,7 @@ _I2V_MODULES = ("hyvideo_i2v.modules.models_mul",)
 _WAN_MODULES = ("wan.modules.model_mul",)
 STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "wan_self": 0, "fallback": 0,
          "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0,
-         "wan_i2v_cross": 0}
+         "wan_i2v_cross": 0, "linear_fp8": 0}
 # the CLIP image tokens at the head of the Wan2.1-I2V context (model_mul.py:230-231)
 _WAN_I2V_IMG_TOKENS = 257
 # the HunyuanVideo-I2V operator's text_blocks default (hyvideo_i2v/…/attention_block_triton_diffres.py:409);
@@ -108,6 +108,60 @@ def _gate_res(mod, x, y, gate, tr=None):
     if tr is None:
         return x + mod.apply_gate(y, gate=gate)
     return x + mod.apply_gate(y, gate=gate, condition_type="token_replace", tr_gate=tr[0], first_frame_mask=tr[1])
+
+
+def _fp8_weight(layer, x):
+    """DN.fp8_weight(layer) when the opt-in FP8 Linears (DN.LINEAR_FP8) take `layer` on input x — a
+    bf16 CUDA tensor with 16-byte aligned rows of the layer's K, and a shape in DN.FP8_ROUTED — else None"""
+    if not (DN.LINEAR_FP8 and DN.FP8_ROUTED and isinstance(x, torch.Tensor) and x.is_cuda
+            and x.dtype == torch.bfloat16 and x.dim() >= 2 and x.stride(-1) == 1 and x.stride(-2) % 8 == 0
+            and x.data_ptr() % 16 == 0 and isinstance(layer, torch.nn.Module)):
+        return None
+    w = DN.fp8_weight(layer)
+    if w is None or w[0].shape[1] != x.shape[-1]:
+        return None
+    return w if (DN.fp8_weight_kind(layer), *w[0].shape[::-1]) in DN.FP8_ROUTED else None
+
+
+def _linear(layer, x, x8=None):
+    """layer(x), or with the FP8 Linears on, one jenga_linear_fp8 launch on the e4m3 rows of x.
+    x8: (codes, a_scale) of x made by the caller (ln_modulate_fp8), which has checked _fp8_weight."""
+    w = _fp8_weight(layer, x)
+    if w is None:
+        return layer(x)
+    if x8 is None:
+        try:
+            x8 = DN.quantize_rows_fp8(x)
+        except ValueError:                   # rows that are not uniformly strided
+            return layer(x)
+    STATS["linear_fp8"] += 1
+    return DN.linear_fp8(*x8, *w).view(*x.shape[:-1], w[0].shape[0])
+
+
+def _mod_linear(mod, layer, norm, x, shift, scale, tr=None):
+    """layer(_ln_mod(...)); with the FP8 Linears on, the modulated rows go straight to e4m3
+    (ln_modulate_fp8) and are never written in bf16"""
+    if (_fp8_weight(layer, x) is not None and x.shape[-1] % 16 == 0
+            and DN.ln_modulate_supported(x, norm, shift, scale, tr=tr)):
+        STATS["ln_modulate"] += 1
+        return _linear(layer, x, DN.ln_modulate_fp8(x, shift, scale, eps=norm.eps, tr=tr))
+    return _linear(layer, _ln_mod(mod, norm, x, shift, scale, tr=tr))
+
+
+def _plain_mlp(mlp) -> bool:
+    """the reference MLP (hyvideo/modules/mlp_layers.py:13-58) with tanh-GELU, no norm and no dropout"""
+    act, norm, d1, d2 = (getattr(mlp, n, None) for n in ("act", "norm", "drop1", "drop2"))
+    return (type(mlp).__name__ == "MLP" and all(hasattr(mlp, n) for n in ("fc1", "fc2"))
+            and "forward" not in mlp.__dict__ and not mlp._forward_hooks and not mlp._forward_pre_hooks
+            and isinstance(act, torch.nn.GELU) and act.approximate == "tanh" and isinstance(norm, torch.nn.Identity)
+            and all(isinstance(d, torch.nn.Dropout) and d.p == 0.0 for d in (d1, d2)))
+
+
+def _mlp(mod, mlp, norm, x, shift, scale, tr=None):
+    """mlp(_ln_mod(...)); with the FP8 Linears on, a plain MLP is opened into fc1 -> act -> fc2"""
+    if DN.LINEAR_FP8 and DN.FP8_ROUTED and _plain_mlp(mlp):
+        return _linear(mlp.fc2, mlp.act(_mod_linear(mod, mlp.fc1, norm, x, shift, scale, tr=tr)))
+    return mlp(_ln_mod(mod, norm, x, shift, scale, tr=tr))
 
 
 def _modulation(layer, vec, n, tr):
@@ -168,7 +222,7 @@ def _double_stream(mod, self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, freqs_
     (i_shift1, i_scale1, i_gate1, i_shift2, i_scale2, i_gate2), (tr_mod1, tr_gate1, tr_mod2, tr_gate2) = \
         _modulation(self.img_mod, vec, 6, tr)
     t_shift1, t_scale1, t_gate1, t_shift2, t_scale2, t_gate2 = self.txt_mod(vec).chunk(6, dim=-1)
-    img_qkv = self.img_attn_qkv(_ln_mod(mod, self.img_norm1, img, i_shift1, i_scale1, tr=tr_mod1))
+    img_qkv = _mod_linear(mod, self.img_attn_qkv, self.img_norm1, img, i_shift1, i_scale1, tr=tr_mod1)
     txt_qkv = self.txt_attn_qkv(_ln_mod(mod, self.txt_norm1, txt, t_shift1, t_scale1))
     assert cu_seqlens_q.shape[0] == 2 * img.shape[0] + 1                         # :244-246
     attn = _attention_section(self, mod, img_qkv, txt_qkv, norms, freqs_cis=freqs_cis, cu_seqlens_q=cu_seqlens_q,
@@ -178,8 +232,8 @@ def _double_stream(mod, self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, freqs_
     STATS[stat] += 1
     L = img.shape[1]
     img_attn, txt_attn = attn[:, :L], attn[:, L:]
-    img = _gate_res(mod, img, self.img_attn_proj(img_attn), i_gate1, tr=tr_gate1)   # :297-305
-    img = _gate_res(mod, img, self.img_mlp(_ln_mod(mod, self.img_norm2, img, i_shift2, i_scale2, tr=tr_mod2)),
+    img = _gate_res(mod, img, _linear(self.img_attn_proj, img_attn), i_gate1, tr=tr_gate1)   # :297-305
+    img = _gate_res(mod, img, _mlp(mod, self.img_mlp, self.img_norm2, img, i_shift2, i_scale2, tr=tr_mod2),
                     i_gate2, tr=tr_gate2)
     txt = _gate_res(mod, txt, self.txt_attn_proj(txt_attn), t_gate1)                 # :307-315
     txt = _gate_res(mod, txt, self.txt_mlp(_ln_mod(mod, self.txt_norm2, txt, t_shift2, t_scale2)), t_gate2)
@@ -193,7 +247,7 @@ def _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freq
             and _carved_call(self, x, norms, sa_drop_rate, curve_sel, cu_seqlens_q, per_block_token)):
         return None
     (shift, scale, gate), (tr_mod, tr_gate) = _modulation(self.modulation, vec, 3, tr)
-    lin1 = self.linear1(_ln_mod(mod, self.pre_norm, x, shift, scale, tr=tr_mod))
+    lin1 = _mod_linear(mod, self.linear1, self.pre_norm, x, shift, scale, tr=tr_mod)
     C3 = 3 * self.hidden_size
     L = x.shape[1] - txt_len
     # strided views into linear1's output: no split / rearrange / cat copies (:413-441)
@@ -219,9 +273,9 @@ def _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freq
     if fuse_cat:
         STATS["gelu_cat"] += 1
         DN.gelu_tanh_into(mlp, cat[:, :, C3 // 3:])
-        out = self.linear2(cat)
+        out = _linear(self.linear2, cat)
     else:
-        out = self.linear2(torch.cat((attn, act(mlp)), 2))
+        out = _linear(self.linear2, torch.cat((attn, act(mlp)), 2))
     return _gate_res(mod, x, out, gate, tr=tr_gate)                              # :500
 
 

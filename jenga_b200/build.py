@@ -20,7 +20,7 @@ OUT_DIR = PKG / "_C"
 LIB = OUT_DIR / "libjenga_b200.so"
 STAMP = OUT_DIR / "build.stamp"
 
-CU_SOURCES = ["api.cu", "carved_attn.cu", "prologue.cu", "prologue_bulk.cu", "select.cu", "stepcache.cu", "dense_fused.cu", "gilbert_device.cu", "fp8.cu", "qk_int8.cu", "wan_cross_attn.cu"]
+CU_SOURCES = ["api.cu", "carved_attn.cu", "prologue.cu", "prologue_bulk.cu", "select.cu", "stepcache.cu", "dense_fused.cu", "gilbert_device.cu", "fp8.cu", "qk_int8.cu", "wan_cross_attn.cu", "linear_fp8.cu"]
 CXX_SOURCES = ["gilbert.cpp"]
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -94,6 +94,14 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes "
+      "[%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+
 // ---------------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA, sm_90a).  All four warps of a warpgroup execute these together.
 // ---------------------------------------------------------------------------------------------
@@ -151,6 +159,12 @@ __device__ __forceinline__ void wgmma_128_rs_bmn(float (&d)[64], const uint32_t 
 __device__ __forceinline__ void wgmma_128_rs_e4m3(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc,
                                                   uint32_t scale_d) {
   JENGA_WGMMA_RS("m64n128k32", "e4m3", "");
+}
+// D[64x128 f32, registers] (+)= A[smem, K-major] * B[smem, K-major], K = 32, e4m3 x e4m3
+__device__ __forceinline__ void wgmma_128_ss_e4m3(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 " JENGA_WGMMA_D64 ", %64, %65, p, 1, 1;\n\t}\n"
+               : JENGA_WGMMA_OUT64 : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
 // D[64x128 s32, registers] (+)= A[smem, K-major] * B[smem, K-major], K = 32, s8 x s8 (exact integer sums)
 __device__ __forceinline__ void wgmma_128_ss_s8(int32_t (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {

@@ -281,3 +281,145 @@ def wan_gate_residual(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor) -> t
         check(lib.jenga_wan_gate_residual(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys, g.data_ptr(), out.data_ptr(),
                                           C, rows, C, _stream_ptr(x.device)), "wan_gate_residual")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Opt-in FP8 Linears (csrc/linear_fp8.cu): `jenga_b200.dense.LINEAR_FP8 = True` or JENGA_LINEAR_FP8=1.
+# W8A8 e4m3 with one scale per activation row and per weight output channel (or per tensor for the
+# reference's --use-fp8 checkpoints); fp32 accumulation.  Its own tolerance row (tests/test_linear_fp8_gpu.py).
+# ------------------------------------------------------------------------------------------------
+import os as _os
+
+LINEAR_FP8: bool = _os.environ.get("JENGA_LINEAR_FP8", "0") == "1"
+# (weight kind, K, N) of the block Linears the switch routes: only those where quantisation + FP8 GEMM
+# measured faster than the call it replaces (bench_linear_fp8.py; kind "bf16" against bf16 F.linear,
+# "fp8_ref" against the reference's --use-fp8 forward).  On an H100 80GB at 700 W none of the six
+# HunyuanVideo image-row shapes did (README, "Opt-in FP8 Linears"), so the switch routes nothing yet.
+FP8_ROUTED: frozenset = frozenset()
+
+
+def linear_fp8_shape_ok(k: int, n: int) -> bool:
+    """the GEMM's shape rules: K % 16 == 0 and N % 8 == 0 (any M)"""
+    return k > 0 and n > 0 and k % 16 == 0 and n % 8 == 0
+
+
+def quantize_rows_fp8(x: torch.Tensor):
+    """x [..., K] bf16 (uniformly strided rows) -> (codes float8_e4m3fn [rows, K], scale fp32 [rows]):
+    scale = amax(row) / 448 (1 for a zero row), codes = e4m3_rn_satfinite(x / scale)."""
+    _require_cuda(x)
+    if x.dtype != torch.bfloat16:
+        raise ValueError("x must be bf16")
+    rows, xs = _rows2d(x)
+    K = x.shape[-1]
+    out = torch.empty((rows, K), dtype=torch.float8_e4m3fn, device=x.device)
+    scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.jenga_quantize_rows_fp8(x.data_ptr(), xs, rows, K, out.data_ptr(), K, scale.data_ptr(),
+                                          _stream_ptr(x.device)), "quantize_rows_fp8")
+    return out, scale
+
+
+def ln_modulate_fp8(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6, tr=None):
+    """`quantize_rows_fp8(ln_modulate(x, shift, scale, eps, tr))` in one pass, bit for bit; the bf16 rows
+    are never written.  Returns (codes float8_e4m3fn [L, C], a_scale fp32 [L])."""
+    _require_cuda(x, shift, scale)
+    rows, xs = _rows2d(x)
+    C = x.shape[-1]
+    out = torch.empty((rows, C), dtype=torch.float8_e4m3fn, device=x.device)
+    a_scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
+    sc, sh = _per_channel(scale, C, "scale"), _per_channel(shift, C, "shift")
+    with torch.cuda.device(x.device):
+        if tr is None:
+            check(lib.jenga_ln_modulate_fp8(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(), C,
+                                            a_scale.data_ptr(), rows, C, float(eps), _stream_ptr(x.device)),
+                  "ln_modulate_fp8")
+            return out, a_scale
+        tr_shift, tr_scale, mask = tr
+        _require_cuda(tr_shift, tr_scale)
+        tsc, tsh = _per_channel(tr_scale, C, "tr_scale"), _per_channel(tr_shift, C, "tr_shift")
+        if mask.dim() != 1 or mask.numel() != rows:
+            raise ValueError("row mask must hold one entry per row")
+        m = _row_mask(mask, x.device)
+        check(lib.jenga_ln_modulate_tr_fp8(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), tsc.data_ptr(),
+                                           tsh.data_ptr(), m.data_ptr(), out.data_ptr(), C, a_scale.data_ptr(), rows,
+                                           C, float(eps), _stream_ptr(x.device)), "ln_modulate_tr_fp8")
+    return out, a_scale
+
+
+def linear_fp8(x8: torch.Tensor, a_scale: torch.Tensor, w8: torch.Tensor, w_scale: torch.Tensor,
+               bias: torch.Tensor | None = None) -> torch.Tensor:
+    """bf16( (x8 . w8^T) * a_scale[m] * w_scale[n] + bias[n] ), fp32 accumulation.
+    x8 e4m3 [M, K] (rows may be strided), a_scale fp32 [M], w8 e4m3 [N, K] contiguous, w_scale fp32 [N]
+    or one value (per tensor), bias bf16 / fp32 [N] or None -> bf16 [M, N]."""
+    _require_cuda(x8, a_scale, w8, w_scale)
+    if x8.dtype != torch.float8_e4m3fn or w8.dtype != torch.float8_e4m3fn:
+        raise ValueError("x8 / w8 must be float8_e4m3fn")
+    if a_scale.dtype != torch.float32 or w_scale.dtype != torch.float32:
+        raise ValueError("scales must be fp32")
+    if x8.dim() != 2 or w8.dim() != 2 or x8.stride(-1) != 1 or not w8.is_contiguous():
+        raise ValueError("x8 must be [M, K] with contiguous rows and w8 a contiguous [N, K]")
+    M, K = x8.shape
+    N = w8.shape[0]
+    if w8.shape[1] != K or a_scale.numel() != M or w_scale.numel() not in (1, N):
+        raise ValueError("shape mismatch")
+    a_scale, w_scale = a_scale.contiguous(), w_scale.contiguous()
+    codes = {torch.bfloat16: _lib.JENGA_BF16, torch.float32: _lib.JENGA_F32}
+    if bias is not None:
+        _require_cuda(bias)
+        if bias.dtype not in codes or bias.numel() != N:
+            raise ValueError("bias must be bf16 or fp32 with N values")
+        bias = bias.contiguous()
+    out = torch.empty((M, N), dtype=torch.bfloat16, device=x8.device)
+    args = _lib.JengaLinearFp8Args(
+        a=x8.data_ptr(), a_stride=x8.stride(0), a_scale=a_scale.data_ptr(), w=w8.data_ptr(),
+        w_scale=w_scale.data_ptr(), w_scale_stride=1 if w_scale.numel() == N and N > 1 else 0,
+        bias=bias.data_ptr() if bias is not None else None,
+        bias_dtype=codes[bias.dtype] if bias is not None else _lib.JENGA_BF16,
+        out=out.data_ptr(), out_stride=N, m=M, n=N, k=K)
+    with torch.cuda.device(x8.device):
+        check(lib.jenga_linear_fp8(_lib.C.byref(args), _stream_ptr(x8.device)), "linear_fp8")
+    return out
+
+
+def fp8_weight_kind(layer: torch.nn.Module) -> str:
+    """the FP8_ROUTED kind of a layer fp8_weight takes: "fp8_ref" for a --use-fp8 layer, else "bf16"
+    """
+    return "fp8_ref" if layer.weight.dtype == torch.float8_e4m3fn else "bf16"
+
+
+def fp8_weight(layer: torch.nn.Module):
+    """(w8 e4m3 [N, K], w_scale fp32, bias) of an nn.Linear, or None when the layer is not one the FP8
+    path takes.  A bf16 weight is quantised once per output channel (w_scale[n] = amax / 448) and the
+    result is cached on the module, keyed on the weight's data_ptr and _version (one extra byte per
+    parameter).  A reference --use-fp8 layer (e4m3 weight and `fp8_scale`, hyvideo/modules/
+    fp8_optimization.py:convert_fp8_linear) is used as it is with the per-tensor scale
+    float(fp8_scale.to(bf16)) that fp8_activation_dequant multiplies by."""
+    w = getattr(layer, "weight", None)
+    if not isinstance(w, torch.Tensor) or not w.is_cuda or w.dim() != 2 or not w.is_contiguous():
+        return None
+    s = getattr(layer, "fp8_scale", None)
+    fp8_ref = w.dtype == torch.float8_e4m3fn and isinstance(s, torch.Tensor) and s.numel() == 1
+    plain = (type(layer) is torch.nn.Linear and w.dtype == torch.bfloat16 and "forward" not in layer.__dict__)
+    if not (fp8_ref or plain) or layer._forward_hooks or layer._forward_pre_hooks:
+        return None
+    if not linear_fp8_shape_ok(w.shape[1], w.shape[0]):
+        return None
+    b = getattr(layer, "bias", None)
+    if b is not None and (not b.is_cuda or b.dtype not in (torch.bfloat16, torch.float32)):
+        return None
+    if fp8_ref:
+        key = ("ref", w.data_ptr(), w._version, s.data_ptr(), s._version)
+    else:
+        key = ("bf16", w.data_ptr(), w._version)
+    hit = layer.__dict__.get("_jenga_fp8")
+    if hit is not None and hit[0] == key:
+        return hit[1], hit[2], b
+    with torch.no_grad():
+        if fp8_ref:
+            w8 = w
+            w_scale = torch.tensor([float(s.to(torch.bfloat16))], dtype=torch.float32,
+                                   device=w.device)
+        else:
+            w8, w_scale = quantize_rows_fp8(w)
+    layer.__dict__["_jenga_fp8"] = (key, w8, w_scale)
+    return w8, w_scale, b
