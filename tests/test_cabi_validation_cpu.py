@@ -159,6 +159,14 @@ def test_round2_entry_points_validate_before_touching_cuda():
         (lambda: lib.jenga_ln_modulate(P, 8192, P, P, P, 8192, 10, 8192, 1e-6, None), E_UNSUPPORTED, "6144"),
         (lambda: lib.jenga_gate_residual(P, 64, P, 64, P, P, 64, 0, 64, None), E_INVALID, "shape"),
         (lambda: lib.jenga_gelu_tanh(P, 64, P + 2, 64, 4, 64, None), E_INVALID, "aligned"),
+        # row strides shorter than a row: the rows would overlap and their stores race
+        (lambda: lib.jenga_gate_residual(P, 8, P, 64, P, P, 64, 4, 64, None), E_INVALID, "shape"),
+        (lambda: lib.jenga_gate_residual(P, 64, P, 8, P, P, 64, 4, 64, None), E_INVALID, "shape"),
+        (lambda: lib.jenga_gate_residual(P, 64, P, 64, P, P, 8, 4, 64, None), E_INVALID, "shape"),
+        (lambda: lib.jenga_gate_residual_tr(P, 56, P, 64, P, P, P, P, 64, 4, 64, None), E_INVALID, "shape"),
+        (lambda: lib.jenga_gate_residual_tr(P, 64, P, 64, P, P, P, P, 56, 4, 64, None), E_INVALID, "shape"),
+        (lambda: lib.jenga_gelu_tanh(P, 8, P, 64, 4, 64, None), E_INVALID, "shape"),
+        (lambda: lib.jenga_gelu_tanh(P, 64, P, 56, 4, 64, None), E_INVALID, "shape"),
         (lambda: lib.jenga_quantize_v_fp8(P, _lib.JENGA_F32, 1, 128, 2, 128 * 256, 256, 128, P, P, None), E_INVALID, "dtype"),
         (lambda: lib.jenga_quantize_v_fp8(P, _lib.JENGA_BF16, 1, 128, 2, 128 * 256, 250, 128, P, P, None), E_INVALID, "alignment"),
         (lambda: lib.jenga_prores_switch(P, P, None, P, 16, 4, 4, 4, 4, 8, 8, 0.1, 0.5, None), E_INVALID, "null"),

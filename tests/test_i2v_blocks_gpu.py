@@ -40,6 +40,8 @@ def _mask(kind, rows, seed):
         return torch.ones(rows, dtype=torch.bool, device="cuda")
     if kind == "none":
         return torch.zeros(rows, dtype=torch.bool, device="cuda")
+    if kind == "alternating":
+        return torch.arange(rows, device="cuda") % 2 == 0
     return torch.rand(rows, generator=g, device="cuda") < 0.3             # scattered
 
 
@@ -50,8 +52,9 @@ def _vec(C, g, s=0.3):
 # ------------------------------------------------------------------------------------------------
 # kernels
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("kind", ["all", "none", "scattered"])
-@pytest.mark.parametrize("L,C,strided", [(2048 + 37, 3072, False), (515, 3072, True), (1001, 1536, False)])
+@pytest.mark.parametrize("kind", ["all", "none", "alternating", "scattered"])
+@pytest.mark.parametrize("L,C,strided", [(2048 + 37, 3072, False), (515, 3072, True), (1001, 1536, False),
+                                         (8449, 4096, False), (16897, 6136, True)])
 def test_ln_modulate_tr_rows_equal_the_plain_kernel(kind, L, C, strided):
     from jenga_b200 import dense as DN
     g = torch.Generator(device="cuda").manual_seed(L + C)
@@ -72,8 +75,9 @@ def test_ln_modulate_tr_rows_equal_the_plain_kernel(kind, L, C, strided):
     assert DN._row_mask(cpu, x.device) is DN._row_mask(cpu, x.device)
 
 
-@pytest.mark.parametrize("kind", ["all", "none", "scattered"])
-@pytest.mark.parametrize("L,C,strided", [(3001, 3072, False), (515, 3072, True)])
+@pytest.mark.parametrize("kind", ["all", "none", "alternating", "scattered"])
+@pytest.mark.parametrize("L,C,strided", [(3001, 3072, False), (515, 3072, True), (2113, 1032, False),
+                                         (4225, 6144, True)])
 def test_gate_residual_tr_rows_equal_the_plain_kernel(kind, L, C, strided):
     from jenga_b200 import dense as DN
     g = torch.Generator(device="cuda").manual_seed(L + 7)

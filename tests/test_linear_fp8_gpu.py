@@ -76,7 +76,8 @@ def test_quantize_rows_matches_the_restatement(M, K, strided):
 
 
 @pytest.mark.parametrize("tr", [False, True])
-@pytest.mark.parametrize("L,C", [(1, 3072), (257, 3072), (130, 512)])
+@pytest.mark.parametrize("L,C", [(1, 3072), (257, 3072), (130, 512), (2, 16), (8448, 1040), (8449, 4096),
+                                 (16897, 6128)])
 def test_ln_modulate_fp8_is_quantize_of_ln_modulate(L, C, tr):
     from jenga_b200 import dense as DN
     dev = _dev()
