@@ -26,7 +26,8 @@ extern "C" {
 #endif
 
 /* The version changes when an existing struct layout or signature changes; entry points that are only
- * added (the FP8 Linear ones below, jenga_wan_i2v_cross_attn) keep it, so older callers stay valid. */
+ * added (the FP8 Linear ones below, jenga_wan_i2v_cross_attn, the INT8 _ex / _lse_shift ones) keep it,
+ * so older callers stay valid. */
 #define JENGA_B200_ABI_VERSION 3
 
 enum {
@@ -518,13 +519,23 @@ int jenga_quantize_v_fp8(const void* v, int32_t dtype, int32_t batch, int64_t ro
 int jenga_quantize_int8(const void* x, int32_t dtype, int32_t batch, int64_t rows, int32_t heads,
                         int64_t stride_b, int64_t stride_s, int64_t stride_h, int32_t group_rows,
                         int32_t smooth, float* mean, int8_t* out, int64_t out_rows, float* scale, void* stream);
+/* jenga_quantize_int8(q, group_rows 64, smooth 0) that also writes, for every row i of every (b, h), the
+ * fp32 shift[(b*H + h) * out_rows + i] = Q'_i . k_mean[b*H + h], Q'_i = the row's codes times its group
+ * scale (0 on the padding rows).  k_mean is the mean jenga_quantize_int8(k, 128, smooth 1) wrote, so K
+ * is quantised first.  Each row's dot product is summed in a fixed order (8 channels per thread, then a
+ * shuffle tree over 16 threads), so the shift is deterministic.  The codes and scales are bit for bit
+ * those of jenga_quantize_int8.  shift: f32 [B*H, out_rows], 4-byte aligned. */
+int jenga_quantize_q_int8_lse_shift(const void* q, int32_t dtype, int32_t batch, int64_t rows, int32_t heads,
+                                    int64_t stride_b, int64_t stride_s, int64_t stride_h, const float* k_mean,
+                                    int8_t* out, int64_t out_rows, float* scale, float* shift, void* stream);
 
 /* (f-3) opt-in INT8 Q.K^T variant of jenga_carved_attn_fwd (SageAttention's recipe): Q.K^T runs as
  * s8 x s8 -> s32 on the tensor cores from per-block-scaled int8 Q (64-row groups) and K (128-key
  * blocks, K smoothed by its per-head mean, which leaves every softmax unchanged).  `args` means what
  * it means for jenga_carved_attn_fwd (the FP8 P.V variant included) except that Q.K^T reads these
- * operands.  Not built: lse_out (smoothing shifts the LSE by q.mean), the Ulysses epilogue
- * (sp_world > 0), FP8 P.V with f16.  Lower precision than the default path; never implicit. */
+ * operands.  Refused here: lse_out (smoothing shifts the LSE by q.mean) and the Ulysses epilogue
+ * (sp_world > 0), both built by jenga_carved_attn_fwd_qk_int8_ex below; FP8 P.V with f16 is not built.
+ * Lower precision than the default path; never implicit. */
 typedef struct JengaQkInt8Args {
   const int8_t* q_i8;   const float* q_scale;   /* from jenga_quantize_int8(q, group_rows 64, smooth 0)  */
   const int8_t* k_i8;   const float* k_scale;   /* from jenga_quantize_int8(k, group_rows 128, smooth 1) */
@@ -547,6 +558,22 @@ typedef struct JengaAttnSched {
 int jenga_carved_attn_fwd_sched(const JengaAttnArgs* args, const JengaQkInt8Args* qk /* nullable */,
                                 const JengaAttnSched* sched, void* stream);
 int64_t jenga_carved_attn_sched_workspace_bytes(int32_t batch, int32_t heads, int32_t nq_sparse, int32_t nq_dense);
+
+/* The INT8 Q.K^T variant with everything jenga_carved_attn_fwd_qk_int8 refuses to do, and the work
+ * order of jenga_carved_attn_fwd_sched when `sched` is non-NULL.  Checks what those two check, and:
+ *   - the Ulysses epilogue (sp_world > 0) is built;
+ *   - lse_out is built when q_lse_shift is given (from jenga_quantize_q_int8_lse_shift over the same Q
+ *     and the mean of the same K): the natural-log LSE of each dense row is that of the smoothed scores
+ *     plus sm_scale * shift, i.e. of Q'.(K' + mean) with Q', K' the dequantised operands.  lse_out
+ *     without q_lse_shift returns JENGA_E_UNSUPPORTED; q_lse_shift must be 4-byte aligned.
+ * Without lse_out and sp_world the results are bit for bit those of jenga_carved_attn_fwd_sched (or
+ * jenga_carved_attn_fwd_qk_int8 when sched is NULL) with the same operands. */
+typedef struct JengaQkInt8ExArgs {
+  JengaQkInt8Args base;       /* the four operands and padded row counts                 */
+  const float* q_lse_shift;   /* [B*H, q_rows_padded] f32, or NULL when lse_out is NULL  */
+} JengaQkInt8ExArgs;
+int jenga_carved_attn_fwd_qk_int8_ex(const JengaAttnArgs* args, const JengaQkInt8ExArgs* qk,
+                                     const JengaAttnSched* sched /* nullable */, void* stream);
 
 #ifdef __cplusplus
 }

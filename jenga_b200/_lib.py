@@ -48,6 +48,10 @@ class JengaQkInt8Args(C.Structure):
     ]
 
 
+class JengaQkInt8ExArgs(C.Structure):
+    _fields_ = [("base", JengaQkInt8Args), ("q_lse_shift", C.c_void_p)]
+
+
 class JengaAttnSched(C.Structure):
     _fields_ = [("workspace", C.c_void_p), ("workspace_bytes", C.c_int64)]
 
@@ -230,6 +234,13 @@ def _load() -> C.CDLL:
     lib.jenga_carved_attn_fwd_sched.argtypes = [C.POINTER(JengaAttnArgs), C.POINTER(JengaQkInt8Args),
                                                 C.POINTER(JengaAttnSched), C.c_void_p]
     lib.jenga_carved_attn_fwd_sched.restype = C.c_int
+    lib.jenga_carved_attn_fwd_qk_int8_ex.argtypes = [C.POINTER(JengaAttnArgs), C.POINTER(JengaQkInt8ExArgs),
+                                                     C.POINTER(JengaAttnSched), C.c_void_p]
+    lib.jenga_carved_attn_fwd_qk_int8_ex.restype = C.c_int
+    lib.jenga_quantize_q_int8_lse_shift.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int64,
+                                                    C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                                    C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.jenga_quantize_q_int8_lse_shift.restype = C.c_int
     lib.jenga_carved_attn_sched_workspace_bytes.argtypes = [C.c_int32] * 4
     lib.jenga_carved_attn_sched_workspace_bytes.restype = C.c_int64
     lib.jenga_wan_i2v_cross_attn.argtypes = [C.POINTER(JengaWanCrossArgs), C.c_void_p]

@@ -173,12 +173,38 @@ def quantize_int8(x: torch.Tensor, group_rows: int, smooth: bool):
     return x8, scale, mean
 
 
-def quantize_qk_int8(q: torch.Tensor, k: torch.Tensor):
+def quantize_qk_int8(q: torch.Tensor, k: torch.Tensor, lse_shift: bool = False):
     """Operands of the opt-in INT8 Q.K^T variant: Q per 64-row group, K per 128-key block after
-    subtracting its per-head channel mean.  Returns (q8, q_scale, k8, k_scale)."""
-    q8, q_scale, _ = quantize_int8(q, 64, False)
-    k8, k_scale, _ = quantize_int8(k, 128, True)
-    return q8, q_scale, k8, k_scale
+    subtracting its per-head channel mean.  Returns (q8, q_scale, k8, k_scale), and with lse_shift
+    also shift f32 [B*H, round_up(Sq,128)] = Q'_i . mean(K) (C-ABI jenga_quantize_q_int8_lse_shift):
+    what the kernel needs to write the LSE of the unsmoothed scores."""
+    k8, k_scale, k_mean = quantize_int8(k, 128, True)
+    if not lse_shift:
+        q8, q_scale, _ = quantize_int8(q, 64, False)
+        return q8, q_scale, k8, k_scale
+    _require_cuda(q)
+    B, S, H, D = q.shape
+    if D != 128 or q.stride(3) != 1 or k.shape[0] != B or k.shape[2] != H:
+        raise ValueError("q must be [B,S,H,128] with contiguous channels, with k's batch and heads")
+    rows_p = (S + BLOCK - 1) // BLOCK * BLOCK
+    q8 = torch.empty((B, rows_p, H, D), dtype=torch.int8, device=q.device)
+    q_scale = torch.empty((B * H, rows_p // 64), dtype=torch.float32, device=q.device)
+    shift = torch.empty((B * H, rows_p), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        check(lib.jenga_quantize_q_int8_lse_shift(q.data_ptr(), _dtype_code(q), B, S, H, q.stride(0), q.stride(1),
+                                                  q.stride(2), k_mean.data_ptr(), q8.data_ptr(), rows_p,
+                                                  q_scale.data_ptr(), shift.data_ptr(), _stream_ptr(q.device)),
+              "quantize_q_int8_lse_shift")
+    return q8, q_scale, k8, k_scale, shift
+
+
+def quantize_operands(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, pv_fp8: bool, qk_int8: bool,
+                      lse_shift: bool = False):
+    """(v_fp8, qk_int8) arguments of _launch for the opt-in variants: V in e4m3 when pv_fp8 and q is
+    bf16 (the FP8 P.V kernel is built for bf16 only), int8 Q / K when qk_int8; None where off."""
+    v8 = quantize_v_fp8(v) if pv_fp8 and q.dtype == torch.bfloat16 else None
+    qk8 = quantize_qk_int8(q, k, lse_shift) if qk_int8 else None
+    return v8, qk8
 
 
 # Opt-in (never the default): route every operator call of this process through the FP8 P.V variant
@@ -187,7 +213,8 @@ def quantize_qk_int8(q: torch.Tensor, k: torch.Tensor):
 import os as _os
 PV_FP8: bool = _os.environ.get("JENGA_PV_FP8", "0") == "1"
 # Opt-in, the same way: INT8 Q.K^T with K smoothing (`QK_INT8 = True` or JENGA_QK_INT8=1); composes with
-# PV_FP8.  Its own tolerance row (tests/test_qk_int8_gpu.py); the mask selection is unchanged.
+# PV_FP8.  Its own tolerance row (tests/test_qk_int8_gpu.py); the mask selection is unchanged.  Both
+# switches also reach the fused Ulysses path (sp_out below) and the flash_attn shims.
 QK_INT8: bool = _os.environ.get("JENGA_QK_INT8", "0") == "1"
 
 _NBR_CACHE: dict = {}
@@ -339,9 +366,12 @@ def block_sparse_attention_variant(
                                   nbr_bits=nbr)
     want_dtype = out_dtype if variant == "wan" else q.dtype
     if sp_out is not None:
-        # fused Ulysses epilogue: rows are stored into the owners' peer-mapped buffers
+        # fused Ulysses epilogue: rows are stored into the owners' peer-mapped buffers.  q, k, v are
+        # strided views of the exchanged buffer; the quantisers read them on the current stream, after
+        # the exchange of this head group (UlyssesFusedAttention waits for it first)
+        v8, qk8 = quantize_operands(q, k, v, pv_fp8 or PV_FP8, qk_int8 or QK_INT8)
         _launch(q, k, v, mask_bits, normal_blocks, text_blocks, D ** -0.5, text_amp, normal_blocks,
-                S, S, nb * BLOCK, None, seqlen_dev, q.dtype, sp_out=sp_out)
+                S, S, nb * BLOCK, None, seqlen_dev, q.dtype, sp_out=sp_out, v_fp8=v8, qk_int8=qk8)
         return mask_bits if return_mask_bits else None
     if out is None:
         out = torch.empty((B, S, H, D), dtype=want_dtype, device=q.device)
@@ -350,10 +380,9 @@ def block_sparse_attention_variant(
     a_out_dtype = out.dtype
     limit = S  # no cu_seqlens: seqlens = [context_size] (:336 / wan :452)
     # pv_fp8 (opt-in, SURVEY §8 f-3): V is quantised per head to e4m3 and P.V runs on the FP8 tensor
-    # path; NOT the reference's arithmetic — its own tolerance row, never enabled implicitly
-    v8 = quantize_v_fp8(v) if (pv_fp8 or PV_FP8) and sp_out is None and q.dtype == torch.bfloat16 else None
+    # path; NOT the reference's arithmetic — its own tolerance row, never enabled implicitly.
     # qk_int8 (opt-in): int8 Q and smoothed int8 K in Q.K^T (for Wan, of the bf16 copies)
-    qk8 = quantize_qk_int8(q, k) if (qk_int8 or QK_INT8) else None
+    v8, qk8 = quantize_operands(q, k, v, pv_fp8 or PV_FP8, qk_int8 or QK_INT8)
     o = _launch(q, k, v, mask_bits, normal_blocks, text_blocks, D ** -0.5, text_amp, normal_blocks,
                 limit, limit, nb * BLOCK, out, seqlen_dev, a_out_dtype, v_fp8=v8, qk_int8=qk8)
     if not shape_xfuse:
@@ -364,7 +393,9 @@ def block_sparse_attention_variant(
 def _launch(q, k, v, mask_bits, nq_sparse, nq_dense, sm_scale, text_amp, text_block_start,
             kv_limit_sparse, q_limit_sparse, kv_limit_dense, out, seqlen_dev, out_dtype, sp_out=None, lse_out=None,
             v_fp8=None, qk_int8=None):
-    """qk_int8: None, or (q8, q_scale, k8, k_scale) from quantize_qk_int8 — the INT8 Q.K^T variant."""
+    """qk_int8: None, or (q8, q_scale, k8, k_scale[, lse_shift]) from quantize_qk_int8 — the INT8 Q.K^T
+    variant, launched through jenga_carved_attn_fwd_qk_int8_ex (which also builds sp_out, and lse_out
+    given the shift)."""
     B, Sq, H, D = q.shape
     a = JengaAttnArgs()
     a.q, a.k, a.v = q.data_ptr(), k.data_ptr(), v.data_ptr()
@@ -396,10 +427,12 @@ def _launch(q, k, v, mask_bits, nq_sparse, nq_dense, sm_scale, text_amp, text_bl
     a.err_flag = None
     x = None
     if qk_int8 is not None:
-        q8, q_scale, k8, k_scale = qk_int8
-        x = _lib.JengaQkInt8Args()
-        x.q_i8, x.q_scale, x.k_i8, x.k_scale = q8.data_ptr(), q_scale.data_ptr(), k8.data_ptr(), k_scale.data_ptr()
-        x.q_rows_padded, x.kv_rows_padded = q8.shape[1], k8.shape[1]
+        q8, q_scale, k8, k_scale = qk_int8[:4]
+        x = _lib.JengaQkInt8ExArgs()
+        b = x.base
+        b.q_i8, b.q_scale, b.k_i8, b.k_scale = q8.data_ptr(), q_scale.data_ptr(), k8.data_ptr(), k_scale.data_ptr()
+        b.q_rows_padded, b.kv_rows_padded = q8.shape[1], k8.shape[1]
+        x.q_lse_shift = qk_int8[4].data_ptr() if len(qk_int8) > 4 else None
     with torch.cuda.device(q.device):
         # the work order of this launch (jenga_carved_attn_fwd_sched): stream-ordered from the caching
         # allocator, so launches on other streams each get their own
@@ -407,8 +440,12 @@ def _launch(q, k, v, mask_bits, nq_sparse, nq_dense, sm_scale, text_amp, text_bl
         sched.workspace_bytes = lib.jenga_carved_attn_sched_workspace_bytes(B, H, nq_sparse, nq_dense)
         ws = torch.empty(max(sched.workspace_bytes, 1), dtype=torch.uint8, device=q.device)
         sched.workspace = ws.data_ptr()
-        check(lib.jenga_carved_attn_fwd_sched(C.byref(a), C.byref(x) if x is not None else None, C.byref(sched),
-                                              _stream_ptr(q.device)), "carved_attn_fwd_sched")
+        if x is None:
+            check(lib.jenga_carved_attn_fwd_sched(C.byref(a), None, C.byref(sched), _stream_ptr(q.device)),
+                  "carved_attn_fwd_sched")
+        else:
+            check(lib.jenga_carved_attn_fwd_qk_int8_ex(C.byref(a), C.byref(x), C.byref(sched), _stream_ptr(q.device)),
+                  "carved_attn_fwd_qk_int8_ex")
     return out
 
 

@@ -161,6 +161,12 @@ extern "C" int jenga_carved_attn_fwd_qk_int8(const JengaAttnArgs* args, const Je
   return carved_attn_fwd_impl(args, static_cast<cudaStream_t>(stream), qk);
 }
 
+extern "C" int jenga_carved_attn_fwd_qk_int8_ex(const JengaAttnArgs* args, const JengaQkInt8ExArgs* qk,
+                                                const JengaAttnSched* sched, void* stream) {
+  if (!qk) return set_error(JENGA_E_INVALID, "qk_int8_ex: null pointer");
+  return carved_attn_fwd_impl(args, static_cast<cudaStream_t>(stream), &qk->base, sched, true, qk->q_lse_shift);
+}
+
 extern "C" int jenga_carved_attn_fwd_sched(const JengaAttnArgs* args, const JengaQkInt8Args* qk,
                                            const JengaAttnSched* sched, void* stream) {
   if (!sched) return set_error(JENGA_E_INVALID, "sched: null pointer");

@@ -208,9 +208,13 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     float inv_l = zero_row ? 0.f : 1.0f / cons.l_sum[r];
     if constexpr (kPvFp8) inv_l *= __ldg(p.v_fp8_amax + b * p.heads + h) * (1.0f / 448.0f);   // undo the V scale
     if (p.lse_out && dense && in_tensor && cons.qd == 0) {
-      // softmax_lse of flash_attn (natural log): ln sum_j exp(s_j * sm_scale) = (m + log2 l) * ln 2
+      // softmax_lse of flash_attn (natural log): ln sum_j exp(s_j * sm_scale) = (m + log2 l) * ln 2.
+      // kQkInt8 scored Q'.(K - mean): every score of the row is short by sm_scale * c_i, in log2
+      // units qk_scale * c_i
+      float lse2 = cons.m_used[r] + log2f(cons.l_sum[r]);
+      if constexpr (kQkInt8) lse2 += p.qk_scale * __ldg(p.q_lse_shift + bh * p.q_groups * 64 + q_row);
       p.lse_out[(static_cast<long long>(b) * p.heads + h) * p.q_rows + q_row] =
-          zero_row ? -INFINITY : (cons.m_used[r] + log2f(cons.l_sum[r])) * 0.6931471805599453f;
+          zero_row ? -INFINITY : lse2 * 0.6931471805599453f;
     }
     if (!in_tensor) continue;
     // destination(s) of this row
@@ -334,7 +338,7 @@ int64_t carved_attn_sched_workspace_bytes(long long batch, long long heads, long
 }
 
 int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const JengaQkInt8Args* qk,
-                         const JengaAttnSched* sched) {
+                         const JengaAttnSched* sched, bool qk_ex, const float* q_lse_shift) {
   if (!a || !a->q || !a->k || !a->v || (!a->out && a->sp_world <= 0)) return set_error(JENGA_E_INVALID, "null pointer");
   if (a->dtype != JENGA_BF16 && a->dtype != JENGA_F16)
     return set_error(JENGA_E_INVALID, "dtype must be bf16 or f16");
@@ -369,9 +373,12 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
   if (qk) {
     if (!qk->q_i8 || !qk->q_scale || !qk->k_i8 || !qk->k_scale)
       return set_error(JENGA_E_INVALID, "qk_int8: null int8 operand or scale pointer");
-    if (a->lse_out)
-      return set_error(JENGA_E_UNSUPPORTED, "qk_int8: lse_out is not built (K smoothing shifts the LSE by q.mean)");
-    if (a->sp_world > 0) return set_error(JENGA_E_UNSUPPORTED, "qk_int8: the Ulysses epilogue is not built");
+    // jenga_carved_attn_fwd_qk_int8 / _sched refuse both; jenga_carved_attn_fwd_qk_int8_ex (qk_ex) builds
+    // the Ulysses epilogue, and the LSE when it is given the per-row shift that undoes K smoothing
+    if (a->lse_out && (!qk_ex || !q_lse_shift))
+      return set_error(JENGA_E_UNSUPPORTED, "qk_int8: lse_out needs q_lse_shift (K smoothing shifts the LSE by q.mean)");
+    if (a->sp_world > 0 && !qk_ex)
+      return set_error(JENGA_E_UNSUPPORTED, "qk_int8: the Ulysses epilogue is built only in jenga_carved_attn_fwd_qk_int8_ex");
     const long long q_need = (a->q_rows + kBlock - 1) / kBlock * kBlock;
     const long long kv_need = (a->kv_rows + kBlock - 1) / kBlock * kBlock;
     if (qk->q_rows_padded < q_need || qk->kv_rows_padded < kv_need || qk->q_rows_padded % kBlock ||
@@ -380,7 +387,8 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
                        static_cast<long long>(qk->q_rows_padded), static_cast<long long>(qk->kv_rows_padded),
                        q_need, kv_need);
     if (reinterpret_cast<uintptr_t>(qk->q_i8) % 16 || reinterpret_cast<uintptr_t>(qk->k_i8) % 16 ||
-        reinterpret_cast<uintptr_t>(qk->q_scale) % 4 || reinterpret_cast<uintptr_t>(qk->k_scale) % 4)
+        reinterpret_cast<uintptr_t>(qk->q_scale) % 4 || reinterpret_cast<uintptr_t>(qk->k_scale) % 4 ||
+        reinterpret_cast<uintptr_t>(q_lse_shift) % 4)
       return set_error(JENGA_E_INVALID, "qk_int8: int8 operands must be 16-byte and scales 4-byte aligned");
   }
   if (a->sp_world != 0 &&
@@ -468,6 +476,7 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
     p.k_scale = qk->k_scale;
     p.q_groups = qk->q_rows_padded / 64;
     p.k_groups = qk->kv_rows_padded / kBlock;
+    p.q_lse_shift = q_lse_shift;
   }
 
   cudaError_t ce;

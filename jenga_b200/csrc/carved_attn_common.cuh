@@ -39,6 +39,9 @@ struct KernelParams {
   const float* q_scale;
   const float* k_scale;
   long long q_groups, k_groups;   // scales per (batch, head): q_rows_padded / 64, kv_rows_padded / 128
+  // INT8 Q.K^T with lse_out: [B*H, q_rows_padded] shift c_i = Q'_i . mean(K) that K smoothing took
+  // off every score of row i (jenga_quantize_q_int8_lse_shift); the LSE adds sm_scale * c_i back
+  const float* q_lse_shift;
   int* err_flag;
   // optional [grid] item of each CTA (carved_attn_order_kernel); NULL: CTA i runs item i
   const int* order;

@@ -25,8 +25,11 @@ int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dt, uint32_t rank, v
 
 // qk != nullptr: the opt-in INT8 Q.K^T variant (jenga_carved_attn_fwd_qk_int8)
 // sched != nullptr: order the work first (jenga_carved_attn_fwd_sched)
+// qk_ex: called by jenga_carved_attn_fwd_qk_int8_ex, which also builds the Ulysses epilogue and, given
+// q_lse_shift, lse_out with INT8 Q.K^T
 int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const JengaQkInt8Args* qk = nullptr,
-                         const JengaAttnSched* sched = nullptr);
+                         const JengaAttnSched* sched = nullptr, bool qk_ex = false,
+                         const float* q_lse_shift = nullptr);
 int64_t carved_attn_sched_workspace_bytes(long long batch, long long heads, long long nq_sparse, long long nq_dense);
 int block_pool_impl(const void* x, void* pooled, void* cast_out, int in_dtype, int out_dtype,
                     int batch, int heads, int head_dim, long long rows, long long sb, long long ss,

@@ -8,6 +8,8 @@
 // the zero padding of a ragged sequence, so their keys must be the smoothed zero, not a zero code.
 // Up to three HBM-bound passes: partial column sums per 128-row block (into `out`, used as scratch),
 // their reduction to the mean in a fixed order (deterministic), and one quantising pass per group.
+// For the LSE of the INT8 path the Q pass can also write each row's shift Q'_i . mean(K): every score
+// of row i is short by that much after K smoothing.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -83,7 +85,7 @@ template <bool kBF16, int kGroup>
 __global__ void __launch_bounds__(kThreads)
 quantize_kernel(const uint16_t* __restrict__ x, long long sb, long long ss, long long sh, long long rows, int heads,
                 const float* __restrict__ mean, long long out_rows, int8_t* __restrict__ out,
-                float* __restrict__ scale) {
+                float* __restrict__ scale, const float* __restrict__ shift_mean, float* __restrict__ shift) {
   constexpr int kPer = kGroup / 16;   // rows per thread
   __shared__ float wmax[kThreads / 32];
   const int cc = threadIdx.x & 15, r0 = threadIdx.x >> 4;
@@ -124,9 +126,24 @@ quantize_kernel(const uint16_t* __restrict__ x, long long sb, long long ss, long
       for (int k = 0; k < 8; ++k) {
         const float qv = sc > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(y[i][k], sc)), -127.f), 127.f) : 0.f;
         w[k >> 2] |= (static_cast<uint32_t>(static_cast<int>(qv)) & 0xffu) << (8 * (k & 3));
+        y[i][k] = qv;   // the code, for the shift below
       }
       *reinterpret_cast<uint2*>(out + ((static_cast<long long>(b) * out_rows + row) * heads + h) * kD + cc * 8) =
           make_uint2(w[0], w[1]);
+    }
+    if (shift) {   // shift[bh][row] = sc * sum_c code[row][c] * shift_mean[bh][c]; a row is 16 lanes of a half-warp
+      float km[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) km[k] = shift_mean[bh * kD + cc * 8 + k];
+#pragma unroll
+      for (int i = 0; i < kPer; ++i) {
+        float d = 0.f;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) d = fmaf(y[i][k], km[k], d);
+#pragma unroll
+        for (int o = 8; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+        if (cc == 0) shift[bh * out_rows + g * kGroup + r0 + 16 * i] = d * sc;
+      }
     }
   }
 }
@@ -134,7 +151,7 @@ quantize_kernel(const uint16_t* __restrict__ x, long long sb, long long ss, long
 template <bool kBF16>
 int launch_all(const uint16_t* x, long long sb, long long ss, long long sh, int batch, long long rows, int heads,
                int group_rows, int smooth, float* mean, int8_t* out, long long out_rows, float* scale,
-               cudaStream_t s) {
+               const float* shift_mean, float* shift, cudaStream_t s) {
   const long long bhs = static_cast<long long>(batch) * heads;
   if (smooth) {
     const long long nblk = (rows + 127) / 128;
@@ -155,9 +172,11 @@ int launch_all(const uint16_t* x, long long sb, long long ss, long long sh, int 
   const dim3 grid(static_cast<unsigned>(per_bh), static_cast<unsigned>(bhs));
   const float* mu = smooth ? mean : nullptr;
   if (group_rows == 64)
-    quantize_kernel<kBF16, 64><<<grid, kThreads, 0, s>>>(x, sb, ss, sh, rows, heads, mu, out_rows, out, scale);
+    quantize_kernel<kBF16, 64><<<grid, kThreads, 0, s>>>(x, sb, ss, sh, rows, heads, mu, out_rows, out, scale,
+                                                         shift_mean, shift);
   else
-    quantize_kernel<kBF16, 128><<<grid, kThreads, 0, s>>>(x, sb, ss, sh, rows, heads, mu, out_rows, out, scale);
+    quantize_kernel<kBF16, 128><<<grid, kThreads, 0, s>>>(x, sb, ss, sh, rows, heads, mu, out_rows, out, scale,
+                                                          shift_mean, shift);
   const cudaError_t ce = cudaGetLastError();
   return ce == cudaSuccess ? JENGA_OK : set_cuda_error(ce, "quantize_int8 launch");
 }
@@ -167,10 +186,11 @@ int launch_all(const uint16_t* x, long long sb, long long ss, long long sh, int 
 
 using namespace jenga;
 
-extern "C" int jenga_quantize_int8(const void* x, int32_t dtype, int32_t batch, int64_t rows, int32_t heads,
-                                   int64_t stride_b, int64_t stride_s, int64_t stride_h, int32_t group_rows,
-                                   int32_t smooth, float* mean, int8_t* out, int64_t out_rows, float* scale,
-                                   void* stream) {
+// The checks of jenga_quantize_int8, shared with jenga_quantize_q_int8_lse_shift; then the launch.
+static int quantize_checked(const void* x, int32_t dtype, int32_t batch, int64_t rows, int32_t heads, int64_t stride_b,
+                            int64_t stride_s, int64_t stride_h, int32_t group_rows, int32_t smooth, float* mean,
+                            int8_t* out, int64_t out_rows, float* scale, const float* shift_mean, float* shift,
+                            void* stream) {
   if (!x || !out || !scale || (smooth && !mean)) return set_error(JENGA_E_INVALID, "quantize_int8: null pointer");
   if (dtype != JENGA_BF16 && dtype != JENGA_F16) return set_error(JENGA_E_INVALID, "quantize_int8: dtype must be bf16/f16");
   if (group_rows != 64 && group_rows != 128)
@@ -182,13 +202,31 @@ extern "C" int jenga_quantize_int8(const void* x, int32_t dtype, int32_t batch, 
                      static_cast<long long>(out_rows));
   if (stride_b <= 0 || stride_s <= 0 || stride_h <= 0 || stride_b % 8 || stride_s % 8 || stride_h % 8 ||
       reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(out) % 16 ||
-      reinterpret_cast<uintptr_t>(scale) % 4 || reinterpret_cast<uintptr_t>(mean) % 4)
+      reinterpret_cast<uintptr_t>(scale) % 4 || reinterpret_cast<uintptr_t>(mean) % 4 ||
+      reinterpret_cast<uintptr_t>(shift_mean) % 4 || reinterpret_cast<uintptr_t>(shift) % 4)
     return set_error(JENGA_E_INVALID, "quantize_int8: bad strides / alignment");
   const uint16_t* xp = static_cast<const uint16_t*>(x);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   return dtype == JENGA_BF16
              ? launch_all<true>(xp, stride_b, stride_s, stride_h, batch, rows, heads, group_rows, smooth, mean, out,
-                                out_rows, scale, s)
+                                out_rows, scale, shift_mean, shift, s)
              : launch_all<false>(xp, stride_b, stride_s, stride_h, batch, rows, heads, group_rows, smooth, mean, out,
-                                 out_rows, scale, s);
+                                 out_rows, scale, shift_mean, shift, s);
+}
+
+extern "C" int jenga_quantize_int8(const void* x, int32_t dtype, int32_t batch, int64_t rows, int32_t heads,
+                                   int64_t stride_b, int64_t stride_s, int64_t stride_h, int32_t group_rows,
+                                   int32_t smooth, float* mean, int8_t* out, int64_t out_rows, float* scale,
+                                   void* stream) {
+  return quantize_checked(x, dtype, batch, rows, heads, stride_b, stride_s, stride_h, group_rows, smooth, mean, out,
+                          out_rows, scale, nullptr, nullptr, stream);
+}
+
+extern "C" int jenga_quantize_q_int8_lse_shift(const void* q, int32_t dtype, int32_t batch, int64_t rows,
+                                               int32_t heads, int64_t stride_b, int64_t stride_s, int64_t stride_h,
+                                               const float* k_mean, int8_t* out, int64_t out_rows, float* scale,
+                                               float* shift, void* stream) {
+  if (!k_mean || !shift) return set_error(JENGA_E_INVALID, "quantize_q_int8_lse_shift: null k_mean / shift pointer");
+  return quantize_checked(q, dtype, batch, rows, heads, stride_b, stride_s, stride_h, 64, 0, nullptr, out, out_rows,
+                          scale, k_mean, shift, stream);
 }

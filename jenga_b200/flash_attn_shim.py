@@ -9,11 +9,18 @@ Shadows exactly what the reference imports (SURVEY §8b):
   flash_attn.__version__                                   attenion.py:220
 Forward only, no dropout, non-causal, head_dim 128 — the only way the Jenga paths call them;
 anything else raises instead of silently doing something different.
+
+The opt-in switches of the operator apply here too, read at call time: `attention.QK_INT8`
+(JENGA_QK_INT8=1; bf16 / fp16) runs Q.K^T in int8 with K smoothing, and `attention.PV_FP8`
+(JENGA_PV_FP8=1; bf16 only, like the operator) runs P.V in e4m3.  Each launched segment is quantised
+on its own.  _flash_attn_forward's softmax_lse stays the LSE of the unsmoothed scores: the kernel
+adds back the per-row shift that K smoothing takes off.
 """
 from __future__ import annotations
 
 import torch
 
+from . import attention as A
 from .attention import BLOCK, _launch, _require_cuda
 
 __version__ = "2.8.3+jenga_b200"
@@ -38,8 +45,9 @@ def _dense(q, k, v, softmax_scale, out=None, lse=None):
     if out is None:
         out = torch.empty((B, Sq, H, D), dtype=q.dtype, device=q.device)
     scale = D ** -0.5 if softmax_scale is None else float(softmax_scale)
+    v8, qk8 = A.quantize_operands(q, k, v, A.PV_FP8, A.QK_INT8, lse_shift=lse is not None)
     _launch(q, k, v, None, 0, (Sq + BLOCK - 1) // BLOCK, scale, 0.0, 1 << 30, Sk, Sq, Sk, out, None,
-            q.dtype, lse_out=lse)
+            q.dtype, lse_out=lse, v_fp8=v8, qk_int8=qk8)
     return out
 
 

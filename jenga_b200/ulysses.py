@@ -146,7 +146,9 @@ class UlyssesFusedAttention:
            buffered across calls (no copy out): the tensor returned by call i stays valid until
            call i+2 is issued on the same stream.
     Device-side barriers (symmetric-memory signal pads) order the peer traffic: one per sub-group
-    after its exchange, one per call after the attention."""
+    after its exchange, one per call after the attention.  The operator's opt-in switches
+    (attention.QK_INT8, attention.PV_FP8) apply: a sub-group's q, k, v are quantised on the main
+    stream once its exchange is complete, and the next call's exchange waits for the main stream."""
 
     def __init__(self, group=None, variant: str = "hyvideo", groups: int | None = None):
         self.group = group if group is not None else dist.group.WORLD
