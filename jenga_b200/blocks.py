@@ -19,8 +19,10 @@ followed by select_blocks + the carved-attention launch.  Everything around the 
 section (modulation, linear layers, gates, MLP) is executed by the block's own sub-modules and
 the reference module's own helper functions (`modulate`, `apply_gate`), so those numerics are the
 reference's by construction.  Whenever a call is not the carved configuration (sa_drop_rate == 0,
-no RMS qk-norm, unusual dtype, batch > 1 for Wan, sequence parallel for I2V, …) the ORIGINAL forward
-runs, with the caller's own arguments (`_patched`).
+no RMS qk-norm, unusual dtype, batch > 1 for Wan, the reference's own sequence parallel for I2V, …) the
+ORIGINAL forward runs, with the caller's own arguments (`_patched`).  An I2V block with `jenga_sp` set
+(the Hilbert-sharded forward of hyi2v_sp.py) routes its attention section through that Ulysses object
+and has no such fall-back.
 
 The I2V blocks differ from the HunyuanVideo ones in three ways the fused forwards follow: the
 token-replace modulation (rows of the first frame take the `tr_` shift / scale / gate; the
@@ -53,12 +55,29 @@ import torch
 
 from . import dense as DN
 from . import hyvideo as HY
+from . import ulysses as U
 from . import wan as WAN
 
 _HY_MODULES = ("hyvideo.modules.models_mul_block_gc_ha_multigpu",)
 _I2V_MODULES = ("hyvideo_i2v.modules.models_mul",)
 _WAN_MODULES = ("wan.modules.model_mul",)
-STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "wan_self": 0, "fallback": 0,
+# opt-in (install(i2v_sp=True) / JENGA_I2V_SP=1): hyvideo_i2v/inference.py's parallelize_transformer
+# is swapped for the Hilbert-sharded forward of hyi2v_sp.py
+_I2V_SP_MODULES = ("hyvideo_i2v.inference",)
+I2V_SP = False
+
+
+def set_i2v_sp(on: bool) -> None:
+    """Turns the sequence-parallel I2V route on or off for the rest of the process.  Off also puts the
+    reference's parallelize_transformer back if hyvideo_i2v.inference was already swapped."""
+    global I2V_SP
+    I2V_SP = bool(on)
+    inf = sys.modules.get(_I2V_SP_MODULES[0])
+    fn = getattr(inf, "parallelize_transformer", None)
+    if not I2V_SP and getattr(fn, "__jenga_b200__", False):
+        inf.parallelize_transformer = fn.__wrapped__
+STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "i2v_double_sp": 0,
+         "i2v_single_sp": 0, "wan_self": 0, "fallback": 0,
          "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0,
          "wan_i2v_cross": 0, "linear_fp8": 0}
 # the CLIP image tokens at the head of the Wan2.1-I2V context (model_mul.py:230-231)
@@ -184,10 +203,29 @@ def _attention_section(self, mod, img_qkv, txt_qkv, norms, *, freqs_cis, cu_seql
                        sa_drop_rate, txt_amp, curve_sel, p_remain_rates, text_blocks, pad_ragged, out=None):
     """prologue -> (SP exchange | select + carved attention).  Returns attn [B, L+T, H*D]
     (written into `out`, a [B, L+T, H, D] view, when given and not under SP).
-    pad_ragged: S = L+T need not be a multiple of 128 (the I2V operator zero-pads it)."""
+    pad_ragged: S = L+T need not be a multiple of 128 (the I2V operator zero-pads it).
+    Under `jenga_sp` (the sharded I2V forward, hyi2v_sp.py) L is the rank's image slice."""
     (wq_i, eps), (wk_i, _), (wq_t, _), (wk_t, _) = norms
     L = img_qkv.shape[1]
     _, _, block_neighbor_list = mod.random.choice(curve_sel)                       # :232 / :438
+    jsp = getattr(self, "jenga_sp", None)
+    if jsp is not None:
+        if (txt_qkv.shape[1] + HY.BLOCK - 1) // HY.BLOCK != text_blocks:
+            # the Ulysses objects hand the operator ceil(T/128) text blocks; the I2V operator always
+            # takes four (text_blocks=4), so the two agree only for 385 <= T <= 512 text tokens
+            raise ValueError(f"sequence-parallel HunyuanVideo-I2V needs {text_blocks} text blocks "
+                             f"({(text_blocks - 1) * HY.BLOCK + 1}..{text_blocks * HY.BLOCK} text tokens), "
+                             f"got {txt_qkv.shape[1]} text tokens")
+        # top_k is the single-GPU rule over the GLOBAL image length, not the T2V SP quirk
+        # P*int((1-drop)*(L_loc//128)) (SURVEY a-7, App. A-12): the sharded I2V forward computes
+        # what one GPU computes
+        top_k = HY.select_block_num(sa_drop_rate, L * U._group_size_rank(jsp.group)[0])
+        q, k, v, _ = HY.attention_prologue(img_qkv, txt_qkv, self.heads_num, wq_i, wk_i, wq_t, wk_t, eps, freqs_cis,
+                                           want_pool=False)
+        # the I2V reference module has no my_parallel_attention: the restatement of attenion.py:159-195
+        return U.my_parallel_attention(jsp, q, k, v, img_q_len=L, img_kv_len=L, cu_seqlens_q=cu_seqlens_q,
+                                       cu_seqlens_kv=cu_seqlens_kv, top_k=top_k, text_amp=txt_amp,
+                                       block_neighbor_list=block_neighbor_list, p_remain_rates=p_remain_rates)
     sp = getattr(self, "hybrid_seq_parallel_attn", None)
     top_k = HY.select_block_num(sa_drop_rate, L, mod.get_sequence_parallel_world_size() if sp else 1)  # :242, :249-251
     q, k, v, pools = HY.attention_prologue(img_qkv, txt_qkv, self.heads_num, wq_i, wk_i, wq_t, wk_t, eps, freqs_cis,
@@ -260,7 +298,7 @@ def _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freq
     act = self.mlp_act
     fuse_cat = (isinstance(act, torch.nn.GELU) and getattr(act, "approximate", "none") == "tanh"
                 and lin1.dtype == torch.bfloat16 and x.shape[0] == 1
-                and not getattr(self, "hybrid_seq_parallel_attn", None))
+                and not getattr(self, "hybrid_seq_parallel_attn", None) and getattr(self, "jenga_sp", None) is None)
     cat = attn_view = None
     if fuse_cat:
         cat = torch.empty((x.shape[0], x.shape[1], C3 // 3 + mlp.shape[-1]), dtype=lin1.dtype, device=lin1.device)
@@ -301,13 +339,33 @@ def _hy_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=None
                           text_blocks=txt_block_num, pad_ragged=False, ok=_hy_ok(self, x.shape[1]))
 
 
-def _i2v_ok(self, S, condition_type, first_frame_mask):
-    # sequence parallel: the reference runs the dense parallel_attention (:264-274, :483-493); the
-    # prefix form of token replace (frist_frame_token_num) is only reached outside the Jenga forward;
-    # with text_blocks=4 the operator needs at least one image block
-    return (not getattr(self, "hybrid_seq_parallel_attn", None)
-            and not (condition_type == "token_replace" and first_frame_mask is None)
+def _i2v_ok(self, L, T, condition_type, first_frame_mask):
+    # the reference's sequence parallel (hybrid_seq_parallel_attn) runs the dense parallel_attention
+    # (:264-274, :483-493): the original forward; `jenga_sp` is the sharded I2V forward of hyi2v_sp.py,
+    # whose L is the rank's slice of the global image length; the prefix form of token replace
+    # (frist_frame_token_num) is only reached outside the Jenga forward; with text_blocks=4 the
+    # operator needs at least one image block
+    if getattr(self, "hybrid_seq_parallel_attn", None):
+        return False
+    jsp = getattr(self, "jenga_sp", None)
+    S = L * (U._group_size_rank(jsp.group)[0] if jsp is not None else 1) + T
+    return (not (condition_type == "token_replace" and first_frame_mask is None)
             and (S + HY.BLOCK - 1) // HY.BLOCK > _I2V_TEXT_BLOCKS)
+
+
+def _i2v_stat(self, stat):
+    return stat + "_sp" if getattr(self, "jenga_sp", None) is not None else stat
+
+
+def _i2v_sharded_result(self, out):
+    """the sharded I2V forward has no fall-back: the original forward would attend over the rank's
+    rows alone"""
+    if out is None and getattr(self, "jenga_sp", None) is not None and \
+            not getattr(self, "hybrid_seq_parallel_attn", None):
+        raise RuntimeError(f"{type(self).__name__} under jenga_sp: the call is not the carved configuration "
+                           "(sa_drop_rate 0, no curve, no RMS qk-norm, head_dim != 128, or a dtype / device "
+                           "the fused forward does not take); the sharded I2V forward has no fall-back")
+    return out
 
 
 def _i2v_tr(condition_type, token_replace_vec, first_frame_mask):
@@ -318,11 +376,11 @@ def _i2v_double(mod, self, img, txt, vec, cu_seqlens_q=None, cu_seqlens_kv=None,
                 max_seqlen_kv=None, freqs_cis=None, sa_drop_rate=0.0, first_frame_mask=None,
                 condition_type=None, token_replace_vec=None, frist_frame_token_num=None, txt_amp=0.0,
                 curve_sel=None, p_remain_rates=0.5, per_block_token=128):
-    return _double_stream(mod, self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp,
-                          curve_sel, p_remain_rates, per_block_token, stat="i2v_double",
-                          tr=_i2v_tr(condition_type, token_replace_vec, first_frame_mask),
-                          text_blocks=_I2V_TEXT_BLOCKS, pad_ragged=True,
-                          ok=_i2v_ok(self, img.shape[1] + txt.shape[1], condition_type, first_frame_mask))
+    return _i2v_sharded_result(self, _double_stream(
+        mod, self, img, txt, vec, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp, curve_sel,
+        p_remain_rates, per_block_token, stat=_i2v_stat(self, "i2v_double"),
+        tr=_i2v_tr(condition_type, token_replace_vec, first_frame_mask), text_blocks=_I2V_TEXT_BLOCKS,
+        pad_ragged=True, ok=_i2v_ok(self, img.shape[1], txt.shape[1], condition_type, first_frame_mask)))
 
 
 def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=None, max_seqlen_q=None,
@@ -330,12 +388,12 @@ def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=Non
                 condition_type=None, token_replace_vec=None, frist_frame_token_num=None, txt_amp=0.0,
                 curve_sel=None, p_remain_rates=0.5, per_block_token=128):
     # first_frame_mask here is full_first_frame_mask (jenga_hyi2v.py:129-130): a CPU bool over L+T rows
-    return _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp,
-                          curve_sel, p_remain_rates, per_block_token, stat="i2v_single",
-                          tr=_i2v_tr(condition_type, token_replace_vec, first_frame_mask),
-                          text_blocks=_I2V_TEXT_BLOCKS, pad_ragged=True,
-                          ok=(_i2v_ok(self, x.shape[1], condition_type, first_frame_mask)
-                              and 0 < txt_len < x.shape[1]))
+    return _i2v_sharded_result(self, _single_stream(
+        mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freqs_cis, sa_drop_rate, txt_amp, curve_sel,
+        p_remain_rates, per_block_token, stat=_i2v_stat(self, "i2v_single"),
+        tr=_i2v_tr(condition_type, token_replace_vec, first_frame_mask), text_blocks=_I2V_TEXT_BLOCKS,
+        pad_ragged=True, ok=(_i2v_ok(self, x.shape[1] - txt_len, txt_len, condition_type, first_frame_mask)
+                             and 0 < txt_len < x.shape[1])))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -475,6 +533,9 @@ def _patched(orig, fused):
 def patch_module(mod) -> list[str]:
     """Patches the block classes of an already imported reference module; returns what it did."""
     name = mod.__name__
+    if name in _I2V_SP_MODULES:
+        from .hyi2v_sp import install_parallelize_transformer
+        return [f"{name}.parallelize_transformer"] if I2V_SP and install_parallelize_transformer(mod) else []
     fused = {}
     if name.startswith(("hyvideo.", "hyvideo_i2v.")):
         # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
@@ -507,7 +568,9 @@ class _PatchingLoader(importlib.abc.Loader):
         self.inner.exec_module(module)
         done = patch_module(module)
         if done:
-            print(f"[jenga_b200] fused attention section installed: {', '.join(done)}", file=sys.stderr)
+            what = ("sequence-parallel I2V route" if module.__name__ in _I2V_SP_MODULES
+                    else "fused attention section")
+            print(f"[jenga_b200] {what} installed: {', '.join(done)}", file=sys.stderr)
 
     def __getattr__(self, item):
         return getattr(self.inner, item)
@@ -517,7 +580,7 @@ class _PatchFinder(importlib.abc.MetaPathFinder):
     targets = _HY_MODULES + _I2V_MODULES + _WAN_MODULES
 
     def find_spec(self, fullname, path, target=None):
-        if fullname not in self.targets:
+        if fullname not in self.targets and not (I2V_SP and fullname in _I2V_SP_MODULES):
             return None
         for finder in sys.meta_path:
             if finder is self or not hasattr(finder, "find_spec"):
@@ -533,7 +596,7 @@ def install_block_hook() -> None:
     """Idempotent.  Also patches target modules that were imported before the hook existed."""
     if not any(isinstance(f, _PatchFinder) for f in sys.meta_path):
         sys.meta_path.insert(0, _PatchFinder())
-    for name in _PatchFinder.targets:
+    for name in _PatchFinder.targets + (_I2V_SP_MODULES if I2V_SP else ()):
         if name in sys.modules and not getattr(sys.modules[name], "__jenga_b200__", False):
             patch_module(sys.modules[name])
 
