@@ -22,7 +22,8 @@ reference's by construction.  Whenever a call is not the carved configuration (s
 no RMS qk-norm, unusual dtype, batch > 1 for Wan, the reference's own sequence parallel for I2V, …) the
 ORIGINAL forward runs, with the caller's own arguments (`_patched`).  An I2V block with `jenga_sp` set
 (the Hilbert-sharded forward of hyi2v_sp.py) routes its attention section through that Ulysses object
-and has no such fall-back.
+and has no such fall-back; so does a WanSelfAttention with `jenga_sp` set (the Hilbert-sharded Wan
+forward of wan_sp.py), whose carved and dense calls both go through the exchange.
 
 The I2V blocks differ from the HunyuanVideo ones in three ways the fused forwards follow: the
 token-replace modulation (rows of the first frame take the `tr_` shift / scale / gate; the
@@ -65,6 +66,10 @@ _WAN_MODULES = ("wan.modules.model_mul",)
 # is swapped for the Hilbert-sharded forward of hyi2v_sp.py
 _I2V_SP_MODULES = ("hyvideo_i2v.inference",)
 I2V_SP = False
+# opt-in (install(wan_sp=True) / JENGA_WAN_SP=1): wan/distributed/xdit_context_parallel.py's
+# usp_dit_forward / usp_attn_forward are swapped for the Hilbert-sharded TeaCache forward of wan_sp.py
+_WAN_SP_MODULES = ("wan.distributed.xdit_context_parallel",)
+WAN_SP = False
 
 
 def set_i2v_sp(on: bool) -> None:
@@ -76,8 +81,26 @@ def set_i2v_sp(on: bool) -> None:
     fn = getattr(inf, "parallelize_transformer", None)
     if not I2V_SP and getattr(fn, "__jenga_b200__", False):
         inf.parallelize_transformer = fn.__wrapped__
+
+
+def set_wan_sp(on: bool) -> None:
+    """Turns the sequence-parallel Wan route on or off for the rest of the process.  Off also puts the
+    reference's usp_dit_forward / usp_attn_forward back if wan.distributed.xdit_context_parallel was
+    already swapped (a model that has bound them keeps what it bound)."""
+    global WAN_SP
+    WAN_SP = bool(on)
+    xdit = sys.modules.get(_WAN_SP_MODULES[0])
+    if not WAN_SP and xdit is not None:
+        from .wan_sp import uninstall_usp
+        uninstall_usp(xdit)
+
+
+def _sp_modules():
+    return (_I2V_SP_MODULES if I2V_SP else ()) + (_WAN_SP_MODULES if WAN_SP else ())
+
+
 STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "i2v_double_sp": 0,
-         "i2v_single_sp": 0, "wan_self": 0, "fallback": 0,
+         "i2v_single_sp": 0, "wan_self": 0, "wan_self_sp": 0, "wan_self_dense_sp": 0, "fallback": 0,
          "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0,
          "wan_i2v_cross": 0, "linear_fp8": 0}
 # the CLIP image tokens at the head of the Wan2.1-I2V context (model_mul.py:230-231)
@@ -399,8 +422,50 @@ def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=Non
 # ------------------------------------------------------------------------------------------------
 # Wan blocks
 # ------------------------------------------------------------------------------------------------
+def _wan_self_sp(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates, freq_remap,
+                 block_neighbor_list):
+    """WanSelfAttention.forward on a rank's n rows of the Hilbert-sharded Wan forward (wan_sp.py): the
+    norm + RoPE prologue on the rank's rows, then the Ulysses exchange and the operator over the first
+    L (the global token count) exchanged rows.  top_k and first_frame_blocks follow the single-GPU rule
+    over L (model_mul.py:161-164); sa_drop_rate <= 0.25 (:153, the warm-up steps) runs the dense class
+    over the same exchange.  No fall-back: the original forward would attend over the rank's rows."""
+    b, n = x.shape[:2]
+    wq = getattr(self.norm_q, "weight", None)
+    wk = getattr(self.norm_k, "weight", None)
+    if (not x.is_cuda or b != 1 or self.head_dim != 128 or per_block_tokens != 128 or wq is None or wk is None
+            or type(self.norm_q).__name__ != "WanRMSNorm" or type(self.norm_k).__name__ != "WanRMSNorm"
+            or freq_remap is None):
+        raise RuntimeError(f"{type(self).__name__} under jenga_sp: the call is not one the sharded Wan forward "
+                           "takes (a CUDA batch-1 input, head_dim 128, 128-token blocks, WanRMSNorm q / k "
+                           "norms with weights and a freq_remap); it has no fall-back")
+    q_lin, k_lin = self.q(x), self.k(x)
+    if q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype != q_lin.dtype:
+        raise RuntimeError(f"{type(self).__name__} under jenga_sp: q / k Linears return {q_lin.dtype}, "
+                           "the prologue takes bf16 or fp32")
+    grid = [int(g) for g in grid_sizes[0].tolist()]
+    L = grid[0] * grid[1] * grid[2]
+    eps = float(self.norm_q.eps)
+    q = WAN.norm_rope(q_lin, wq, self.num_heads, grid, freqs, freq_remap, eps)
+    k = WAN.norm_rope(k_lin, wk, self.num_heads, grid, freqs, freq_remap, eps)
+    # the bf16 v both single-GPU routes attend: flash_attention's half() and the operator's cast
+    v = self.v(x).view(b, n, self.num_heads, self.head_dim).to(torch.bfloat16).contiguous()
+    dense = sa_drop_rate <= 0.25
+    top_k, ff = (0, 0) if dense else WAN.block_counts(L, sa_drop_rate)
+    out = jsp(None, q, k, v, top_k=top_k, block_neighbor_list=None if dense else block_neighbor_list,
+              p_remain_rates=p_remain_rates, first_frame_blocks=ff, dense=dense, seq_len=L)
+    STATS["wan_self_dense_sp" if dense else "wan_self_sp"] += 1
+    out = out.flatten(2)
+    if not torch.is_autocast_enabled():
+        out = out.float()       # the query dtype the reference returns, as in _wan_self
+    return self.o(out)
+
+
 def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128, p_remain_rates=0.8,
               freq_remap=None, block_neighbor_list=None):
+    jsp = getattr(self, "jenga_sp", None)
+    if jsp is not None:
+        return _wan_self_sp(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
+                            freq_remap, block_neighbor_list)
     b, s = x.shape[:2]
     wq = getattr(self.norm_q, "weight", None)
     wk = getattr(self.norm_k, "weight", None)
@@ -536,6 +601,9 @@ def patch_module(mod) -> list[str]:
     if name in _I2V_SP_MODULES:
         from .hyi2v_sp import install_parallelize_transformer
         return [f"{name}.parallelize_transformer"] if I2V_SP and install_parallelize_transformer(mod) else []
+    if name in _WAN_SP_MODULES:
+        from .wan_sp import install_usp
+        return [f"{name}.usp_dit_forward", f"{name}.usp_attn_forward"] if WAN_SP and install_usp(mod) else []
     fused = {}
     if name.startswith(("hyvideo.", "hyvideo_i2v.")):
         # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
@@ -569,6 +637,7 @@ class _PatchingLoader(importlib.abc.Loader):
         done = patch_module(module)
         if done:
             what = ("sequence-parallel I2V route" if module.__name__ in _I2V_SP_MODULES
+                    else "sequence-parallel Wan route" if module.__name__ in _WAN_SP_MODULES
                     else "fused attention section")
             print(f"[jenga_b200] {what} installed: {', '.join(done)}", file=sys.stderr)
 
@@ -580,7 +649,7 @@ class _PatchFinder(importlib.abc.MetaPathFinder):
     targets = _HY_MODULES + _I2V_MODULES + _WAN_MODULES
 
     def find_spec(self, fullname, path, target=None):
-        if fullname not in self.targets and not (I2V_SP and fullname in _I2V_SP_MODULES):
+        if fullname not in self.targets and fullname not in _sp_modules():
             return None
         for finder in sys.meta_path:
             if finder is self or not hasattr(finder, "find_spec"):
@@ -596,7 +665,7 @@ def install_block_hook() -> None:
     """Idempotent.  Also patches target modules that were imported before the hook existed."""
     if not any(isinstance(f, _PatchFinder) for f in sys.meta_path):
         sys.meta_path.insert(0, _PatchFinder())
-    for name in _PatchFinder.targets + (_I2V_SP_MODULES if I2V_SP else ()):
+    for name in _PatchFinder.targets + _sp_modules():
         if name in sys.modules and not getattr(sys.modules[name], "__jenga_b200__", False):
             patch_module(sys.modules[name])
 

@@ -29,18 +29,20 @@ import torch.distributed as dist
 STEP_CALC = (0, 1, 2, 3, 5, 7, 10, 13, 16, 19, 22, 25, 28, 31, 34, 37, 40, 42, 44, 45, 46, 47, 48, 49)
 
 
-def check_degree(img_tokens: int, heads: int, world: int) -> None:
-    """The layout needs whole image slices per rank and whole head groups per rank."""
+def check_degree(img_tokens: int, heads: int, world: int, model: str = "HunyuanVideo-I2V") -> None:
+    """The layout needs whole head groups per rank and, for a non-zero img_tokens, whole image slices
+    per rank.  `model` names the model in the message (the Wan route, wan_sp.py, pads its slices
+    instead and passes 0)."""
     if heads % world:
-        raise ValueError(f"sequence-parallel HunyuanVideo-I2V: {heads} attention heads do not split over "
+        raise ValueError(f"sequence-parallel {model}: {heads} attention heads do not split over "
                          f"{world} ranks (the degree must divide the head count)")
     if img_tokens % world:
-        raise ValueError(f"sequence-parallel HunyuanVideo-I2V: {img_tokens} image tokens do not split over "
+        raise ValueError(f"sequence-parallel {model}: {img_tokens} image tokens do not split over "
                          f"{world} ranks (the degree must divide the image token count)")
 
 
-def default_attention(group=None):
-    """UlyssesFusedAttention(variant="hyvideo_i2v") when every rank can map symmetric memory, else
+def default_attention(group=None, variant: str = "hyvideo_i2v"):
+    """UlyssesFusedAttention(variant=variant) when every rank can map symmetric memory, else
     UlyssesCarvedAttention (NCCL all-to-all) — the all-ranks agreement install() uses for HunyuanVideo.
     JENGA_ULYSSES=nccl picks the NCCL form."""
     from .ulysses import UlyssesCarvedAttention, UlyssesFusedAttention
@@ -56,8 +58,8 @@ def default_attention(group=None):
         t = torch.tensor([ok], device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MIN, group=g)
         ok = int(t.item())
-    return (UlyssesFusedAttention(group=g, variant="hyvideo_i2v") if ok
-            else UlyssesCarvedAttention(group=group, variant="hyvideo_i2v"))
+    return (UlyssesFusedAttention(group=g, variant=variant) if ok
+            else UlyssesCarvedAttention(group=group, variant=variant))
 
 
 def get_cu_seqlens(text_mask: torch.Tensor, img_len: int, device) -> torch.Tensor:
@@ -72,9 +74,16 @@ def get_cu_seqlens(text_mask: torch.Tensor, img_len: int, device) -> torch.Tenso
 
 
 def shard(x: torch.Tensor, dim: int, world: int, rank: int) -> torch.Tensor:
-    """The contiguous slice `rank` of `world` along `dim` (the length divides by world)."""
-    n = x.shape[dim] // world
-    return x.narrow(dim, rank * n, n).contiguous()
+    """The contiguous slice `rank` of `world` along `dim`: rows [rank*n, min((rank+1)*n, len)) with
+    n = ceil(len / world), zero-padded to n rows (no padding when the length divides by world)."""
+    n = -(-x.shape[dim] // world)
+    lo = min(rank * n, x.shape[dim])
+    part = x.narrow(dim, lo, min(n, x.shape[dim] - lo))
+    if part.shape[dim] == n:
+        return part.contiguous()
+    pad = list(x.shape)
+    pad[dim] = n - part.shape[dim]
+    return torch.cat([part, x.new_zeros(pad)], dim)
 
 
 def _step_calc(transformer):

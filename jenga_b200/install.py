@@ -28,19 +28,27 @@ def _module(name: str, **attrs) -> types.ModuleType:
 
 
 def install(flash_attn: bool = True, gilbert: bool = True, ulysses: bool = True, fused_blocks: bool = True,
-            gather: bool = True, i2v_sp: bool | None = None) -> list[str]:
+            gather: bool = True, i2v_sp: bool | None = None, wan_sp: bool | None = None) -> list[str]:
     """Pre-seeds sys.modules; returns the names it installed.
     fused_blocks: also patch the reference block classes right after they are imported so that
     RMSNorm + RoPE + cat + pooling run as the fused prologue kernel (jenga_b200/blocks.py).
     gather: route the token reorder `x[:, hilbert_order]` to the gather kernel.
     i2v_sp: `jenga_hyi2v.py --ulysses-degree N` runs the Hilbert-sharded I2V forward over the Ulysses
     exchange (jenga_b200/hyi2v_sp.py) instead of the reference's spatial-chunk dense SP; off by
-    default, None reads JENGA_I2V_SP=1.  Needs fused_blocks."""
+    default, None reads JENGA_I2V_SP=1.  Needs fused_blocks.
+    wan_sp: `jenga_wan.py --ulysses_size N` runs the Hilbert-sharded TeaCache forward over the Ulysses
+    exchange (jenga_b200/wan_sp.py) instead of the reference's usp_dit_forward / usp_attn_forward; off
+    by default, None reads JENGA_WAN_SP=1.  Needs fused_blocks."""
     import os
     if i2v_sp is None:
         i2v_sp = os.environ.get("JENGA_I2V_SP", "") == "1"
+    if wan_sp is None:
+        wan_sp = os.environ.get("JENGA_WAN_SP", "") == "1"
     if i2v_sp and not fused_blocks:
         raise ValueError("i2v_sp routes the attention through the fused I2V block forwards: it needs fused_blocks")
+    if wan_sp and not fused_blocks:
+        raise ValueError("wan_sp routes the self-attention through the fused WanSelfAttention forward: it needs "
+                         "fused_blocks")
     from . import attention as A
     from . import flash_attn_shim as F
     from . import gilbert as G
@@ -122,11 +130,14 @@ def install(flash_attn: bool = True, gilbert: bool = True, ulysses: bool = True,
         done.append("gilbert")
     from . import blocks
     blocks.set_i2v_sp(i2v_sp)
+    blocks.set_wan_sp(wan_sp)
     if fused_blocks:
         blocks.install_block_hook()
         done.append("block-forward hook")
         if i2v_sp:
             done.append("sequence-parallel I2V route")
+        if wan_sp:
+            done.append("sequence-parallel Wan route")
     if gather:
         from . import blocks
         blocks.install_gather_hook()

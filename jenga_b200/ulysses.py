@@ -14,6 +14,16 @@ sequence.  Data movement (SURVEY Appendix A2):
                             all-to-alls them, :207,:215-217 — same result)
 Collectives are NCCL via torch.distributed (`gloo` works for the CPU tests of the layout
 logic); the attention itself is the single-GPU operator on the rank's head group.
+
+Three keyword arguments serve the Hilbert-sharded Wan forward (wan_sp.py); their defaults leave every
+other call as it was:
+  first_frame_blocks  handed to the operator (the Wan first-frame rule, wan/…:400-406)
+  dense               no selection: the dense class of the attention kernel over all rows, exactly
+                      as the flash_attn shim runs it on one GPU (the Wan warm-up steps,
+                      model_mul.py:153), following attention.QK_INT8 / PV_FP8 the same way
+  seq_len             the global valid length L when the ranks' equal slices are zero-padded
+                      (P*n_loc > L): the operator sees the first L rows only, so its blocks, pooling
+                      and limits are those of one GPU; the result rows past L are zero
 """
 from __future__ import annotations
 
@@ -60,6 +70,25 @@ def heads_to_seq(x: torch.Tensor, group=None) -> torch.Tensor:
     return recv.permute(1, 2, 0, 3, 4).reshape(B, n, P * h, D)
 
 
+def _valid_rows(seq_len, N, n, T, dense, first_frame_blocks):
+    """L, the rows the operator sees (the seq_len / dense / first_frame_blocks arguments checked)"""
+    L = N if seq_len is None else int(seq_len)
+    if not N - n < L <= N:
+        raise ValueError(f"seq_len {L} does not fit {N // n} slices of {n} rows with a real row in each")
+    if (L != N or dense) and T:
+        raise ValueError("seq_len < P * n_loc and dense are built for image rows alone (no joint tensors)")
+    if dense and first_frame_blocks:
+        raise ValueError("a dense call has no selection: first_frame_blocks must be 0")
+    return L
+
+
+def _dense_shim(q, k, v):
+    """the single-GPU dense call of the Wan self-attention (the flash_attn_varlen_func shim over one
+    segment of all rows)"""
+    from .flash_attn_shim import flash_attn_func
+    return flash_attn_func(q, k, v)
+
+
 def gather_heads(x: torch.Tensor, group=None) -> torch.Tensor:
     """[B, T, H/P, D] on every rank (different head groups) -> [B, T, H, D] everywhere."""
     P, _ = _group_size_rank(group)
@@ -71,13 +100,15 @@ def gather_heads(x: torch.Tensor, group=None) -> torch.Tensor:
 
 class UlyssesCarvedAttention:
     """Callable with the signature the DiT blocks use for `hybrid_seq_parallel_attn`
-    (xdit_ring_atten.py:61-85).  `attn_fn` is injectable so the CPU tests can exercise the
-    layout logic with the oracle; by default it is the sm_90a operator."""
+    (xdit_ring_atten.py:61-85).  `attn_fn` and `dense_fn` (q, k, v -> out, the dense=True call) are
+    injectable so the CPU tests can exercise the layout logic with the oracle; by default they are
+    the sm_90a operator and the flash_attn shim."""
 
-    def __init__(self, group=None, attn_fn=None, variant: str = "hyvideo"):
+    def __init__(self, group=None, attn_fn=None, variant: str = "hyvideo", dense_fn=None):
         self.group = group
         self._attn_fn = attn_fn
-        self.variant = variant  # "hyvideo" | "hyvideo_i2v" (ragged text: 400 tokens -> 4 blocks)
+        self._dense_fn = dense_fn or _dense_shim
+        self.variant = variant  # "hyvideo" | "hyvideo_i2v" (ragged text: 400 tokens -> 4 blocks) | "wan"
 
     def _attn(self, *a, **k):
         if self._attn_fn is None:
@@ -89,7 +120,7 @@ class UlyssesCarvedAttention:
     def __call__(self, attn, query, key, value, *, joint_tensor_query=None, joint_tensor_key=None,
                  joint_tensor_value=None, joint_strategy="none", top_k=0, text_amp=0.0,
                  block_neighbor_list=None, p_remain_rates=0.0, cu_seqlens_q=None, cu_seqlens_kv=None,
-                 **_unused):
+                 first_frame_blocks=0, dense=False, seq_len=None, **_unused):
         P, r = _group_size_rank(self.group)
         B, q_len, H, D = query.shape
         h = H // P
@@ -101,6 +132,7 @@ class UlyssesCarvedAttention:
             raise ValueError("joint_tensor_query/key/value must be given together")
         T = joint_tensor_query.shape[1] if joint else 0
         N = P * q_len
+        L = _valid_rows(seq_len, N, q_len, T, dense, first_frame_blocks)
         dev, dt = query.device, query.dtype
         # receive buffers already shaped [B, N+T, h, D] so text rows are appended in place
         qkv = [torch.empty((B, N + T, h, D), dtype=dt, device=dev) for _ in range(3)]
@@ -119,10 +151,20 @@ class UlyssesCarvedAttention:
                             torch.full((1,), N + T, dtype=torch.int32, device=dev)])
         else:
             cu = None
-        out = self._attn(qkv[0], qkv[1], qkv[2], top_k=top_k, block_size_M=128, block_size_N=128,
-                         cu_seqlens_q=cu, cu_seqlens_kv=cu, text_amp=text_amp,
-                         block_neighbor_list=block_neighbor_list, p_remain_rates=p_remain_rates,
-                         shape_xfuse=True, text_blocks=(T + BLOCK - 1) // BLOCK if joint else 0)
+        if dense:
+            out = self._dense_fn(*(x[:, :L] for x in qkv))
+        else:
+            # the first L rows (all N + T without seq_len); first_frame_blocks only when given, so the
+            # attn_fn of every other caller sees the arguments it always saw
+            ff = {"first_frame_blocks": first_frame_blocks} if first_frame_blocks else {}
+            out = self._attn(*(x[:, :L + T] for x in qkv), top_k=top_k, block_size_M=128, block_size_N=128,
+                             cu_seqlens_q=cu, cu_seqlens_kv=cu, text_amp=text_amp,
+                             block_neighbor_list=block_neighbor_list, p_remain_rates=p_remain_rates,
+                             shape_xfuse=True, text_blocks=(T + BLOCK - 1) // BLOCK if joint else 0, **ff)
+        if L < N:
+            full = torch.zeros((B, N, h, D), dtype=out.dtype, device=out.device)   # the pad rows stay zero
+            full[:, :L] = out
+            out = full
         img = heads_to_seq(out[:, :N], self.group)
         if not joint:
             return img
@@ -159,6 +201,7 @@ class UlyssesFusedAttention:
             groups = int(env) if env.isdigit() and int(env) > 0 else None   # tuning / test override
         self.groups = groups
         self._bufs = {}
+        self._pad_len = {}          # result buffer -> the seq_len of its last call
         self._side = None
         self._call = 0
 
@@ -204,9 +247,10 @@ class UlyssesFusedAttention:
     def __call__(self, attn, query, key, value, *, joint_tensor_query=None, joint_tensor_key=None,
                  joint_tensor_value=None, joint_strategy="none", top_k=0, text_amp=0.0,
                  block_neighbor_list=None, p_remain_rates=0.0, cu_seqlens_q=None, cu_seqlens_kv=None,
-                 _hooks=None, **_unused):
+                 first_frame_blocks=0, dense=False, seq_len=None, _hooks=None, **_unused):
         import ctypes as C
         from . import _lib
+        from . import attention as A
         from ._lib import check, lib
         from .attention import _stream_ptr, block_sparse_attention_variant
         P, r = _group_size_rank(self.group)
@@ -222,16 +266,23 @@ class UlyssesFusedAttention:
             raise ValueError("joint_tensor_query/key/value must be given together")
         T = joint_tensor_query.shape[1] if joint else 0
         N = P * n
+        L = _valid_rows(seq_len, N, n, T, dense, first_frame_blocks)
         dev, dt = query.device, query.dtype
         qkv, h_qkv, p_qkv, outs = self._buffers(N, T, h, D, n, H, dt, dev)
         out, h_out, p_out = outs[self._call & 1]
         self._call += 1
-        G = self._n_groups(h, self.groups, (N + T + BLOCK - 1) // BLOCK)
+        # this rank's pad rows (global rows >= L): no rank stores them, so they are zeroed whenever the
+        # buffer is first used at this L
+        pad0 = min(n, max(0, L - r * n))
+        if self._pad_len.get(out.data_ptr(), N) != L and pad0 < n:
+            out[pad0:n].zero_()
+        self._pad_len[out.data_ptr()] = L
+        G = self._n_groups(h, self.groups, (L + T + BLOCK - 1) // BLOCK)
         hg = h // G
         xs = [t[0] for t in (query, key, value)]
         for t in xs:
-            if t.stride(2) != 1 or t.stride(1) != D:
-                raise ValueError("q/k/v must be [1, n, H, D] views with contiguous heads")
+            if t.stride(2) != 1 or t.stride(1) != D or t.stride(0) != xs[0].stride(0):
+                raise ValueError("q/k/v must be [1, n, H, D] views with contiguous heads and one row stride")
         a = _lib.JengaUlyssesScatterArgs()
         a.x = (C.c_void_p * 3)(*[t.data_ptr() for t in xs])
         a.x_stride_s = xs[0].stride(0)
@@ -275,11 +326,18 @@ class UlyssesFusedAttention:
                 main.wait_event(events[g])
             sl = slice(g * hg, (g + 1) * hg)
             sp = dict(world=P, rank=r, heads_total=H, rows=n, peers=p_out, head_base=r * h + g * hg)
-            block_sparse_attention_variant(self.variant, qkv[0][None, :, sl], qkv[1][None, :, sl], qkv[2][None, :, sl],
-                                           top_k, cu_seqlens_q=cu, cu_seqlens_kv=cu,
-                                           text_blocks=(T + BLOCK - 1) // BLOCK, text_amp=text_amp,
-                                           block_neighbor_list=block_neighbor_list,
-                                           p_remain_rates=p_remain_rates, sp_out=sp)
+            q, k, v = (x[None, :L + T, sl] for x in qkv)       # all N + T rows without seq_len
+            if dense:
+                # flash_attn_shim._dense's launch, with the peer-store epilogue instead of `out`
+                v8, qk8 = A.quantize_operands(q, k, v, A.PV_FP8, A.QK_INT8)
+                A._launch(q, k, v, None, 0, (L + BLOCK - 1) // BLOCK, D ** -0.5, 0.0, 1 << 30, L, L, L, None,
+                          None, q.dtype, sp_out=sp, v_fp8=v8, qk_int8=qk8)
+            else:
+                block_sparse_attention_variant(self.variant, q, k, v, top_k, cu_seqlens_q=cu, cu_seqlens_kv=cu,
+                                               text_blocks=(T + BLOCK - 1) // BLOCK, text_amp=text_amp,
+                                               block_neighbor_list=block_neighbor_list,
+                                               p_remain_rates=p_remain_rates, first_frame_blocks=first_frame_blocks,
+                                               sp_out=sp)
             if "post_attention" in hooks:
                 # per-group completion across ranks, so the caller may drain this group's heads
                 h_out.barrier(channel=0)
