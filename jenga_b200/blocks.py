@@ -12,6 +12,8 @@ reference module is executed,
   WanSelfAttention.forward            (wan/modules/model_mul.py:134-180)
   WanT2VCrossAttention.forward        (wan/modules/model_mul.py:183-205)
   WanAttentionBlock.forward           (wan/modules/model_mul.py:303-346)
+  WanSelfAttention.forward / WanAttentionBlock.forward of wan/modules/model.py (:127-156, :274-313),
+      the plain model WanI2V loads, only under install(wan_sp=True)
 
 with versions whose attention section is `jenga_hy_prologue` / `jenga_wan_prologue` (RMSNorm +
 RoPE + img||txt concatenation + block pooling in one pass over the QKV projection output)
@@ -23,7 +25,9 @@ no RMS qk-norm, unusual dtype, batch > 1 for Wan, the reference's own sequence p
 ORIGINAL forward runs, with the caller's own arguments (`_patched`).  An I2V block with `jenga_sp` set
 (the Hilbert-sharded forward of hyi2v_sp.py) routes its attention section through that Ulysses object
 and has no such fall-back; so does a WanSelfAttention with `jenga_sp` set (the Hilbert-sharded Wan
-forward of wan_sp.py), whose carved and dense calls both go through the exchange.
+forward of wan_sp.py), whose carved and dense calls both go through the exchange; and so does a
+plain-module WanSelfAttention under `jenga_sp` (the raster-sharded I2V forward of wan_sp.py), whose
+block then runs the fused I2V cross-attention on the rank's rows or raises.
 
 The I2V blocks differ from the HunyuanVideo ones in three ways the fused forwards follow: the
 token-replace modulation (rows of the first frame take the `tr_` shift / scale / gate; the
@@ -69,6 +73,10 @@ I2V_SP = False
 # opt-in (install(wan_sp=True) / JENGA_WAN_SP=1): wan/distributed/xdit_context_parallel.py's
 # usp_dit_forward / usp_attn_forward are swapped for the Hilbert-sharded TeaCache forward of wan_sp.py
 _WAN_SP_MODULES = ("wan.distributed.xdit_context_parallel",)
+# under the same switch: wan/modules/model.py, the plain Wan model WanI2V loads (image2video.py:21), gets
+# the fused WanAttentionBlock.forward and a WanSelfAttention.forward for its signatures; without the
+# switch it is not touched
+_WAN_PLAIN_MODULES = ("wan.modules.model",)
 WAN_SP = False
 
 
@@ -93,16 +101,22 @@ def set_wan_sp(on: bool) -> None:
     if not WAN_SP and xdit is not None:
         from .wan_sp import uninstall_usp
         uninstall_usp(xdit)
+    plain = sys.modules.get(_WAN_PLAIN_MODULES[0])
+    if not WAN_SP and plain is not None:
+        for cls in ("WanSelfAttention", "WanAttentionBlock"):
+            fn = getattr(getattr(plain, cls, None), "forward", None)
+            if getattr(fn, "__jenga_b200__", False):
+                getattr(plain, cls).forward = fn.__wrapped__
 
 
 def _sp_modules():
-    return (_I2V_SP_MODULES if I2V_SP else ()) + (_WAN_SP_MODULES if WAN_SP else ())
+    return (_I2V_SP_MODULES if I2V_SP else ()) + (_WAN_SP_MODULES + _WAN_PLAIN_MODULES if WAN_SP else ())
 
 
 STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "i2v_double_sp": 0,
          "i2v_single_sp": 0, "wan_self": 0, "wan_self_sp": 0, "wan_self_dense_sp": 0, "fallback": 0,
          "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0,
-         "wan_i2v_cross": 0, "linear_fp8": 0}
+         "wan_i2v_cross": 0, "linear_fp8": 0, "wan_i2v_self_sp": 0, "wan_i2v_cross_sp": 0}
 # the CLIP image tokens at the head of the Wan2.1-I2V context (model_mul.py:230-231)
 _WAN_I2V_IMG_TOKENS = 257
 # the HunyuanVideo-I2V operator's text_blocks default (hyvideo_i2v/…/attention_block_triton_diffres.py:409);
@@ -423,12 +437,13 @@ def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=Non
 # Wan blocks
 # ------------------------------------------------------------------------------------------------
 def _wan_self_sp(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates, freq_remap,
-                 block_neighbor_list):
+                 block_neighbor_list, stat=None):
     """WanSelfAttention.forward on a rank's n rows of the Hilbert-sharded Wan forward (wan_sp.py): the
     norm + RoPE prologue on the rank's rows, then the Ulysses exchange and the operator over the first
     L (the global token count) exchanged rows.  top_k and first_frame_blocks follow the single-GPU rule
     over L (model_mul.py:161-164); sa_drop_rate <= 0.25 (:153, the warm-up steps) runs the dense class
-    over the same exchange.  No fall-back: the original forward would attend over the rank's rows."""
+    over the same exchange.  No fall-back: the original forward would attend over the rank's rows.
+    stat: the STATS key of the call (default: the T2V route's, by class)."""
     b, n = x.shape[:2]
     wq = getattr(self.norm_q, "weight", None)
     wk = getattr(self.norm_k, "weight", None)
@@ -453,11 +468,28 @@ def _wan_self_sp(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens
     top_k, ff = (0, 0) if dense else WAN.block_counts(L, sa_drop_rate)
     out = jsp(None, q, k, v, top_k=top_k, block_neighbor_list=None if dense else block_neighbor_list,
               p_remain_rates=p_remain_rates, first_frame_blocks=ff, dense=dense, seq_len=L)
-    STATS["wan_self_dense_sp" if dense else "wan_self_sp"] += 1
+    STATS[stat or ("wan_self_dense_sp" if dense else "wan_self_sp")] += 1
     out = out.flatten(2)
     if not torch.is_autocast_enabled():
         out = out.float()       # the query dtype the reference returns, as in _wan_self
     return self.o(out)
+
+
+def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs):
+    """WanSelfAttention.forward of wan/modules/model.py (:127-156), hooked only under install(wan_sp=True).
+    Under `jenga_sp` (the raster-sharded I2V forward, wan_sp.parallelize_wan_i2v) x holds rank r's n rows
+    [r*n, min((r+1)*n, L)): the fused prologue runs on them with that raster slice as the RoPE index (pad
+    rows index row 0), then the dense class over the first L exchanged rows, so the pad keys are excluded
+    as flash_attention(k_lens=seq_lens) excludes them on one GPU.  Without jenga_sp: the original forward."""
+    jsp = getattr(self, "jenga_sp", None)
+    if jsp is None:
+        return None
+    _, r = U._group_size_rank(jsp.group)
+    n = x.shape[1]
+    L = int(torch.prod(grid_sizes[0]))
+    rows = torch.arange(r * n, (r + 1) * n, device=x.device)
+    remap = torch.where(rows < L, rows, torch.zeros_like(rows))
+    return _wan_self_sp(self, jsp, x, grid_sizes, freqs, 0.0, 128, 0.0, remap, None, stat="wan_i2v_self_sp")
 
 
 def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128, p_remain_rates=0.8,
@@ -528,7 +560,7 @@ def wan_i2v_cross_eligible(ca, x, context, context_lens):
     return _wan_i2v_cross_shape_ok(ca, x, context, context_lens) and x.is_cuda and DN._autocast_bf16()
 
 
-def _wan_i2v_cross(ca, x, context, context_lens):
+def _wan_i2v_cross(ca, x, context, context_lens, stat="wan_i2v_cross"):
     """WanI2VCrossAttention.forward (model_mul.py:223-249) with its attention part as one
     jenga_wan_i2v_cross_attn launch; the module's own q / k / v / k_img / v_img / o Linears run around
     it.  Anything else runs the module's own forward."""
@@ -542,7 +574,7 @@ def _wan_i2v_cross(ca, x, context, context_lens):
             out = WAN.i2v_cross_attention(q_lin, k_lin, v.view(1, -1, n, 128), kimg_lin, vimg.view(1, -1, n, 128),
                                           ca.norm_q.weight, ca.norm_k.weight, ca.norm_k_img.weight, n,
                                           eps=float(ca.norm_q.eps))
-            STATS["wan_i2v_cross"] += 1
+            STATS[stat] += 1
             return ca.o(out.flatten(2))
     STATS["fallback"] += 1
     return ca(x, context, context_lens)
@@ -550,10 +582,40 @@ def _wan_i2v_cross(ca, x, context, context_lens):
 
 def _wan_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=0.0, freq_remap=None,
                block_neighbor_list=None, p_remain_rates=0.0):
+    return _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens,
+                           dict(sa_drop_rate=sa_drop_rate, freq_remap=freq_remap,
+                                block_neighbor_list=block_neighbor_list, p_remain_rates=p_remain_rates))
+
+
+def _wan_plain_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens):
+    """WanAttentionBlock.forward of wan/modules/model.py (:274-313), hooked only under install(wan_sp=True):
+    the fused body, with the self-attention called in that module's signature.  Under `self_attn.jenga_sp`
+    (parallelize_wan_i2v) x is a rank's rows and there is no fall-back: the checks run before the
+    exchange, so every rank raises alike."""
+    if getattr(self.self_attn, "jenga_sp", None) is None:
+        return _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, {})
+    if not (type(self.cross_attn).__name__ == "WanI2VCrossAttention"
+            and _wan_i2v_cross_shape_ok(self.cross_attn, x, context, context_lens)):
+        raise RuntimeError(f"{type(self).__name__} under jenga_sp: the cross-attention is not one the fused I2V "
+                           "kernel takes (a WanI2VCrossAttention with WanRMSNorm q / k / k_img norms, head_dim "
+                           f"128, batch 1, context_lens None and more than {_WAN_I2V_IMG_TOKENS} context rows); "
+                           "the sharded I2V forward has no fall-back")
+    out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, {}, sharded=True)
+    if out is None:
+        raise RuntimeError(f"{type(self).__name__} under jenga_sp: the call is not one the fused block takes (a "
+                           "CUDA input under bf16 autocast, fp32 modulation, cross_attn_norm=True); the sharded "
+                           "I2V forward has no fall-back")
+    return out
+
+
+def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded=False):
+    """attn_kw: the Jenga self-attention arguments of model_mul.py (empty for wan/modules/model.py).
+    sharded: the I2V rows of parallelize_wan_i2v; the cross-attention must then be the fused one."""
     i2v = type(self.cross_attn).__name__ == "WanI2VCrossAttention"
     ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
           and (i2v or type(self.cross_attn).__name__ == "WanT2VCrossAttention")
-          and self.modulation.dtype == torch.float32)
+          and self.modulation.dtype == torch.float32
+          and (not sharded or wan_i2v_cross_eligible(self.cross_attn, x, context, context_lens)))
     if ok:
         with torch.autocast("cuda", dtype=torch.float32):                      # :326-327
             e6 = self.modulation + e
@@ -566,12 +628,12 @@ def _wan_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, s
     e = e6.chunk(6, dim=1)
     # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to
     y = self.self_attn(DN.wan_ln_modulate(x, e[0], e[1], eps=self.norm1.eps), seq_lens, grid_sizes, freqs,
-                       sa_drop_rate=sa_drop_rate, freq_remap=freq_remap, block_neighbor_list=block_neighbor_list,
-                       p_remain_rates=p_remain_rates)                          # :331-333
+                       **attn_kw)                                              # :331-333
     x, h = DN.wan_residual_ln(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight,
                               bias=self.norm3.bias)                            # :334-335, :339
     # WanI2VCrossAttention.forward itself stays unpatched: the block routes it here
-    cross = _wan_i2v_cross(self.cross_attn, h, context, context_lens) if i2v else \
+    cross = _wan_i2v_cross(self.cross_attn, h, context, context_lens,
+                           stat="wan_i2v_cross_sp" if sharded else "wan_i2v_cross") if i2v else \
         self.cross_attn(h, context, context_lens)
     x, h = DN.wan_residual_ln(x, cross, None, eps=self.norm2.eps, shift=e[3], scale=e[4])   # :339-340
     STATS["wan_block"] += 1
@@ -605,6 +667,13 @@ def patch_module(mod) -> list[str]:
         from .wan_sp import install_usp
         return [f"{name}.usp_dit_forward", f"{name}.usp_attn_forward"] if WAN_SP and install_usp(mod) else []
     fused = {}
+    if name in _WAN_PLAIN_MODULES:
+        if not WAN_SP:
+            return []
+        # the block hands its self-attention (x, seq_lens, grid_sizes, freqs) and runs the fused I2V
+        # cross-attention; WanT2VCrossAttention and WanI2VCrossAttention stay as they are
+        fused.update(WanSelfAttention=_wan_i2v_self, WanAttentionBlock=_wan_plain_block)
+        return _patch_classes(mod, fused)
     if name.startswith(("hyvideo.", "hyvideo_i2v.")):
         # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
         # a ragged S with four text blocks: its own pair of entry points
@@ -614,11 +683,15 @@ def patch_module(mod) -> list[str]:
     # WanI2VCrossAttention overrides forward itself and is left as it is; the fused block forward runs
     # its fused form (_wan_i2v_cross)
     fused.update(WanSelfAttention=_wan_self, WanT2VCrossAttention=_wan_cross, WanAttentionBlock=_wan_block)
+    return _patch_classes(mod, fused)
+
+
+def _patch_classes(mod, fused) -> list[str]:
     done = []
     for cls, body in fused.items():
         if hasattr(mod, cls) and not getattr(getattr(mod, cls).forward, "__jenga_b200__", False):
             getattr(mod, cls).forward = _patched(getattr(mod, cls).forward, body)
-            done.append(f"{name}.{cls}.forward")
+            done.append(f"{mod.__name__}.{cls}.forward")
     return done
 
 
