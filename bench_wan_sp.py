@@ -9,7 +9,8 @@ over the N ranks of `torchrun --nproc-per-node N`.
           the Ulysses exchange (peer stores, or the NCCL all-to-all where symmetric memory is unavailable)
 
 Same inputs as bench_wan_blocks.py --model 14b (grid 21x45x80, 512 context tokens, p_remain_rates 0.8,
-bf16 autocast), in two legs each: the carved leg at sa_drop_rate 0.7 and the dense leg at 0.2 (the
+bf16 autocast); --model 1.3b takes Wan2.1-1.3B's blocks (dim 1536, 12 heads, FFN 8960) at its 480p grid
+21x30x52, where 8 ranks need the ragged head split (JENGA_ULYSSES_RAGGED=1: 2,2,2,2,1,1,1,1 heads), in two legs each: the carved leg at sa_drop_rate 0.7 and the dense leg at 0.2 (the
 warm-up steps, model_mul.py:153).  Reports seconds per stack (the slowest rank, CUDA events), the SM
 clock at the start and end of each leg, and the distance of the gathered sp rows from the single-GPU
 rows in units of their RMS.  The sp leg's timed region is the block stack plus the all-gather of the
@@ -17,7 +18,7 @@ rows that the sharded forward adds once per forward (here of the stack's output 
 gathers the head's 64 output channels instead); the Hilbert gather, the slicing of the inputs and the
 inverse scatter are outside both legs.  Rank 0 prints one JSON line; nothing is written to the tree.
 
-    torchrun --nproc-per-node N bench_wan_sp.py [--blocks 4] [--reps 3]
+    torchrun --nproc-per-node N bench_wan_sp.py [--model 14b|1.3b] [--blocks 4] [--reps 3]
 """
 from __future__ import annotations
 
@@ -34,12 +35,15 @@ ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "tests"))
 
+MODELS = {"14b": (5120, 40, 13824, "21,45,80"), "1.3b": (1536, 12, 8960, "21,30,52")}   # dim, heads, FFN, grid
+
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--blocks", type=int, default=4, help="blocks in the stack")
     ap.add_argument("--reps", type=int, default=3, help="timed stack forwards per leg")
-    ap.add_argument("--grid", default="21,45,80", help="latent f,h,w (after patching)")
+    ap.add_argument("--model", choices=sorted(MODELS), default="14b", help="Wan2.1 block shapes")
+    ap.add_argument("--grid", default=None, help="latent f,h,w (after patching); default: the model's")
     args = ap.parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit("bench_wan_sp.py measures on GPUs; none is visible")
@@ -56,8 +60,9 @@ def main(argv=None):
     from jenga_b200.hyi2v_sp import default_attention, shard
     from jenga_b200.wan_sp import _check_world, shard_rows
 
-    f, h, w = (int(v) for v in args.grid.split(","))
-    dim, heads, ffn, p_remain, Lc = 5120, 40, 13824, 0.8, 512
+    dim, heads, ffn, grid_default = MODELS[args.model]
+    f, h, w = (int(v) for v in (args.grid or grid_default).split(","))
+    p_remain, Lc = 0.8, 512
     drops = {"carved": 0.7, "dense": 0.2}
     L = f * h * w
     _check_world(heads, P)

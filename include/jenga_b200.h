@@ -237,6 +237,18 @@ typedef struct JengaUlyssesScatterArgs {
 
 int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* args, void* stream);
 
+/* Ragged head split: the same exchange when `world` need not divide `heads`.
+ * head_offsets_host (HOST array of world+1 int32) gives rank p the global heads
+ * [off[p], off[p+1]); offsets run monotone from 0 to `heads` and no group exceeds
+ * slots = ceil(heads/world) (jenga_b200.ulysses.head_offsets: sizes heads/world + (p < heads%world)).
+ * Every rank's receive buffer is [3, world*n_loc + n_text, slots, head_dim]; slot s of rank p holds
+ * global head off[p] + s, for s < off[p+1]-off[p] only (the other slots are not written).
+ * head_begin/head_count select a slot range (head_count == 0: all slots); each destination takes
+ * its intersection with its own group, which may be empty.  Text rows copy the local heads
+ * [off[rank] + s).  With off[p] = p*heads/world the bytes written equal jenga_ulysses_scatter's. */
+int jenga_ulysses_scatter_ragged(const JengaUlyssesScatterArgs* args, const int32_t* head_offsets_host,
+                                 void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Host <-> device staging for callers whose q/k/v live in (pinned) host memory: a strided 2-D
  * copy on `stream` (cudaMemcpy2DAsync), used to move one head group of a [B,S,H,D] tensor

@@ -179,6 +179,8 @@ def _load() -> C.CDLL:
     lib.jenga_copy2d_async.restype = C.c_int
     lib.jenga_ulysses_scatter.argtypes = [C.POINTER(JengaUlyssesScatterArgs), C.c_void_p]
     lib.jenga_ulysses_scatter.restype = C.c_int
+    lib.jenga_ulysses_scatter_ragged.argtypes = [C.POINTER(JengaUlyssesScatterArgs), C.c_void_p, C.c_void_p]
+    lib.jenga_ulysses_scatter_ragged.restype = C.c_int
     lib.jenga_block_neighbors_from_mapping_host.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int,
                                                             C.c_void_p, C.c_void_p]
     lib.jenga_block_neighbors_from_mapping_host.restype = C.c_int

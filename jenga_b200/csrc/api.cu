@@ -145,6 +145,58 @@ ulysses_scatter_kernel(const ScatterParams p) {
   }
 }
 
+// Ragged form: destination p owns `cnt[p]` heads of this call, starting at slot hg0 of its
+// group, whose global head 0 is off[p]; cstart[p] is the prefix of cnt (in heads) within one
+// image token's vectors.  Every buffer has `slots` head slots.
+struct ScatterRaggedParams {
+  const uint4* x[3];
+  const uint4* joint[3];
+  long long x_stride_v, joint_stride_v;
+  int world, rank, slots, vec_per_head;
+  int hg0;
+  int off[9], cnt[8], cstart[9];   // cstart[world] = heads moved per image token
+  long long n_loc, n_text;
+  unsigned long long peer[8];
+};
+__global__ void __launch_bounds__(256)
+ulysses_scatter_ragged_kernel(const ScatterRaggedParams p) {
+  const int w = blockIdx.y;  // 0:q 1:k 2:v
+  const int vec_per_tok = p.cstart[p.world] * p.vec_per_head;
+  const long long n_total = static_cast<long long>(p.world) * p.n_loc + p.n_text;
+  const long long img_vecs = p.n_loc * vec_per_tok;
+  const int txt_per_tok = p.cnt[p.rank] * p.vec_per_head;
+  const long long txt_vecs = p.n_text * static_cast<long long>(txt_per_tok);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < img_vecs + txt_vecs;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    if (i < img_vecs) {
+      const long long tok = i / vec_per_tok;
+      const int c = static_cast<int>(i - tok * vec_per_tok);
+      const int j = c / p.vec_per_head;                          // head of this token's call
+      const int v_in_head = c - j * p.vec_per_head;
+      int dst_rank = 0;
+      while (j >= p.cstart[dst_rank + 1]) ++dst_rank;
+      const int slot = p.hg0 + (j - p.cstart[dst_rank]);
+      const int head = p.off[dst_rank] + slot;                   // global head = column of x
+      const uint4 v = __ldg(p.x[w] + tok * p.x_stride_v + head * p.vec_per_head + v_in_head);
+      uint4* dst = reinterpret_cast<uint4*>(p.peer[dst_rank]) +
+                   ((static_cast<long long>(w) * n_total + p.rank * p.n_loc + tok) * p.slots + slot) * p.vec_per_head +
+                   v_in_head;
+      *dst = v;
+    } else {
+      const long long k = i - img_vecs;
+      const long long tok = k / txt_per_tok;
+      const int r = static_cast<int>(k - tok * txt_per_tok);
+      const int slot = p.hg0 + r / p.vec_per_head;
+      const int v_in_head = r - (r / p.vec_per_head) * p.vec_per_head;
+      const uint4 v = __ldg(p.joint[w] + tok * p.joint_stride_v + (p.off[p.rank] + slot) * p.vec_per_head + v_in_head);
+      uint4* dst = reinterpret_cast<uint4*>(p.peer[p.rank]) +
+                   ((static_cast<long long>(w) * n_total + p.world * p.n_loc + tok) * p.slots + slot) * p.vec_per_head +
+                   v_in_head;
+      *dst = v;
+    }
+  }
+}
+
 }  // namespace jenga
 
 using namespace jenga;
@@ -278,6 +330,60 @@ extern "C" int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* a, void* str
   ulysses_scatter_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   cudaError_t ce = cudaGetLastError();
   return ce == cudaSuccess ? JENGA_OK : set_cuda_error(ce, "ulysses_scatter launch");
+}
+
+extern "C" int jenga_ulysses_scatter_ragged(const JengaUlyssesScatterArgs* a, const int32_t* off, void* stream) {
+  if (!a || !off || !a->x[0] || !a->x[1] || !a->x[2] || !a->peer_qkv_host)
+    return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: null pointer");
+  if (a->world <= 0 || a->world > 8 || a->rank < 0 || a->rank >= a->world || a->heads <= 0 ||
+      a->head_dim % 8 || a->n_loc <= 0 || a->n_text < 0 || a->x_stride_s % 8 || a->joint_stride_s % 8)
+    return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: bad shape (world must be 1..8)");
+  if (a->n_text > 0 && (!a->joint[0] || !a->joint[1] || !a->joint[2]))
+    return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: joint tensors missing");
+  if (off[0] != 0 || off[a->world] != a->heads)
+    return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: head offsets must run from 0 to heads (%d), got %d..%d",
+                     a->heads, off[0], off[a->world]);
+  const int slots = (a->heads + a->world - 1) / a->world;
+  for (int r = 0; r < a->world; ++r) {
+    if (off[r + 1] < off[r])
+      return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: head offsets decrease at rank %d", r);
+    if (off[r + 1] - off[r] > slots)
+      return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: rank %d's group of %d heads exceeds the %d slots",
+                       r, off[r + 1] - off[r], slots);
+  }
+  for (int r = 0; r < a->world; ++r)
+    if (!a->peer_qkv_host[r] || a->peer_qkv_host[r] % 16)
+      return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: peer_qkv_host[%d] is null or not 16-byte aligned", r);
+  ScatterRaggedParams p{};
+  for (int w = 0; w < 3; ++w) {
+    p.x[w] = static_cast<const uint4*>(a->x[w]);
+    p.joint[w] = static_cast<const uint4*>(a->joint[w]);
+  }
+  p.x_stride_v = a->x_stride_s / 8;
+  p.joint_stride_v = a->joint_stride_s / 8;
+  p.world = a->world; p.rank = a->rank; p.slots = slots; p.vec_per_head = a->head_dim / 8;
+  p.hg0 = a->head_count > 0 ? a->head_begin : 0;
+  const int hg = a->head_count > 0 ? a->head_count : slots;
+  if (p.hg0 < 0 || p.hg0 + hg > slots)
+    return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: slot range out of range");
+  p.cstart[0] = 0;
+  for (int r = 0; r < a->world; ++r) {
+    const int end = off[r + 1] - off[r] < p.hg0 + hg ? off[r + 1] - off[r] : p.hg0 + hg;
+    p.off[r] = off[r];
+    p.cnt[r] = end > p.hg0 ? end - p.hg0 : 0;
+    p.cstart[r + 1] = p.cstart[r] + p.cnt[r];
+  }
+  p.off[a->world] = off[a->world];
+  p.n_loc = a->n_loc; p.n_text = a->n_text;
+  for (int r = 0; r < a->world; ++r) p.peer[r] = a->peer_qkv_host[r];
+  const long long total = (a->n_loc * p.cstart[a->world] + a->n_text * p.cnt[a->rank]) * p.vec_per_head;
+  if (total == 0) return JENGA_OK;
+  long long blocks = (total + 255) / 256;
+  if (blocks > static_cast<long long>(kNumSMs) * 16) blocks = static_cast<long long>(kNumSMs) * 16;
+  dim3 grid(static_cast<unsigned>(blocks), 3);
+  ulysses_scatter_ragged_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  cudaError_t ce = cudaGetLastError();
+  return ce == cudaSuccess ? JENGA_OK : set_cuda_error(ce, "ulysses_scatter_ragged launch");
 }
 
 extern "C" int64_t jenga_select_blocks_workspace_bytes(int32_t batch_heads, int32_t nq, int32_t n_img) {

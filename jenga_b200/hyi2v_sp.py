@@ -32,8 +32,13 @@ STEP_CALC = (0, 1, 2, 3, 5, 7, 10, 13, 16, 19, 22, 25, 28, 31, 34, 37, 40, 42, 4
 def check_degree(img_tokens: int, heads: int, world: int, model: str = "HunyuanVideo-I2V") -> None:
     """The layout needs whole head groups per rank and, for a non-zero img_tokens, whole image slices
     per rank.  `model` names the model in the message (the Wan route, wan_sp.py, pads its slices
-    instead and passes 0)."""
-    if heads % world:
+    instead and passes 0).  Under the ragged head split (ulysses.RAGGED_HEADS) any head count of at
+    least `world` is accepted."""
+    from .ulysses import ragged
+    if ragged(heads, world) and heads < world:
+        raise ValueError(f"sequence-parallel {model}: {heads} attention heads over {world} ranks leave a rank "
+                         "without a head")
+    if heads % world and not ragged(heads, world):
         raise ValueError(f"sequence-parallel {model}: {heads} attention heads do not split over "
                          f"{world} ranks (the degree must divide the head count)")
     if img_tokens % world:

@@ -24,22 +24,76 @@ other call as it was:
   seq_len             the global valid length L when the ranks' equal slices are zero-padded
                       (P*n_loc > L): the operator sees the first L rows only, so its blocks, pooling
                       and limits are those of one GPU; the result rows past L are zero
+
+Ragged head split (opt-in: RAGGED_HEADS = True or JENGA_ULYSSES_RAGGED=1): a degree P that does not
+divide the head count H.  Rank r owns the contiguous heads head_offsets(H, P)[r:r+2], ⌈H/P⌉ heads on
+the first H % P ranks and ⌊H/P⌋ on the others; the ranks with fewer heads wait for the others at the
+end of every call.  Without the switch such a degree is refused as before; with it and P | H nothing
+changes (the same launches, the same bytes).
 """
 from __future__ import annotations
+
+import os
 
 import torch
 import torch.distributed as dist
 
 BLOCK = 128
 
+RAGGED_HEADS: bool = os.environ.get("JENGA_ULYSSES_RAGGED", "0") == "1"
+
+
+def head_offsets(heads: int, world: int) -> tuple[int, ...]:
+    """The head assignment of every Ulysses layout: rank r owns the global heads [off[r], off[r+1]),
+    h_r = heads//world + (r < heads%world) of them (larger groups first; r*heads/world when world
+    divides heads)."""
+    q, m = divmod(heads, world)
+    return tuple(r * q + min(r, m) for r in range(world + 1))
+
+
+def ragged(heads: int, world: int) -> bool:
+    """True when this call takes the ragged head split: the switch is on and world does not divide
+    heads.  The refusals of the divisible layout stay in force while this is False."""
+    return RAGGED_HEADS and heads % world != 0
+
 
 def _group_size_rank(group):
     return dist.get_world_size(group), dist.get_rank(group)
 
 
-def seq_to_heads(x: torch.Tensor, group=None, out: torch.Tensor | None = None) -> torch.Tensor:
+def _layout(H: int, P: int, r: int):
+    """(offsets or None, my head count, my first head, head slots of the receive buffer); offsets is
+    None for the divisible layout, whose refusals stay where they were"""
+    if not ragged(H, P):
+        return None, H // P, r * (H // P), H // P
+    if H < P:
+        raise ValueError(f"{H} attention heads over {P} ranks: the ragged split needs a head on every rank")
+    off = head_offsets(H, P)
+    return off, off[r + 1] - off[r], off[r], off[1]
+
+
+def _seq_to_heads_ragged(x, group, off, out):
+    P, r = _group_size_rank(group)
+    B, n, H, D = x.shape
+    h = off[r + 1] - off[r]
+    send = torch.cat([x[:, :, off[p]:off[p + 1]].reshape(-1) for p in range(P)])     # [p][B, n, h_p, D]
+    recv = torch.empty(P * B * n * h * D, dtype=x.dtype, device=x.device)
+    dist.all_to_all_single(recv, send, output_split_sizes=[B * n * h * D] * P,
+                           input_split_sizes=[B * n * (off[p + 1] - off[p]) * D for p in range(P)], group=group)
+    y = recv.view(P, B, n, h, D).permute(1, 0, 2, 3, 4).reshape(B, P * n, h, D)
+    if out is not None:
+        out.copy_(y)
+        return out
+    return y
+
+
+def seq_to_heads(x: torch.Tensor, group=None, out: torch.Tensor | None = None,
+                 offsets: tuple[int, ...] | None = None) -> torch.Tensor:
     """[B, n_loc, H, D] (all heads, my token slice) -> [B, P*n_loc, H/P, D] (my heads, all
-    tokens, slices concatenated in rank order).  == SeqAllToAll4D(scatter_idx=2, gather_idx=1)."""
+    tokens, slices concatenated in rank order).  == SeqAllToAll4D(scatter_idx=2, gather_idx=1).
+    offsets (head_offsets(H, P)): the ragged form, my heads [offsets[r], offsets[r+1])."""
+    if offsets is not None:
+        return _seq_to_heads_ragged(x, group, offsets, out)
     P, _ = _group_size_rank(group)
     B, n, H, D = x.shape
     assert H % P == 0, "heads must divide by the SP degree"
@@ -58,8 +112,20 @@ def seq_to_heads(x: torch.Tensor, group=None, out: torch.Tensor | None = None) -
     return y
 
 
-def heads_to_seq(x: torch.Tensor, group=None) -> torch.Tensor:
-    """[B, P*n_loc, H/P, D] -> [B, n_loc, H, D].  == SeqAllToAll4D(scatter_idx=1, gather_idx=2)."""
+def heads_to_seq(x: torch.Tensor, group=None, offsets: tuple[int, ...] | None = None) -> torch.Tensor:
+    """[B, P*n_loc, H/P, D] -> [B, n_loc, H, D].  == SeqAllToAll4D(scatter_idx=1, gather_idx=2).
+    offsets: the ragged form ([B, P*n_loc, h_r, D] in, rank p's heads at [offsets[p], offsets[p+1]))."""
+    if offsets is not None:
+        P, _ = _group_size_rank(group)
+        B, N, h, D = x.shape
+        n = N // P
+        hs = [offsets[p + 1] - offsets[p] for p in range(P)]
+        send = x.reshape(B, P, n, h, D).permute(1, 0, 2, 3, 4).contiguous().reshape(-1)
+        recv = torch.empty(B * n * offsets[P] * D, dtype=x.dtype, device=x.device)
+        dist.all_to_all_single(recv, send, output_split_sizes=[B * n * hp * D for hp in hs],
+                               input_split_sizes=[B * n * h * D] * P, group=group)
+        parts = recv.split([B * n * hp * D for hp in hs])
+        return torch.cat([t.view(B, n, hp, D) for t, hp in zip(parts, hs)], dim=2)
     P, _ = _group_size_rank(group)
     B, N, h, D = x.shape
     assert N % P == 0
@@ -89,8 +155,20 @@ def _dense_shim(q, k, v):
     return flash_attn_func(q, k, v)
 
 
-def gather_heads(x: torch.Tensor, group=None) -> torch.Tensor:
-    """[B, T, H/P, D] on every rank (different head groups) -> [B, T, H, D] everywhere."""
+def gather_heads(x: torch.Tensor, group=None, offsets: tuple[int, ...] | None = None) -> torch.Tensor:
+    """[B, T, H/P, D] on every rank (different head groups) -> [B, T, H, D] everywhere.
+    offsets: the ragged form, [B, T, h_r, D] in; padded to the largest group for the all-gather."""
+    if offsets is not None:
+        P, _ = _group_size_rank(group)
+        B, T, h, D = x.shape
+        hs = [offsets[p + 1] - offsets[p] for p in range(P)]
+        slots = max(hs)
+        pad = x.new_zeros((B, T, slots, D))
+        pad[:, :, :h] = x
+        recv = torch.empty((P * B, T, slots, D), dtype=x.dtype, device=x.device)
+        dist.all_gather_into_tensor(recv, pad, group=group)
+        recv = recv.view(P, B, T, slots, D)
+        return torch.cat([recv[p, :, :, :hp] for p, hp in enumerate(hs)], dim=2)
     P, _ = _group_size_rank(group)
     B, T, h, D = x.shape
     recv = torch.empty((P * B, T, h, D), dtype=x.dtype, device=x.device)
@@ -123,7 +201,7 @@ class UlyssesCarvedAttention:
                  first_frame_blocks=0, dense=False, seq_len=None, **_unused):
         P, r = _group_size_rank(self.group)
         B, q_len, H, D = query.shape
-        h = H // P
+        off, h, b, _ = _layout(H, P, r)
         joint = joint_tensor_query is not None
         if joint and joint_strategy != "rear":
             # the reference also implements "front"; Jenga's blocks only ever pass "rear"
@@ -137,9 +215,9 @@ class UlyssesCarvedAttention:
         # receive buffers already shaped [B, N+T, h, D] so text rows are appended in place
         qkv = [torch.empty((B, N + T, h, D), dtype=dt, device=dev) for _ in range(3)]
         for buf, x in zip(qkv, (query, key, value)):
-            seq_to_heads(x, self.group, out=buf[:, :N])
+            seq_to_heads(x, self.group, out=buf[:, :N], offsets=off)
         if joint:
-            sl = slice(r * h, (r + 1) * h)
+            sl = slice(b, b + h)
             qkv[0][:, N:] = joint_tensor_query[:, :, sl]
             qkv[1][:, N:] = joint_tensor_key[:, :, sl]
             qkv[2][:, N:] = joint_tensor_value[:, :, sl]
@@ -165,10 +243,10 @@ class UlyssesCarvedAttention:
             full = torch.zeros((B, N, h, D), dtype=out.dtype, device=out.device)   # the pad rows stay zero
             full[:, :L] = out
             out = full
-        img = heads_to_seq(out[:, :N], self.group)
+        img = heads_to_seq(out[:, :N], self.group, offsets=off)
         if not joint:
             return img
-        txt = gather_heads(out[:, N:], self.group)
+        txt = gather_heads(out[:, N:], self.group, offsets=off)
         return torch.cat([img, txt], dim=1)
 
 
@@ -190,7 +268,12 @@ class UlyssesFusedAttention:
     Device-side barriers (symmetric-memory signal pads) order the peer traffic: one per sub-group
     after its exchange, one per call after the attention.  The operator's opt-in switches
     (attention.QK_INT8, attention.PV_FP8) apply: a sub-group's q, k, v are quantised on the main
-    stream once its exchange is complete, and the next call's exchange waits for the main stream."""
+    stream once its exchange is complete, and the next call's exchange waits for the main stream.
+
+    Ragged head split (ragged(H, P)): the qkv buffer has slots = ⌈H/P⌉ head slots on every rank (symmetric
+    memory needs one shape), filled by jenga_ulysses_scatter_ragged; G comes from the slot count, so every
+    rank issues the same scatters and barriers, and a rank attends over the part of each sub-group's
+    slots its own group covers."""
 
     def __init__(self, group=None, variant: str = "hyvideo", groups: int | None = None):
         self.group = group if group is not None else dist.group.WORLD
@@ -258,7 +341,7 @@ class UlyssesFusedAttention:
         if B != 1:
             raise ValueError("the fused Ulysses path is built for batch 1 (what the pipelines run)")
         hooks = _hooks or {}
-        h = H // P
+        off, h, b, slots = _layout(H, P, r)
         joint = joint_tensor_query is not None
         if joint and joint_strategy != "rear":
             raise ValueError("only joint_strategy='rear' is built (attenion.py:181)")
@@ -268,7 +351,7 @@ class UlyssesFusedAttention:
         N = P * n
         L = _valid_rows(seq_len, N, n, T, dense, first_frame_blocks)
         dev, dt = query.device, query.dtype
-        qkv, h_qkv, p_qkv, outs = self._buffers(N, T, h, D, n, H, dt, dev)
+        qkv, h_qkv, p_qkv, outs = self._buffers(N, T, slots, D, n, H, dt, dev)
         out, h_out, p_out = outs[self._call & 1]
         self._call += 1
         # this rank's pad rows (global rows >= L): no rank stores them, so they are zeroed whenever the
@@ -277,8 +360,9 @@ class UlyssesFusedAttention:
         if self._pad_len.get(out.data_ptr(), N) != L and pad0 < n:
             out[pad0:n].zero_()
         self._pad_len[out.data_ptr()] = L
-        G = self._n_groups(h, self.groups, (L + T + BLOCK - 1) // BLOCK)
-        hg = h // G
+        # the same G on every rank, from the slot count: every rank issues every scatter and barrier
+        G = self._n_groups(slots, self.groups, (L + T + BLOCK - 1) // BLOCK)
+        hg = slots // G
         xs = [t[0] for t in (query, key, value)]
         for t in xs:
             if t.stride(2) != 1 or t.stride(1) != D or t.stride(0) != xs[0].stride(0):
@@ -295,6 +379,7 @@ class UlyssesFusedAttention:
             a.joint_stride_s = js[0].stride(0)
         a.world, a.rank, a.heads, a.head_dim, a.n_loc, a.n_text = P, r, H, D, n, T
         a.peer_qkv_host = C.addressof(p_qkv)
+        c_off = None if off is None else (C.c_int32 * (P + 1))(*off)
         main = torch.cuda.current_stream(dev)
         if self._side is None:
             self._side = torch.cuda.Stream(device=dev)
@@ -307,7 +392,11 @@ class UlyssesFusedAttention:
                 if "pre_scatter" in hooks:
                     hooks["pre_scatter"](g, side)
                 a.head_begin, a.head_count = g * hg, hg
-                check(lib.jenga_ulysses_scatter(C.byref(a), _stream_ptr(dev)), "ulysses_scatter")
+                if c_off is None:
+                    check(lib.jenga_ulysses_scatter(C.byref(a), _stream_ptr(dev)), "ulysses_scatter")
+                else:
+                    check(lib.jenga_ulysses_scatter_ragged(C.byref(a), c_off, _stream_ptr(dev)),
+                          "ulysses_scatter_ragged")
                 if "post_scatter" in hooks:
                     hooks["post_scatter"](g, side)
                 h_qkv.barrier(channel=0)
@@ -324,20 +413,21 @@ class UlyssesFusedAttention:
         for g in range(G):
             if side is not main:
                 main.wait_event(events[g])
-            sl = slice(g * hg, (g + 1) * hg)
-            sp = dict(world=P, rank=r, heads_total=H, rows=n, peers=p_out, head_base=r * h + g * hg)
-            q, k, v = (x[None, :L + T, sl] for x in qkv)       # all N + T rows without seq_len
-            if dense:
-                # flash_attn_shim._dense's launch, with the peer-store epilogue instead of `out`
-                v8, qk8 = A.quantize_operands(q, k, v, A.PV_FP8, A.QK_INT8)
-                A._launch(q, k, v, None, 0, (L + BLOCK - 1) // BLOCK, D ** -0.5, 0.0, 1 << 30, L, L, L, None,
-                          None, q.dtype, sp_out=sp, v_fp8=v8, qk_int8=qk8)
-            else:
-                block_sparse_attention_variant(self.variant, q, k, v, top_k, cu_seqlens_q=cu, cu_seqlens_kv=cu,
-                                               text_blocks=(T + BLOCK - 1) // BLOCK, text_amp=text_amp,
-                                               block_neighbor_list=block_neighbor_list,
-                                               p_remain_rates=p_remain_rates, first_frame_blocks=first_frame_blocks,
-                                               sp_out=sp)
+            sl = slice(g * hg, min((g + 1) * hg, h))
+            if sl.start < sl.stop:      # a short ragged group may own no head of this slot range
+                sp = dict(world=P, rank=r, heads_total=H, rows=n, peers=p_out, head_base=b + g * hg)
+                q, k, v = (x[None, :L + T, sl] for x in qkv)       # all N + T rows without seq_len
+                if dense:
+                    # flash_attn_shim._dense's launch, with the peer-store epilogue instead of `out`
+                    v8, qk8 = A.quantize_operands(q, k, v, A.PV_FP8, A.QK_INT8)
+                    A._launch(q, k, v, None, 0, (L + BLOCK - 1) // BLOCK, D ** -0.5, 0.0, 1 << 30, L, L, L, None,
+                              None, q.dtype, sp_out=sp, v_fp8=v8, qk_int8=qk8)
+                else:
+                    block_sparse_attention_variant(self.variant, q, k, v, top_k, cu_seqlens_q=cu, cu_seqlens_kv=cu,
+                                                   text_blocks=(T + BLOCK - 1) // BLOCK, text_amp=text_amp,
+                                                   block_neighbor_list=block_neighbor_list,
+                                                   p_remain_rates=p_remain_rates, first_frame_blocks=first_frame_blocks,
+                                                   sp_out=sp)
             if "post_attention" in hooks:
                 # per-group completion across ranks, so the caller may drain this group's heads
                 h_out.barrier(channel=0)
@@ -373,6 +463,10 @@ class HostPipelinedUlysses:
         self.dev = torch.device(device)
         self.n, self.T, self.H, self.D = n_loc, T, H, D
         P = dist.get_world_size(self.fused.group)
+        if ragged(H, P):
+            raise ValueError(f"HostPipelinedUlysses needs the degree to divide the head count ({H} heads over {P} "
+                             "ranks); the ragged split (JENGA_ULYSSES_RAGGED) serves UlyssesFusedAttention and "
+                             "UlyssesCarvedAttention only")
         self.P, self.h = P, H // P
         self.G, self.hg = self.fused.plan(self.h, P * n_loc + T)
         mk = lambda: torch.empty((1, n_loc + T, H, D), dtype=dtype, device=self.dev)  # noqa: E731
