@@ -13,7 +13,8 @@ reference module is executed,
   WanT2VCrossAttention.forward        (wan/modules/model_mul.py:183-205)
   WanAttentionBlock.forward           (wan/modules/model_mul.py:303-346)
   WanSelfAttention.forward / WanAttentionBlock.forward of wan/modules/model.py (:127-156, :274-313),
-      the plain model WanI2V loads, only under install(wan_sp=True)
+      the plain model WanI2V loads, under install(wan_sp=True) at import, and when a single-GPU
+      WanI2V is built (WanI2V.__init__ of wan/image2video.py is wrapped for that)
 
 with versions whose attention section is `jenga_hy_prologue` / `jenga_wan_prologue` (RMSNorm +
 RoPE + img||txt concatenation + block pooling in one pass over the QKV projection output)
@@ -62,6 +63,7 @@ from . import dense as DN
 from . import hyvideo as HY
 from . import ulysses as U
 from . import wan as WAN
+from .flash_attn_shim import flash_attn_func
 
 _HY_MODULES = ("hyvideo.modules.models_mul_block_gc_ha_multigpu",)
 _I2V_MODULES = ("hyvideo_i2v.modules.models_mul",)
@@ -77,6 +79,10 @@ _WAN_SP_MODULES = ("wan.distributed.xdit_context_parallel",)
 # the fused WanAttentionBlock.forward and a WanSelfAttention.forward for its signatures; without the
 # switch it is not touched
 _WAN_PLAIN_MODULES = ("wan.modules.model",)
+# wan/image2video.py: WanI2V(use_usp=False) gets the single-GPU I2V forward of wan_sp.py, and the plain
+# model's blocks the fused forwards, when the pipeline is built (wan.modules.model itself stays untouched
+# at import, which only WanI2V imports)
+_WAN_I2V_PIPE_MODULES = ("wan.image2video",)
 WAN_SP = False
 
 
@@ -116,7 +122,8 @@ def _sp_modules():
 STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "i2v_double_sp": 0,
          "i2v_single_sp": 0, "wan_self": 0, "wan_self_sp": 0, "wan_self_dense_sp": 0, "fallback": 0,
          "gather": 0, "ln_modulate": 0, "gate_residual": 0, "gelu_cat": 0, "wan_block": 0, "wan_cross": 0,
-         "wan_i2v_cross": 0, "linear_fp8": 0, "wan_i2v_self_sp": 0, "wan_i2v_cross_sp": 0}
+         "wan_i2v_cross": 0, "linear_fp8": 0, "wan_i2v_self_sp": 0, "wan_i2v_cross_sp": 0, "wan_i2v_self": 0,
+         "wan_i2v_self_dense": 0, "wan_i2v_self_carved_sp": 0}
 # the CLIP image tokens at the head of the Wan2.1-I2V context (model_mul.py:230-231)
 _WAN_I2V_IMG_TOKENS = 257
 # the HunyuanVideo-I2V operator's text_blocks default (hyvideo_i2v/…/attention_block_triton_diffres.py:409);
@@ -436,68 +443,98 @@ def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=Non
 # ------------------------------------------------------------------------------------------------
 # Wan blocks
 # ------------------------------------------------------------------------------------------------
-def _wan_self_sp(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates, freq_remap,
-                 block_neighbor_list, stat=None):
-    """WanSelfAttention.forward on a rank's n rows of the Hilbert-sharded Wan forward (wan_sp.py): the
-    norm + RoPE prologue on the rank's rows, then the Ulysses exchange and the operator over the first
-    L (the global token count) exchanged rows.  top_k and first_frame_blocks follow the single-GPU rule
-    over L (model_mul.py:161-164); sa_drop_rate <= 0.25 (:153, the warm-up steps) runs the dense class
-    over the same exchange.  No fall-back: the original forward would attend over the rank's rows.
-    stat: the STATS key of the call (default: the T2V route's, by class)."""
+def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates, freq_remap,
+                    block_neighbor_list, stats=("wan_self_sp", "wan_self_dense_sp")):
+    """WanSelfAttention.forward with the fused norm + RoPE prologue and no fall-back.
+    jsp set: x is a rank's n rows of a sharded Wan forward (wan_sp.py); the prologue runs on them, then
+    the Ulysses exchange and the operator over the first L (the global token count) exchanged rows.
+    jsp None: x is all L rows on one GPU (the single-GPU I2V forward of wan_sp.py).
+    top_k and first_frame_blocks follow the single-GPU rule over L (model_mul.py:161-164); sa_drop_rate
+    <= 0.25 (:153, the warm-up steps) runs the dense class, the flash_attn shim's launch.  freq_remap:
+    the RoPE row of each row (None: raster, one GPU only).  stats: the STATS keys of a carved and of a
+    dense call."""
     b, n = x.shape[:2]
-    wq = getattr(self.norm_q, "weight", None)
-    wk = getattr(self.norm_k, "weight", None)
-    if (not x.is_cuda or b != 1 or self.head_dim != 128 or per_block_tokens != 128 or wq is None or wk is None
-            or type(self.norm_q).__name__ != "WanRMSNorm" or type(self.norm_k).__name__ != "WanRMSNorm"
-            or freq_remap is None):
-        raise RuntimeError(f"{type(self).__name__} under jenga_sp: the call is not one the sharded Wan forward "
-                           "takes (a CUDA batch-1 input, head_dim 128, 128-token blocks, WanRMSNorm q / k "
-                           "norms with weights and a freq_remap); it has no fall-back")
+    if not _wan_self_fused_ok(self, x, per_block_tokens) or (jsp is not None and freq_remap is None):
+        raise RuntimeError(f"{type(self).__name__}: the call is not one the fused Wan self-attention takes (a "
+                           "CUDA batch-1 input, head_dim 128, 128-token blocks, WanRMSNorm q / k norms with "
+                           "weights and, under jenga_sp, a freq_remap); this route has no fall-back")
     q_lin, k_lin = self.q(x), self.k(x)
     if q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype != q_lin.dtype:
-        raise RuntimeError(f"{type(self).__name__} under jenga_sp: q / k Linears return {q_lin.dtype}, "
-                           "the prologue takes bf16 or fp32")
+        raise RuntimeError(f"{type(self).__name__}: q / k Linears return {q_lin.dtype}, the prologue takes bf16 "
+                           "or fp32")
     grid = [int(g) for g in grid_sizes[0].tolist()]
     L = grid[0] * grid[1] * grid[2]
     eps = float(self.norm_q.eps)
-    q = WAN.norm_rope(q_lin, wq, self.num_heads, grid, freqs, freq_remap, eps)
-    k = WAN.norm_rope(k_lin, wk, self.num_heads, grid, freqs, freq_remap, eps)
+    wq, wk = self.norm_q.weight, self.norm_k.weight
     # the bf16 v both single-GPU routes attend: flash_attention's half() and the operator's cast
     v = self.v(x).view(b, n, self.num_heads, self.head_dim).to(torch.bfloat16).contiguous()
     dense = sa_drop_rate <= 0.25
-    top_k, ff = (0, 0) if dense else WAN.block_counts(L, sa_drop_rate)
-    out = jsp(None, q, k, v, top_k=top_k, block_neighbor_list=None if dense else block_neighbor_list,
-              p_remain_rates=p_remain_rates, first_frame_blocks=ff, dense=dense, seq_len=L)
-    STATS[stat or ("wan_self_dense_sp" if dense else "wan_self_sp")] += 1
+    if jsp is None and not dense:
+        out = WAN.self_attention(q_lin, k_lin, v, wq, wk, self.num_heads, grid, freqs, sa_drop_rate,
+                                 p_remain_rates=p_remain_rates, freq_remap=freq_remap,
+                                 block_neighbor_list=block_neighbor_list, eps=eps)
+    else:
+        q = WAN.norm_rope(q_lin, wq, self.num_heads, grid, freqs, freq_remap, eps)
+        k = WAN.norm_rope(k_lin, wk, self.num_heads, grid, freqs, freq_remap, eps)
+        if jsp is None:
+            out = flash_attn_func(q, k, v)
+        else:
+            top_k, ff = (0, 0) if dense else WAN.block_counts(L, sa_drop_rate)
+            out = jsp(None, q, k, v, top_k=top_k, block_neighbor_list=None if dense else block_neighbor_list,
+                      p_remain_rates=p_remain_rates, first_frame_blocks=ff, dense=dense, seq_len=L)
+    STATS[stats[dense]] += 1
     out = out.flatten(2)
     if not torch.is_autocast_enabled():
         out = out.float()       # the query dtype the reference returns, as in _wan_self
     return self.o(out)
 
 
-def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs):
-    """WanSelfAttention.forward of wan/modules/model.py (:127-156), hooked only under install(wan_sp=True).
-    Under `jenga_sp` (the raster-sharded I2V forward, wan_sp.parallelize_wan_i2v) x holds rank r's n rows
-    [r*n, min((r+1)*n, L)): the fused prologue runs on them with that raster slice as the RoPE index (pad
-    rows index row 0), then the dense class over the first L exchanged rows, so the pad keys are excluded
-    as flash_attention(k_lens=seq_lens) excludes them on one GPU.  Without jenga_sp: the original forward."""
+def _wan_self_fused_ok(self, x, per_block_tokens=128):
+    """the configuration _wan_self_fused takes, the Linears' output dtype aside"""
+    wq = getattr(self.norm_q, "weight", None)
+    wk = getattr(self.norm_k, "weight", None)
+    return (x.is_cuda and x.shape[0] == 1 and self.head_dim == 128 and per_block_tokens == 128 and wq is not None
+            and wk is not None and type(self.norm_q).__name__ == "WanRMSNorm"
+            and type(self.norm_k).__name__ == "WanRMSNorm")
+
+
+def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=None, freq_remap=None, block_neighbor_list=None,
+                  p_remain_rates=0.8):
+    """WanSelfAttention.forward of wan/modules/model.py (:127-156).  Called in that module's signature
+    (sa_drop_rate None):
+      under `jenga_sp` (the raster-sharded I2V forward, wan_sp.parallelize_wan_i2v) x holds rank r's n
+      rows [r*n, min((r+1)*n, L)): the fused prologue runs on them with that raster slice as the RoPE index
+      (pad rows index row 0), then the dense class over the first L exchanged rows, so the pad keys are
+      excluded as flash_attention(k_lens=seq_lens) excludes them on one GPU;
+      without jenga_sp: the original forward.
+    With the Jenga arguments of model_mul.py (the I2V forwards of wan_sp.py): _wan_self_fused, on one GPU
+    or under jenga_sp.  A call it does not take runs the original forward on raster rows (freq_remap None)
+    and raises on curve-ordered rows, whose RoPE positions the original forward does not know."""
     jsp = getattr(self, "jenga_sp", None)
-    if jsp is None:
-        return None
-    _, r = U._group_size_rank(jsp.group)
-    n = x.shape[1]
-    L = int(torch.prod(grid_sizes[0]))
-    rows = torch.arange(r * n, (r + 1) * n, device=x.device)
-    remap = torch.where(rows < L, rows, torch.zeros_like(rows))
-    return _wan_self_sp(self, jsp, x, grid_sizes, freqs, 0.0, 128, 0.0, remap, None, stat="wan_i2v_self_sp")
+    if sa_drop_rate is None:
+        if jsp is None:
+            return None
+        _, r = U._group_size_rank(jsp.group)
+        n = x.shape[1]
+        L = int(torch.prod(grid_sizes[0]))
+        rows = torch.arange(r * n, (r + 1) * n, device=x.device)
+        remap = torch.where(rows < L, rows, torch.zeros_like(rows))
+        return _wan_self_fused(self, jsp, x, grid_sizes, freqs, 0.0, 128, 0.0, remap, None,
+                               stats=(None, "wan_i2v_self_sp"))
+    if jsp is None and freq_remap is None and not _wan_self_fused_ok(self, x):
+        STATS["fallback"] += 1
+        return type(self).forward.__wrapped__(self, x, seq_lens, grid_sizes, freqs)
+    stats = ("wan_i2v_self_carved_sp", "wan_i2v_self_sp") if jsp is not None else ("wan_i2v_self", "wan_i2v_self_dense")
+    return _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, 128, p_remain_rates, freq_remap,
+                           block_neighbor_list, stats=stats)
 
 
 def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128, p_remain_rates=0.8,
               freq_remap=None, block_neighbor_list=None):
     jsp = getattr(self, "jenga_sp", None)
     if jsp is not None:
-        return _wan_self_sp(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
-                            freq_remap, block_neighbor_list)
+        return _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
+                               freq_remap, block_neighbor_list)
     b, s = x.shape[:2]
     wq = getattr(self.norm_q, "weight", None)
     wk = getattr(self.norm_k, "weight", None)
@@ -587,20 +624,34 @@ def _wan_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, s
                                 block_neighbor_list=block_neighbor_list, p_remain_rates=p_remain_rates))
 
 
-def _wan_plain_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens):
-    """WanAttentionBlock.forward of wan/modules/model.py (:274-313), hooked only under install(wan_sp=True):
-    the fused body, with the self-attention called in that module's signature.  Under `self_attn.jenga_sp`
+def _wan_plain_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=None,
+                     freq_remap=None, block_neighbor_list=None, p_remain_rates=0.8):
+    """WanAttentionBlock.forward of wan/modules/model.py (:274-313): the fused body, with the
+    self-attention called in that module's signature, or, when the I2V forwards of wan_sp.py pass the
+    Jenga arguments of model_mul.py (sa_drop_rate not None), with those.  Under `self_attn.jenga_sp`
     (parallelize_wan_i2v) x is a rank's rows and there is no fall-back: the checks run before the
-    exchange, so every rank raises alike."""
+    exchange, so every rank raises alike.  On one GPU a call the fused body does not take runs the
+    original forward on raster rows and raises on curve-ordered rows (freq_remap set)."""
+    attn_kw = {} if sa_drop_rate is None else dict(sa_drop_rate=sa_drop_rate, freq_remap=freq_remap,
+                                                   block_neighbor_list=block_neighbor_list,
+                                                   p_remain_rates=p_remain_rates)
     if getattr(self.self_attn, "jenga_sp", None) is None:
-        return _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, {})
+        out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw)
+        if out is not None or sa_drop_rate is None:
+            return out
+        if freq_remap is not None:
+            raise RuntimeError(f"{type(self).__name__}: the call is not one the fused block takes (a CUDA input "
+                               "under bf16 autocast, fp32 modulation, cross_attn_norm=True); the original forward "
+                               "cannot take the curve-ordered rows of the carved I2V forward")
+        STATS["fallback"] += 1
+        return type(self).forward.__wrapped__(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens)
     if not (type(self.cross_attn).__name__ == "WanI2VCrossAttention"
             and _wan_i2v_cross_shape_ok(self.cross_attn, x, context, context_lens)):
         raise RuntimeError(f"{type(self).__name__} under jenga_sp: the cross-attention is not one the fused I2V "
                            "kernel takes (a WanI2VCrossAttention with WanRMSNorm q / k / k_img norms, head_dim "
                            f"128, batch 1, context_lens None and more than {_WAN_I2V_IMG_TOKENS} context rows); "
                            "the sharded I2V forward has no fall-back")
-    out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, {}, sharded=True)
+    out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded=True)
     if out is None:
         raise RuntimeError(f"{type(self).__name__} under jenga_sp: the call is not one the fused block takes (a "
                            "CUDA input under bf16 autocast, fp32 modulation, cross_attn_norm=True); the sharded "
@@ -609,7 +660,8 @@ def _wan_plain_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_l
 
 
 def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded=False):
-    """attn_kw: the Jenga self-attention arguments of model_mul.py (empty for wan/modules/model.py).
+    """attn_kw: the Jenga self-attention arguments of model_mul.py (empty for wan/modules/model.py called
+    in its own signature).
     sharded: the I2V rows of parallelize_wan_i2v; the cross-attention must then be the fused one."""
     i2v = type(self.cross_attn).__name__ == "WanI2VCrossAttention"
     ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
@@ -666,14 +718,11 @@ def patch_module(mod) -> list[str]:
     if name in _WAN_SP_MODULES:
         from .wan_sp import install_usp
         return [f"{name}.usp_dit_forward", f"{name}.usp_attn_forward"] if WAN_SP and install_usp(mod) else []
+    if name in _WAN_I2V_PIPE_MODULES:
+        return _wrap_wan_i2v_init(mod)
     fused = {}
     if name in _WAN_PLAIN_MODULES:
-        if not WAN_SP:
-            return []
-        # the block hands its self-attention (x, seq_lens, grid_sizes, freqs) and runs the fused I2V
-        # cross-attention; WanT2VCrossAttention and WanI2VCrossAttention stay as they are
-        fused.update(WanSelfAttention=_wan_i2v_self, WanAttentionBlock=_wan_plain_block)
-        return _patch_classes(mod, fused)
+        return patch_plain_wan(mod) if WAN_SP else []
     if name.startswith(("hyvideo.", "hyvideo_i2v.")):
         # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
         # a ragged S with four text blocks: its own pair of entry points
@@ -684,6 +733,36 @@ def patch_module(mod) -> list[str]:
     # its fused form (_wan_i2v_cross)
     fused.update(WanSelfAttention=_wan_self, WanT2VCrossAttention=_wan_cross, WanAttentionBlock=_wan_block)
     return _patch_classes(mod, fused)
+
+
+def patch_plain_wan(mod) -> list[str]:
+    """Patches WanSelfAttention / WanAttentionBlock of wan/modules/model.py: the block hands its
+    self-attention (x, seq_lens, grid_sizes, freqs), or the Jenga arguments the I2V forwards of wan_sp.py
+    pass, and runs the fused I2V cross-attention; WanT2VCrossAttention and WanI2VCrossAttention stay as
+    they are"""
+    return _patch_classes(mod, dict(WanSelfAttention=_wan_i2v_self, WanAttentionBlock=_wan_plain_block))
+
+
+def _wrap_wan_i2v_init(mod) -> list[str]:
+    """WanI2V.__init__ of wan/image2video.py, followed, for a pipeline built with use_usp=False, by
+    wan_sp.bind_wan_i2v on its WanModel: the single-GPU I2V forward.  With use_usp=True the pipeline keeps
+    what it bound (usp_dit_forward; install(wan_sp=True) decides what that is)."""
+    cls = getattr(mod, "WanI2V", None)
+    if cls is None or getattr(cls.__init__, "__jenga_b200__", False):
+        return []
+    orig = cls.__init__
+
+    @functools.wraps(orig)
+    def __init__(self, *args, **kwargs):
+        orig(self, *args, **kwargs)
+        # a dit_fsdp model is an FSDP wrapper, whose forward gathers the parameters: left as it is
+        if not getattr(self, "use_usp", False) and type(self.model).__name__ == "WanModel":
+            from .wan_sp import bind_wan_i2v
+            bind_wan_i2v(self.model)
+
+    __init__.__jenga_b200__ = True
+    cls.__init__ = __init__
+    return [f"{mod.__name__}.WanI2V.__init__"]
 
 
 def _patch_classes(mod, fused) -> list[str]:
@@ -711,6 +790,7 @@ class _PatchingLoader(importlib.abc.Loader):
         if done:
             what = ("sequence-parallel I2V route" if module.__name__ in _I2V_SP_MODULES
                     else "sequence-parallel Wan route" if module.__name__ in _WAN_SP_MODULES
+                    else "single-GPU Wan I2V route" if module.__name__ in _WAN_I2V_PIPE_MODULES
                     else "fused attention section")
             print(f"[jenga_b200] {what} installed: {', '.join(done)}", file=sys.stderr)
 
@@ -719,7 +799,7 @@ class _PatchingLoader(importlib.abc.Loader):
 
 
 class _PatchFinder(importlib.abc.MetaPathFinder):
-    targets = _HY_MODULES + _I2V_MODULES + _WAN_MODULES
+    targets = _HY_MODULES + _I2V_MODULES + _WAN_MODULES + _WAN_I2V_PIPE_MODULES
 
     def find_spec(self, fullname, path, target=None):
         if fullname not in self.targets and fullname not in _sp_modules():

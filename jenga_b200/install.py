@@ -28,7 +28,8 @@ def _module(name: str, **attrs) -> types.ModuleType:
 
 
 def install(flash_attn: bool = True, gilbert: bool = True, ulysses: bool = True, fused_blocks: bool = True,
-            gather: bool = True, i2v_sp: bool | None = None, wan_sp: bool | None = None) -> list[str]:
+            gather: bool = True, i2v_sp: bool | None = None, wan_sp: bool | None = None,
+            wan_i2v_sa_drop_rates=None, wan_i2v_p_remain=None) -> list[str]:
     """Pre-seeds sys.modules; returns the names it installed.
     fused_blocks: also patch the reference block classes right after they are imported so that
     RMSNorm + RoPE + cat + pooling run as the fused prologue kernel (jenga_b200/blocks.py).
@@ -38,7 +39,14 @@ def install(flash_attn: bool = True, gilbert: bool = True, ulysses: bool = True,
     default, None reads JENGA_I2V_SP=1.  Needs fused_blocks.
     wan_sp: `jenga_wan.py --ulysses_size N` runs the Hilbert-sharded TeaCache forward over the Ulysses
     exchange (jenga_b200/wan_sp.py) instead of the reference's usp_dit_forward / usp_attn_forward; off
-    by default, None reads JENGA_WAN_SP=1.  Needs fused_blocks."""
+    by default, None reads JENGA_WAN_SP=1.  Needs fused_blocks.
+    fused_blocks also gives `WanI2V(use_usp=False)` the single-GPU I2V forward of jenga_b200/wan_sp.py
+    (dense, as the original model).
+    wan_i2v_sa_drop_rates: "d0[,d1]" or one or two numbers, as jenga_wan.py --sa_drop_rates: the Wan2.1-I2V
+    forwards (one GPU and sharded) run the carved self-attention over the Hilbert order with T2V's drop-rate
+    schedule; None reads JENGA_WAN_I2V_SA_DROP, unset or "" keeps them dense.  wan_i2v_p_remain: the
+    carved steps' p_remain_rates, default 0.8; None reads JENGA_WAN_I2V_P_REMAIN.  Carving needs
+    fused_blocks."""
     import os
     if i2v_sp is None:
         i2v_sp = os.environ.get("JENGA_I2V_SP", "") == "1"
@@ -49,6 +57,14 @@ def install(flash_attn: bool = True, gilbert: bool = True, ulysses: bool = True,
     if wan_sp and not fused_blocks:
         raise ValueError("wan_sp routes the self-attention through the fused WanSelfAttention forward: it needs "
                          "fused_blocks")
+    from . import wan_sp as WSP
+    if wan_i2v_sa_drop_rates is None:
+        wan_i2v_sa_drop_rates = os.environ.get("JENGA_WAN_I2V_SA_DROP")
+    if wan_i2v_p_remain is None:
+        wan_i2v_p_remain = os.environ.get("JENGA_WAN_I2V_P_REMAIN")
+    if WSP.parse_sa_drop_rates(wan_i2v_sa_drop_rates) and not fused_blocks:
+        raise ValueError("Wan2.1-I2V carving runs in the fused WanAttentionBlock forward: it needs fused_blocks")
+    WSP.set_i2v_carving(wan_i2v_sa_drop_rates, wan_i2v_p_remain)
     from . import attention as A
     from . import flash_attn_shim as F
     from . import gilbert as G

@@ -32,9 +32,23 @@ state machine of teacache_forward:
 Unlike the reference's USP, which attends to the zero pad rows of seq_len (its TODO at
 xdit_context_parallel.py:172-187), the pad keys are excluded, as the single-GPU
 flash_attention(k_lens=seq_lens) excludes them.
+
+On one GPU (`bind_wan_i2v`, which install()'s hook calls for WanI2V(use_usp=False)) the same I2V forward
+runs with group LOCAL: one rank, no exchange.  jenga_wan.py binds teacache_forward to the I2V model too,
+which cannot run on it (no curve attributes, and model.py's blocks take no Jenga arguments); the
+instance attribute shadows it.  Its self-attention is the fused prologue and the dense class over the L
+raster rows.
+
+Carving (opt-in, I2V_SA_DROP_RATES: install(wan_i2v_sa_drop_rates=...) / JENGA_WAN_I2V_SA_DROP) makes
+both I2V forwards follow teacache_forward's T2V rules: the rows in the sliced Gilbert order of the
+forward's own grid (i2v_curve; on P ranks each rank takes its slice, as parallelize_wan does),
+freq_remap = that order in every step, the drop rate of t2v_generate's schedule (sa_drop_schedule), the
+Wan operator with first_frame_blocks above 0.25 and the dense class below; then the head, the inverse
+scatter and unpatchify.  Both T2V and I2V forwards run one body, _sharded_forward.
 """
 from __future__ import annotations
 
+import functools
 import types
 
 import numpy as np
@@ -45,6 +59,24 @@ from .hyi2v_sp import check_degree, default_attention, shard
 
 MODEL = "Wan2.1"
 MAX_WORLD = 8        # the peer arrays of the fused exchange and of the attention epilogue
+
+
+class _Local:
+    """the group of the one-GPU forward: one rank, no process group, no exchange"""
+
+    def __repr__(self):
+        return "LOCAL"
+
+
+LOCAL = _Local()
+
+
+def _world(group) -> tuple[int, int]:
+    return (1, 0) if group is LOCAL else (dist.get_world_size(group), dist.get_rank(group))
+
+
+def _route(group) -> str:
+    return "single-GPU " if group is LOCAL else "sequence-parallel "
 
 
 def _check_world(heads: int, world: int) -> None:
@@ -75,6 +107,8 @@ def _rel_l1_from_rank0(value: torch.Tensor, group) -> float:
     replicated, but nothing guarantees bit-equal reductions across devices); all ranks then accumulate
     the same number and take the same branch, so no rank skips the blocks while another enters the
     exchange."""
+    if group is LOCAL:
+        return value.cpu().item()
     v = value.reshape(1).clone()
     dist.broadcast(v, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
     return v.cpu().item()
@@ -116,7 +150,7 @@ def _teacache(self, x, e, e0, run_blocks, group):
     """jenga_wan.py:595-652: the TeaCache step decision around `run_blocks` (x -> x after every block),
     with rank 0's rel-L1 value on every rank.  Each rank keeps the residual of its own rows.  stage_start
     is read as False where the model has none (jenga_wan.py sets it on the T2V model only)."""
-    if not self.enable_teacache:
+    if not getattr(self, "enable_teacache", False):     # a model jenga_wan.py has not set up
         return run_blocks(x)
     # :595-626
     modulated_inp = e0 if self.use_ref_steps else e
@@ -154,55 +188,73 @@ def _forward_factory(group):
     def forward(self, x, t, context, seq_len, clip_fea=None, y=None, sa_drop_rate=0.0):
         """jenga_wan.py:503-664 (teacache_forward) on this rank's Hilbert rows; returns the full output
         on every rank"""
-        P, r = dist.get_world_size(group), dist.get_rank(group)
         for name in ("hilbert_order", "linear_to_hilbert"):
             if getattr(self, name, None) is None:
                 raise RuntimeError(f"sequence-parallel {MODEL}: model.{name} is not set (jenga_wan.py sets "
                                    "the Jenga curve attributes before sampling)")
         if self.model_type == 'i2v':
             assert clip_fea is not None and y is not None
-        if len(x) != 1:
-            raise ValueError(f"sequence-parallel {MODEL} runs batch 1, got {len(x)} videos")
-        device = self.patch_embedding.weight.device
-        if self.freqs.device != device:
-            self.freqs = self.freqs.to(device)
-        if y is not None:
-            x = [torch.cat([u, v], dim=0) for u, v in zip(x, y)]
-        # embeddings (replicated)
-        x = [self.patch_embedding(u.unsqueeze(0)) for u in x]
-        grid_sizes = torch.stack([torch.tensor(u.shape[2:], dtype=torch.long) for u in x])
-        x = [u.flatten(2).transpose(1, 2) for u in x]
-        seq_lens = torch.tensor([u.size(1) for u in x], dtype=torch.long)
-        assert seq_lens.max() <= seq_len
-        x = x[0]
-        # the reference pads to the sp_size-rounded seq_len and the Hilbert gather drops those rows
-        # again (:554-559): gathering from the unpadded rows gives the same rows
-        order = self.hilbert_order
-        L = len(order)
-        if L != int(seq_lens[0]):
-            raise ValueError(f"sequence-parallel {MODEL}: hilbert_order has {L} entries for a latent of "
-                             f"{int(seq_lens[0])} tokens (curve and grid out of step)")
+        curve = (self.hilbert_order, self.linear_to_hilbert, self.block_neighbor_list)
+        return _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, lambda grid: curve,
+                                dict(sa_drop_rate=sa_drop_rate, p_remain_rates=self.p_remain_rates))
+    return forward
+
+
+def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of, block_kw):
+    """The body both Wan forwards share.  curve_of(grid) -> (hilbert_order, linear_to_hilbert,
+    block_neighbor_list) or None: rank r takes the curve's rows [r*n, min((r+1)*n, L)) and `freq_remap`
+    is that slice, or, without a curve, the raster rows.  block_kw: what the blocks get besides the
+    arguments of model.py's WanAttentionBlock.forward (with a curve, also freq_remap and
+    block_neighbor_list).  group LOCAL: one GPU, no exchange."""
+    P, r = _world(group)
+    if len(x) != 1:
+        raise ValueError(f"{_route(group)}{MODEL} runs batch 1, got {len(x)} videos")
+    device = self.patch_embedding.weight.device
+    if self.freqs.device != device:
+        self.freqs = self.freqs.to(device)
+    if y is not None:
+        x = [torch.cat([u, v], dim=0) for u, v in zip(x, y)]
+    # embeddings (replicated)
+    x = [self.patch_embedding(u.unsqueeze(0)) for u in x]
+    grid_sizes = torch.stack([torch.tensor(u.shape[2:], dtype=torch.long) for u in x])
+    x = [u.flatten(2).transpose(1, 2) for u in x]
+    seq_lens = torch.tensor([u.size(1) for u in x], dtype=torch.long)
+    assert seq_lens.max() <= seq_len
+    x = x[0]
+    # rows past L (the reference's zero pad to seq_len, which the Hilbert gather drops again,
+    # jenga_wan.py:554-559) are neither attended nor returned
+    L = int(seq_lens[0])
+    curve = curve_of(tuple(grid_sizes[0].tolist()))
+    kwargs = dict(block_kw)
+    if curve is None:
+        shard_rows(L, P, r)                                  # raises when a rank holds no real row
+        x = shard(x, 1, P, r)
+    else:
+        order = curve[0]
+        if len(order) != L:
+            raise ValueError(f"sequence-parallel {MODEL}: hilbert_order has {len(order)} entries for a latent "
+                             f"of {L} tokens (curve and grid out of step)")
         n, real = shard_rows(L, P, r)
         rows = shard(order.to(torch.long), 0, P, r)          # pad entries point at row 0 (any valid row)
         x = x[:, rows.to(x.device)]
         if real < n:
             x[:, real:] = 0
-        freq_remap = rows.to(device)
-        e, e0, context = _time_and_context(self, t, context, clip_fea)
-        kwargs = dict(e=e0, seq_lens=seq_lens, grid_sizes=grid_sizes, freqs=self.freqs, context=context,
-                      context_lens=None, sa_drop_rate=sa_drop_rate, freq_remap=freq_remap,
-                      block_neighbor_list=self.block_neighbor_list, p_remain_rates=self.p_remain_rates)
-        x = _teacache(self, x, e, e0, lambda x: _blocks(self, x, kwargs), group)
-        # head on the rank's rows (row-local, as usp_dit_forward runs it before its gather), then the
-        # [1, n, out] rows of every rank in rank order
-        x = _gather_rows(self.head(x, e), L, P, group)
-        x = x[:, self.linear_to_hilbert]                                      # :655
-        x = self.unpatchify(x, grid_sizes)
+        kwargs.update(freq_remap=rows.to(device), block_neighbor_list=curve[2])
+    e, e0, context = _time_and_context(self, t, context, clip_fea)
+    kwargs.update(e=e0, seq_lens=seq_lens, grid_sizes=grid_sizes, freqs=self.freqs, context=context,
+                  context_lens=None)
+    x = _teacache(self, x, e, e0, lambda x: _blocks(self, x, kwargs), group)
+    # head on the rank's rows (row-local, as usp_dit_forward runs it before its gather), then the
+    # [1, n, out] rows of every rank in rank order
+    x = _gather_rows(self.head(x, e), L, P, group)
+    if curve is not None:
+        x = x[:, curve[1]]                                                    # :655
+    x = self.unpatchify(x, grid_sizes)
+    if getattr(self, "num_steps", None) is not None:     # the TeaCache step counter, where jenga_wan.py set one
         self.cnt += 1
         if self.cnt >= self.num_steps:
             self.cnt = 0
-        return [u.float() for u in x]
-    return forward
+    return [u.float() for u in x]
 
 
 def _blocks(self, x, kwargs):
@@ -227,18 +279,91 @@ def _time_and_context(self, t, context, clip_fea):
 
 def _gather_rows(x, L, P, group):
     """the [1, n, C] rows of every rank in rank order, then the first L"""
+    if group is LOCAL:
+        return x[:, :L]
     parts = [torch.empty_like(x) for _ in range(P)]
     dist.all_gather(parts, x.contiguous(), group=group)
     return torch.cat(parts, dim=1)[:, :L]
 
 
+# ------------------------------------------------------------------------------------------------
+# Wan2.1-I2V: carving (opt-in), the single-GPU forward, the sharded forward
+# ------------------------------------------------------------------------------------------------
+I2V_P_REMAIN_DEFAULT = 0.8      # model_mul.py's WanSelfAttention.forward default
+# the carved self-attention of Wan2.1-I2V: () is dense (the default), else the rates of
+# jenga_wan.py --sa_drop_rates; set by install() (JENGA_WAN_I2V_SA_DROP / JENGA_WAN_I2V_P_REMAIN)
+I2V_SA_DROP_RATES: tuple = ()
+I2V_P_REMAIN = I2V_P_REMAIN_DEFAULT
+
+
+def parse_sa_drop_rates(value) -> tuple:
+    """"d0[,d1]" (or a sequence of one or two numbers) -> (d0[, d1]); "" or None -> () (dense).  Each
+    rate is a drop rate in [0, 1): a rate of 1 would keep no key block."""
+    if value is None:
+        return ()
+    parts = [p.strip() for p in value.split(",")] if isinstance(value, str) else list(value)
+    if parts == [""]:
+        return ()
+    try:
+        rates = tuple(float(p) for p in parts)
+    except (TypeError, ValueError):
+        raise ValueError(f"Wan2.1-I2V sa_drop_rates {value!r}: expected one or two numbers, 'd0[,d1]'") from None
+    if not 1 <= len(rates) <= 2 or not all(0.0 <= d < 1.0 for d in rates):
+        raise ValueError(f"Wan2.1-I2V sa_drop_rates {value!r}: expected one or two drop rates in [0, 1), 'd0[,d1]'")
+    return rates
+
+
+def parse_p_remain(value) -> float:
+    """The p_remain_rates of the carved steps: a number in (0, 1]; "" or None -> 0.8."""
+    if value is None or (isinstance(value, str) and not value.strip()):
+        return I2V_P_REMAIN_DEFAULT
+    try:
+        p = float(value)
+    except (TypeError, ValueError):
+        raise ValueError(f"Wan2.1-I2V p_remain {value!r}: expected a number in (0, 1]") from None
+    if not 0.0 < p <= 1.0:
+        raise ValueError(f"Wan2.1-I2V p_remain {value!r}: expected a number in (0, 1]")
+    return p
+
+
+def set_i2v_carving(sa_drop_rates=None, p_remain=None) -> None:
+    """Turns the carved Wan2.1-I2V self-attention on (rates given) or off (None / "") for every I2V
+    forward of this module, on one GPU and sharded.  Malformed values raise and change nothing."""
+    global I2V_SA_DROP_RATES, I2V_P_REMAIN
+    rates, p = parse_sa_drop_rates(sa_drop_rates), parse_p_remain(p_remain)
+    I2V_SA_DROP_RATES, I2V_P_REMAIN = rates, p
+
+
+def sa_drop_schedule(cnt: int, num_steps: int, rates) -> float:
+    """The drop rate of t2v_generate (jenga_wan.py:189-206) for model call `cnt` of `num_steps`
+    (TeaCache counts the conditional and the unconditional call: sampling step cnt // 2 of
+    num_steps // 2): d0 up to step 25, then d1 (d0 with one rate), warmed up as
+    min(d, step / (steps - 1) * 10 * d).  The blocks run the dense class at <= 0.25."""
+    steps, idx = num_steps // 2, cnt // 2
+    if steps < 2:
+        raise ValueError(f"the Wan drop-rate schedule needs at least two sampling steps, got {steps}")
+    d = rates[0] if idx <= 25 or len(rates) == 1 else rates[1]
+    return min(d, idx / (steps - 1) * 10 * d)
+
+
+@functools.lru_cache(maxsize=8)
+def i2v_curve(f: int, h: int, w: int):
+    """(linear_to_hilbert, hilbert_order, block_neighbor_list) of the latent grid f x h x w: the sliced
+    Gilbert curve and its 128-token block adjacency that jenga_wan.py builds for T2V (:1013-1035) from
+    sliced_gilbert_mapping / sliced_gilbert_block_neighbor_mapping, here from the grid the forward sees
+    (the I2V grid follows the image's aspect ratio, image2video.py:180-193)."""
+    from . import gilbert
+    l2h, h2l = gilbert.mapping_tensors(f, h, w, sliced=True)
+    return l2h, h2l, gilbert.block_neighbor_mapping(f, h, w, sliced=True)
+
+
 def parallelize_wan_i2v(model, group=None, attention=None):
     """Replaces `model.forward` of a Wan2.1-I2V model of wan/modules/model.py (an instance attribute, as
-    WanI2V(use_usp=True) binds usp_dit_forward) with the raster-sharded I2V forward, and sets
+    WanI2V(use_usp=True) binds usp_dit_forward) with the sharded I2V forward, and sets
     `block.self_attn.jenga_sp = attention` on every block.  The blocks must carry the forwards
     install(wan_sp=True) hooks into that module.  attention: a Ulysses object with the
-    hybrid_seq_parallel_attn call contract and the seq_len / dense keywords; None means
-    default_attention(group, "wan").  Returns it."""
+    hybrid_seq_parallel_attn call contract and the seq_len / dense / first_frame_blocks keywords; None
+    means default_attention(group, "wan").  Returns it."""
     _check_model(model, group, "install(wan_sp=True)")
     sp = attention if attention is not None else default_attention(group, variant="wan")
     for block in model.blocks:
@@ -247,41 +372,38 @@ def parallelize_wan_i2v(model, group=None, attention=None):
     return sp
 
 
+def bind_wan_i2v(model) -> None:
+    """The single-GPU Wan2.1-I2V route: hooks the block classes of the model's module (wan/modules/model.py)
+    and binds the one-GPU I2V forward as `model.forward`, an instance attribute that shadows the
+    teacache_forward jenga_wan.py puts on the class."""
+    from . import blocks
+    # the classes the model's blocks are built from (wan/modules/model.py's)
+    blk = model.blocks[0]
+    blocks.patch_plain_wan(types.SimpleNamespace(__name__=type(blk).__module__, WanAttentionBlock=type(blk),
+                                                 WanSelfAttention=type(blk.self_attn)))
+    model.forward = types.MethodType(_i2v_forward_factory(LOCAL), model)
+
+
 def _i2v_forward_factory(group):
     def forward(self, x, t, context, seq_len, clip_fea=None, y=None):
         """usp_dit_forward (xdit_context_parallel.py:66-146) with teacache_forward's step cache, on this
-        rank's raster rows; returns the full output on every rank"""
-        P, r = dist.get_world_size(group), dist.get_rank(group)
+        rank's rows (all rows on one GPU); returns the full output on every rank.  Dense over the raster
+        rows by default; with I2V_SA_DROP_RATES set, teacache_forward's Hilbert order and carved
+        self-attention (jenga_wan.py:559,583-592,655) with the drop rate of sa_drop_schedule."""
         if clip_fea is None or y is None:
-            raise ValueError(f"sequence-parallel {MODEL}-I2V needs clip_fea and y")
-        if len(x) != 1:
-            raise ValueError(f"sequence-parallel {MODEL} runs batch 1, got {len(x)} videos")
-        device = self.patch_embedding.weight.device
-        if self.freqs.device != device:
-            self.freqs = self.freqs.to(device)
-        x = [torch.cat([u, v], dim=0) for u, v in zip(x, y)]
-        # embeddings (replicated)
-        x = [self.patch_embedding(u.unsqueeze(0)) for u in x]
-        grid_sizes = torch.stack([torch.tensor(u.shape[2:], dtype=torch.long) for u in x])
-        x = [u.flatten(2).transpose(1, 2) for u in x]
-        seq_lens = torch.tensor([u.size(1) for u in x], dtype=torch.long)
-        assert seq_lens.max() <= seq_len
-        # rows past L (the sp_size-rounded seq_len of WanI2V.generate) are neither attended nor returned:
-        # each rank takes its raster slice of the L real rows
-        L = int(seq_lens[0])
-        shard_rows(L, P, r)                                  # raises when a rank holds no real row
-        x = shard(x[0], 1, P, r)
-        e, e0, context = _time_and_context(self, t, context, clip_fea)
-        kwargs = dict(e=e0, seq_lens=seq_lens, grid_sizes=grid_sizes, freqs=self.freqs, context=context,
-                      context_lens=None)
-        x = _teacache(self, x, e, e0, lambda x: _blocks(self, x, kwargs), group)
-        # head on the rank's rows (row-local), then the rows of every rank
-        x = _gather_rows(self.head(x, e), L, P, group)
-        x = self.unpatchify(x, grid_sizes)
-        self.cnt += 1
-        if self.cnt >= self.num_steps:
-            self.cnt = 0
-        return [u.float() for u in x]
+            raise ValueError(f"{_route(group)}{MODEL}-I2V needs clip_fea and y")
+        rates = I2V_SA_DROP_RATES
+        if rates:
+            if getattr(self, "num_steps", None) is None:
+                raise RuntimeError(f"{MODEL}-I2V carving follows the sampling step: the model needs the TeaCache "
+                                   "step counter (cnt, num_steps) that jenga_wan.py sets")
+            block_kw = dict(sa_drop_rate=sa_drop_schedule(self.cnt, self.num_steps, rates),
+                            p_remain_rates=I2V_P_REMAIN)
+            return _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, lambda grid: i2v_curve(*grid),
+                                    block_kw)
+        # one GPU: sa_drop_rate 0 on raster rows sends the self-attention to the fused dense call
+        block_kw = dict(sa_drop_rate=0.0) if group is LOCAL else {}
+        return _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, lambda grid: None, block_kw)
     return forward
 
 
