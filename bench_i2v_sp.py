@@ -53,14 +53,14 @@ def main(argv=None):
     from i2v_ref import load_i2v_blocks
     from jenga_b200 import blocks as jb
     from jenga_b200 import gilbert
-    from jenga_b200.hyi2v_sp import check_degree, default_attention, shard
+    from jenga_b200.sharding import check_degree, default_attention, shard
 
     n_double, n_single = (int(v) for v in args.blocks.split(","))
     t, h, w = (int(v) for v in args.grid.split(","))
     hidden, heads, T, valid = 3072, 24, 400, 300
     drop, p_remain, txt_amp = 0.75, 0.3, 0.0
     L = t * h * w
-    check_degree(L, heads, P)
+    check_degree(L, heads, P, "HunyuanVideo-I2V")
     n = L // P
     dev = torch.device("cuda", local)
     mod = load_i2v_blocks(product=True)
@@ -128,7 +128,7 @@ def main(argv=None):
         return torch.cat(parts, 1)
 
     legs = {"single": lambda: forward(L, img_h, cos, sin, ff), "sp": sp_forward}
-    sp = default_attention()
+    sp = default_attention(None, "hyvideo_i2v")
 
     def timed(leg):
         set_sp(sp if leg == "sp" else None)

@@ -53,8 +53,8 @@ def main(argv=None):
     from bench_i2v_blocks import card
     from jenga_b200 import attention as A
     from jenga_b200 import blocks as jb
-    from jenga_b200.hyi2v_sp import default_attention, shard
-    from jenga_b200.wan_sp import _check_world, i2v_curve, shard_rows
+    from jenga_b200.sharding import check_world, default_attention, shard, shard_rows
+    from jenga_b200.wan_sp import i2v_curve
     from test_wan_i2v_sp_cpu import load_plain_wan
     mod = load_plain_wan(wan_sp=False)
     if mod is None:
@@ -65,8 +65,8 @@ def main(argv=None):
     dim, heads, ffn, n_img, n_txt = 5120, 40, 13824, 257, 512
     L = f * h * w
     nb = (L + 127) // 128
-    _check_world(heads, P)
-    n, _ = shard_rows(L, P, r)
+    check_world(heads, P, "Wan2.1")
+    n, _ = shard_rows(L, P, r, "Wan2.1")
     dev = torch.device("cuda", local)
     g = torch.Generator(device=dev).manual_seed(2024)            # the same weights and inputs on every rank
 
@@ -94,7 +94,7 @@ def main(argv=None):
     l2h, h2l, nbr = i2v_curve(f, h, w)
     xh = x0[:, h2l.to(dev)].contiguous()                                # Hilbert rows
     carve = dict(sa_drop_rate=args.sa_drop_rate, block_neighbor_list=nbr, p_remain_rates=0.8)
-    sp = default_attention(variant="wan")
+    sp = default_attention(None, "wan")
     # leg -> (rows, block keyword arguments, sharded)
     legs = {
         "single_dense": (x0, dict(sa_drop_rate=0.0), False),

@@ -51,8 +51,7 @@ def main(argv=None):
     P, r = dist.get_world_size(), dist.get_rank()
     from bench_i2v_blocks import card
     from jenga_b200 import blocks as jb
-    from jenga_b200.hyi2v_sp import default_attention, shard
-    from jenga_b200.wan_sp import _check_world, shard_rows
+    from jenga_b200.sharding import check_world, default_attention, shard, shard_rows
     from test_wan_i2v_sp_cpu import load_plain_wan
     mod = load_plain_wan(wan_sp=True)
     if mod is None:
@@ -61,8 +60,8 @@ def main(argv=None):
     f, h, w = (int(v) for v in args.grid.split(","))
     dim, heads, ffn, n_img, n_txt = 5120, 40, 13824, 257, 512
     L = f * h * w
-    _check_world(heads, P)
-    n, _ = shard_rows(L, P, r)
+    check_world(heads, P, "Wan2.1")
+    n, _ = shard_rows(L, P, r, "Wan2.1")
     dev = torch.device("cuda", local)
     g = torch.Generator(device=dev).manual_seed(2024)            # the same weights and inputs on every rank
 
@@ -100,7 +99,7 @@ def main(argv=None):
         dist.all_gather(parts, out.contiguous())                     # as the sharded forward does (of the head)
         return torch.cat(parts, 1)[:, :L]
 
-    sp = default_attention(variant="wan")
+    sp = default_attention(None, "wan")
 
     def set_sp(on):
         for b_ in blks:

@@ -57,16 +57,15 @@ def main(argv=None):
     from bench_i2v_blocks import card
     from jenga_b200 import blocks as jb
     from jenga_b200 import gilbert
-    from jenga_b200.hyi2v_sp import default_attention, shard
-    from jenga_b200.wan_sp import _check_world, shard_rows
+    from jenga_b200.sharding import check_world, default_attention, shard, shard_rows
 
     dim, heads, ffn, grid_default = MODELS[args.model]
     f, h, w = (int(v) for v in (args.grid or grid_default).split(","))
     p_remain, Lc = 0.8, 512
     drops = {"carved": 0.7, "dense": 0.2}
     L = f * h * w
-    _check_world(heads, P)
-    n, real = shard_rows(L, P, r)
+    check_world(heads, P, "Wan2.1")
+    n, real = shard_rows(L, P, r, "Wan2.1")
     dev = torch.device("cuda", local)
     mod = ref_loader.load_blocks(product=True)[1]
     jb.remove_gather_hook()
@@ -112,7 +111,7 @@ def main(argv=None):
         dist.all_gather(parts, out.contiguous())                     # as wan_sp's forward does (of the head)
         return torch.cat(parts, 1)[:, :L]
 
-    sp = default_attention(variant="wan")
+    sp = default_attention(None, "wan")
 
     def set_sp(on):
         for b_ in blks:

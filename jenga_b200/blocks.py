@@ -54,69 +54,43 @@ from __future__ import annotations
 
 import functools
 import importlib.abc
-import importlib.machinery
 import sys
+from typing import Callable, NamedTuple
 
 import torch
 
 from . import dense as DN
+from . import hyi2v_sp, wan_sp
 from . import hyvideo as HY
 from . import ulysses as U
 from . import wan as WAN
 from .flash_attn_shim import flash_attn_func
+from .sharding import world
 
-_HY_MODULES = ("hyvideo.modules.models_mul_block_gc_ha_multigpu",)
-_I2V_MODULES = ("hyvideo_i2v.modules.models_mul",)
-_WAN_MODULES = ("wan.modules.model_mul",)
-# opt-in (install(i2v_sp=True) / JENGA_I2V_SP=1): hyvideo_i2v/inference.py's parallelize_transformer
-# is swapped for the Hilbert-sharded forward of hyi2v_sp.py
-_I2V_SP_MODULES = ("hyvideo_i2v.inference",)
+# the opt-in routes (install(i2v_sp=True) / JENGA_I2V_SP=1, install(wan_sp=True) / JENGA_WAN_SP=1): see _HOOKS
 I2V_SP = False
-# opt-in (install(wan_sp=True) / JENGA_WAN_SP=1): wan/distributed/xdit_context_parallel.py's
-# usp_dit_forward / usp_attn_forward are swapped for the Hilbert-sharded TeaCache forward of wan_sp.py
-_WAN_SP_MODULES = ("wan.distributed.xdit_context_parallel",)
-# under the same switch: wan/modules/model.py, the plain Wan model WanI2V loads (image2video.py:21), gets
-# the fused WanAttentionBlock.forward and a WanSelfAttention.forward for its signatures; without the
-# switch it is not touched
-_WAN_PLAIN_MODULES = ("wan.modules.model",)
-# wan/image2video.py: WanI2V(use_usp=False) gets the single-GPU I2V forward of wan_sp.py, and the plain
-# model's blocks the fused forwards, when the pipeline is built (wan.modules.model itself stays untouched
-# at import, which only WanI2V imports)
-_WAN_I2V_PIPE_MODULES = ("wan.image2video",)
 WAN_SP = False
 
 
 def set_i2v_sp(on: bool) -> None:
     """Turns the sequence-parallel I2V route on or off for the rest of the process.  Off also puts the
     reference's parallelize_transformer back if hyvideo_i2v.inference was already swapped."""
-    global I2V_SP
-    I2V_SP = bool(on)
-    inf = sys.modules.get(_I2V_SP_MODULES[0])
-    fn = getattr(inf, "parallelize_transformer", None)
-    if not I2V_SP and getattr(fn, "__jenga_b200__", False):
-        inf.parallelize_transformer = fn.__wrapped__
+    _set_route("I2V_SP", on)
 
 
 def set_wan_sp(on: bool) -> None:
     """Turns the sequence-parallel Wan route on or off for the rest of the process.  Off also puts the
     reference's usp_dit_forward / usp_attn_forward back if wan.distributed.xdit_context_parallel was
-    already swapped (a model that has bound them keeps what it bound)."""
-    global WAN_SP
-    WAN_SP = bool(on)
-    xdit = sys.modules.get(_WAN_SP_MODULES[0])
-    if not WAN_SP and xdit is not None:
-        from .wan_sp import uninstall_usp
-        uninstall_usp(xdit)
-    plain = sys.modules.get(_WAN_PLAIN_MODULES[0])
-    if not WAN_SP and plain is not None:
-        for cls in ("WanSelfAttention", "WanAttentionBlock"):
-            fn = getattr(getattr(plain, cls, None), "forward", None)
-            if getattr(fn, "__jenga_b200__", False):
-                getattr(plain, cls).forward = fn.__wrapped__
+    already swapped (a model that has bound them keeps what it bound), and wan.modules.model's forwards."""
+    _set_route("WAN_SP", on)
 
 
-def _sp_modules():
-    return (_I2V_SP_MODULES if I2V_SP else ()) + (_WAN_SP_MODULES + _WAN_PLAIN_MODULES if WAN_SP else ())
+def _set_route(switch: str, on: bool) -> None:
+    globals()[switch] = bool(on)
+    if not on:
+        for name, hook in _HOOKS.items():
+            if hook.switch == switch and hook.restore is not None and name in sys.modules:
+                hook.restore(sys.modules[name])
 
 
 STATS = {"hy_double": 0, "hy_single": 0, "i2v_double": 0, "i2v_single": 0, "i2v_double_sp": 0,
@@ -263,7 +237,7 @@ def _attention_section(self, mod, img_qkv, txt_qkv, norms, *, freqs_cis, cu_seql
         # top_k is the single-GPU rule over the GLOBAL image length, not the T2V SP quirk
         # P*int((1-drop)*(L_loc//128)) (SURVEY a-7, App. A-12): the sharded I2V forward computes
         # what one GPU computes
-        top_k = HY.select_block_num(sa_drop_rate, L * U._group_size_rank(jsp.group)[0])
+        top_k = HY.select_block_num(sa_drop_rate, L * world(jsp.group)[0])
         q, k, v, _ = HY.attention_prologue(img_qkv, txt_qkv, self.heads_num, wq_i, wk_i, wq_t, wk_t, eps, freqs_cis,
                                            want_pool=False)
         # the I2V reference module has no my_parallel_attention: the restatement of attenion.py:159-195
@@ -392,7 +366,7 @@ def _i2v_ok(self, L, T, condition_type, first_frame_mask):
     if getattr(self, "hybrid_seq_parallel_attn", None):
         return False
     jsp = getattr(self, "jenga_sp", None)
-    S = L * (U._group_size_rank(jsp.group)[0] if jsp is not None else 1) + T
+    S = L * (world(jsp.group)[0] if jsp is not None else 1) + T
     return (not (condition_type == "token_replace" and first_frame_mask is None)
             and (S + HY.BLOCK - 1) // HY.BLOCK > _I2V_TEXT_BLOCKS)
 
@@ -514,7 +488,7 @@ def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=None, freq_
     if sa_drop_rate is None:
         if jsp is None:
             return None
-        _, r = U._group_size_rank(jsp.group)
+        _, r = world(jsp.group)
         n = x.shape[1]
         L = int(torch.prod(grid_sizes[0]))
         rows = torch.arange(r * n, (r + 1) * n, device=x.device)
@@ -695,6 +669,26 @@ def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_le
 # ------------------------------------------------------------------------------------------------
 # patching
 # ------------------------------------------------------------------------------------------------
+def _swap(owner, attr: str, replacement) -> bool:
+    """Sets owner.attr = replacement, marked as jenga_b200's (`__jenga_b200__`) with the original as its
+    `__wrapped__`.  False, and nothing changes, when owner has no such attribute or it is swapped already."""
+    orig = getattr(owner, attr, None)
+    if orig is None or getattr(orig, "__jenga_b200__", False):
+        return False
+    replacement.__jenga_b200__ = True
+    replacement.__wrapped__ = orig
+    setattr(owner, attr, replacement)
+    return True
+
+
+def _unswap(owner, *attrs: str) -> None:
+    """Puts back the originals that _swap replaced, where owner.attr is swapped"""
+    for attr in attrs:
+        fn = getattr(owner, attr, None)
+        if getattr(fn, "__jenga_b200__", False):
+            setattr(owner, attr, fn.__wrapped__)
+
+
 def _patched(orig, fused):
     """The patched forward: `fused` takes the reference arguments and returns None for a call it does
     not take; that call then runs `orig` with exactly the caller's arguments."""
@@ -704,35 +698,22 @@ def _patched(orig, fused):
             STATS["fallback"] += 1
             out = orig(self, *args, **kwargs)
         return out
-    forward.__jenga_b200__ = True
-    forward.__wrapped__ = orig
     return forward
 
 
-def patch_module(mod) -> list[str]:
-    """Patches the block classes of an already imported reference module; returns what it did."""
-    name = mod.__name__
-    if name in _I2V_SP_MODULES:
-        from .hyi2v_sp import install_parallelize_transformer
-        return [f"{name}.parallelize_transformer"] if I2V_SP and install_parallelize_transformer(mod) else []
-    if name in _WAN_SP_MODULES:
-        from .wan_sp import install_usp
-        return [f"{name}.usp_dit_forward", f"{name}.usp_attn_forward"] if WAN_SP and install_usp(mod) else []
-    if name in _WAN_I2V_PIPE_MODULES:
-        return _wrap_wan_i2v_init(mod)
-    fused = {}
-    if name in _WAN_PLAIN_MODULES:
-        return patch_plain_wan(mod) if WAN_SP else []
-    if name.startswith(("hyvideo.", "hyvideo_i2v.")):
-        # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and
-        # a ragged S with four text blocks: its own pair of entry points
-        i2v = name.startswith("hyvideo_i2v.")
-        fused["MMDoubleStreamBlock"] = functools.partial(_i2v_double if i2v else _hy_double, mod)
-        fused["MMSingleStreamBlock"] = functools.partial(_i2v_single if i2v else _hy_single, mod)
-    # WanI2VCrossAttention overrides forward itself and is left as it is; the fused block forward runs
-    # its fused form (_wan_i2v_cross)
-    fused.update(WanSelfAttention=_wan_self, WanT2VCrossAttention=_wan_cross, WanAttentionBlock=_wan_block)
-    return _patch_classes(mod, fused)
+def _patch_classes(mod, fused) -> list[str]:
+    done = []
+    for cls, body in fused.items():
+        owner = getattr(mod, cls, None)
+        if owner is not None and _swap(owner, "forward", _patched(owner.forward, body)):
+            done.append(f"{mod.__name__}.{cls}.forward")
+    return done
+
+
+def _patch_hy(double, single):
+    """the patch of a HunyuanVideo block module: both stream kinds, with the module's own helpers"""
+    return lambda mod: _patch_classes(mod, dict(MMDoubleStreamBlock=functools.partial(double, mod),
+                                                MMSingleStreamBlock=functools.partial(single, mod)))
 
 
 def patch_plain_wan(mod) -> list[str]:
@@ -743,12 +724,17 @@ def patch_plain_wan(mod) -> list[str]:
     return _patch_classes(mod, dict(WanSelfAttention=_wan_i2v_self, WanAttentionBlock=_wan_plain_block))
 
 
+def _unpatch_plain_wan(mod) -> None:
+    for cls in ("WanSelfAttention", "WanAttentionBlock"):
+        _unswap(getattr(mod, cls, None), "forward")
+
+
 def _wrap_wan_i2v_init(mod) -> list[str]:
     """WanI2V.__init__ of wan/image2video.py, followed, for a pipeline built with use_usp=False, by
     wan_sp.bind_wan_i2v on its WanModel: the single-GPU I2V forward.  With use_usp=True the pipeline keeps
     what it bound (usp_dit_forward; install(wan_sp=True) decides what that is)."""
     cls = getattr(mod, "WanI2V", None)
-    if cls is None or getattr(cls.__init__, "__jenga_b200__", False):
+    if cls is None:
         return []
     orig = cls.__init__
 
@@ -757,21 +743,56 @@ def _wrap_wan_i2v_init(mod) -> list[str]:
         orig(self, *args, **kwargs)
         # a dit_fsdp model is an FSDP wrapper, whose forward gathers the parameters: left as it is
         if not getattr(self, "use_usp", False) and type(self.model).__name__ == "WanModel":
-            from .wan_sp import bind_wan_i2v
-            bind_wan_i2v(self.model)
+            wan_sp.bind_wan_i2v(self.model)
 
-    __init__.__jenga_b200__ = True
-    cls.__init__ = __init__
-    return [f"{mod.__name__}.WanI2V.__init__"]
+    return [f"{mod.__name__}.WanI2V.__init__"] if _swap(cls, "__init__", __init__) else []
 
 
-def _patch_classes(mod, fused) -> list[str]:
-    done = []
-    for cls, body in fused.items():
-        if hasattr(mod, cls) and not getattr(getattr(mod, cls).forward, "__jenga_b200__", False):
-            getattr(mod, cls).forward = _patched(getattr(mod, cls).forward, body)
-            done.append(f"{mod.__name__}.{cls}.forward")
-    return done
+class _Hook(NamedTuple):
+    patch: Callable[..., list[str]]             # module -> what it patched
+    label: str                                  # the route the stderr line names
+    switch: str | None = None                   # the global (I2V_SP, WAN_SP) of an opt-in route; None: always on
+    restore: Callable[..., None] | None = None  # module -> None: undoes `patch` when the switch is turned off
+
+
+_FUSED = "fused attention section"
+# every module the import hook patches right after it is executed
+_HOOKS = {
+    "hyvideo.modules.models_mul_block_gc_ha_multigpu": _Hook(_patch_hy(_hy_double, _hy_single), _FUSED),
+    # hyvideo_i2v/modules/models_mul.py has its own argument order, the token_replace modulation and a
+    # ragged S with four text blocks: its own pair of entry points
+    "hyvideo_i2v.modules.models_mul": _Hook(_patch_hy(_i2v_double, _i2v_single), _FUSED),
+    # WanI2VCrossAttention overrides forward itself and is left as it is; the fused block forward runs
+    # its fused form (_wan_i2v_cross)
+    "wan.modules.model_mul": _Hook(lambda mod: _patch_classes(mod, dict(
+        WanSelfAttention=_wan_self, WanT2VCrossAttention=_wan_cross, WanAttentionBlock=_wan_block)), _FUSED),
+    # WanI2V(use_usp=False) gets the single-GPU I2V forward of wan_sp.py, and the plain model's blocks the
+    # fused forwards, when the pipeline is built (wan.modules.model itself, which only WanI2V imports,
+    # stays untouched at import without the Wan switch).  Not undone by set_wan_sp(False).
+    "wan.image2video": _Hook(_wrap_wan_i2v_init, "single-GPU Wan I2V route"),
+    # parallelize_transformer is swapped for the Hilbert-sharded forward of hyi2v_sp.py
+    "hyvideo_i2v.inference": _Hook(hyi2v_sp.install_parallelize_transformer, "sequence-parallel I2V route",
+                                   "I2V_SP", lambda mod: _unswap(mod, "parallelize_transformer")),
+    # usp_dit_forward / usp_attn_forward are swapped for the Hilbert-sharded TeaCache forward of wan_sp.py
+    "wan.distributed.xdit_context_parallel": _Hook(
+        wan_sp.install_usp, "sequence-parallel Wan route", "WAN_SP",
+        lambda mod: _unswap(mod, "usp_dit_forward", "usp_attn_forward")),
+    # wan/modules/model.py, the plain Wan model WanI2V loads (image2video.py:21), gets the fused
+    # WanAttentionBlock.forward and a WanSelfAttention.forward for its signatures
+    "wan.modules.model": _Hook(patch_plain_wan, _FUSED, "WAN_SP", _unpatch_plain_wan),
+}
+
+
+def _active_hook(name: str) -> _Hook | None:
+    """the hook of module `name` when there is one and its route is on"""
+    hook = _HOOKS.get(name)
+    return hook if hook is not None and (hook.switch is None or globals()[hook.switch]) else None
+
+
+def patch_module(mod) -> list[str]:
+    """Patches an already imported reference module by its hook; returns what it did."""
+    hook = _active_hook(mod.__name__)
+    return hook.patch(mod) if hook is not None else []
 
 
 # ------------------------------------------------------------------------------------------------
@@ -788,21 +809,17 @@ class _PatchingLoader(importlib.abc.Loader):
         self.inner.exec_module(module)
         done = patch_module(module)
         if done:
-            what = ("sequence-parallel I2V route" if module.__name__ in _I2V_SP_MODULES
-                    else "sequence-parallel Wan route" if module.__name__ in _WAN_SP_MODULES
-                    else "single-GPU Wan I2V route" if module.__name__ in _WAN_I2V_PIPE_MODULES
-                    else "fused attention section")
-            print(f"[jenga_b200] {what} installed: {', '.join(done)}", file=sys.stderr)
+            print(f"[jenga_b200] {_HOOKS[module.__name__].label} installed: {', '.join(done)}", file=sys.stderr)
 
     def __getattr__(self, item):
         return getattr(self.inner, item)
 
 
 class _PatchFinder(importlib.abc.MetaPathFinder):
-    targets = _HY_MODULES + _I2V_MODULES + _WAN_MODULES + _WAN_I2V_PIPE_MODULES
+    targets = tuple(_HOOKS)
 
     def find_spec(self, fullname, path, target=None):
-        if fullname not in self.targets and fullname not in _sp_modules():
+        if _active_hook(fullname) is None:
             return None
         for finder in sys.meta_path:
             if finder is self or not hasattr(finder, "find_spec"):
@@ -818,7 +835,7 @@ def install_block_hook() -> None:
     """Idempotent.  Also patches target modules that were imported before the hook existed."""
     if not any(isinstance(f, _PatchFinder) for f in sys.meta_path):
         sys.meta_path.insert(0, _PatchFinder())
-    for name in _PatchFinder.targets + _sp_modules():
+    for name in _PatchFinder.targets:
         if name in sys.modules and not getattr(sys.modules[name], "__jenga_b200__", False):
             patch_module(sys.modules[name])
 

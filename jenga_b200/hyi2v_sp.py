@@ -18,53 +18,21 @@ step skipping.  Only the Linears run on a rank's rows instead of all rows.
 """
 from __future__ import annotations
 
-import os
+import functools
 import types
 
 import torch
 import torch.distributed as dist
 
+from . import sharding
+from .sharding import check_fused_blocks, default_attention, gather_rows, shard, world
+
+MODEL = "HunyuanVideo-I2V"
 # jenga_hyi2v.py:32 — the denoising steps that run the block loop; every other step adds the
 # residual of the last computed step
 STEP_CALC = (0, 1, 2, 3, 5, 7, 10, 13, 16, 19, 22, 25, 28, 31, 34, 37, 40, 42, 44, 45, 46, 47, 48, 49)
-
-
-def check_degree(img_tokens: int, heads: int, world: int, model: str = "HunyuanVideo-I2V") -> None:
-    """The layout needs whole head groups per rank and, for a non-zero img_tokens, whole image slices
-    per rank.  `model` names the model in the message (the Wan route, wan_sp.py, pads its slices
-    instead and passes 0).  Under the ragged head split (ulysses.RAGGED_HEADS) any head count of at
-    least `world` is accepted."""
-    from .ulysses import ragged
-    if ragged(heads, world) and heads < world:
-        raise ValueError(f"sequence-parallel {model}: {heads} attention heads over {world} ranks leave a rank "
-                         "without a head")
-    if heads % world and not ragged(heads, world):
-        raise ValueError(f"sequence-parallel {model}: {heads} attention heads do not split over "
-                         f"{world} ranks (the degree must divide the head count)")
-    if img_tokens % world:
-        raise ValueError(f"sequence-parallel {model}: {img_tokens} image tokens do not split over "
-                         f"{world} ranks (the degree must divide the image token count)")
-
-
-def default_attention(group=None, variant: str = "hyvideo_i2v"):
-    """UlyssesFusedAttention(variant=variant) when every rank can map symmetric memory, else
-    UlyssesCarvedAttention (NCCL all-to-all) — the all-ranks agreement install() uses for HunyuanVideo.
-    JENGA_ULYSSES=nccl picks the NCCL form."""
-    from .ulysses import UlyssesCarvedAttention, UlyssesFusedAttention
-    g = group if group is not None else dist.group.WORLD
-    ok = 0
-    if os.environ.get("JENGA_ULYSSES", "fused") != "nccl" and dist.get_backend(g) == "nccl":
-        try:
-            import torch.distributed._symmetric_memory as symm
-            symm.enable_symm_mem_for_group(g.group_name)
-            ok = 1
-        except Exception:  # noqa: BLE001
-            ok = 0
-        t = torch.tensor([ok], device="cuda")
-        dist.all_reduce(t, op=dist.ReduceOp.MIN, group=g)
-        ok = int(t.item())
-    return (UlyssesFusedAttention(group=g, variant=variant) if ok
-            else UlyssesCarvedAttention(group=group, variant=variant))
+# check_degree(img_tokens, heads, world): whole head groups and whole image slices per rank
+check_degree = functools.partial(sharding.check_degree, model=MODEL)
 
 
 def get_cu_seqlens(text_mask: torch.Tensor, img_len: int, device) -> torch.Tensor:
@@ -78,19 +46,6 @@ def get_cu_seqlens(text_mask: torch.Tensor, img_len: int, device) -> torch.Tenso
                       torch.full((1,), text_mask.shape[1] + img_len, dtype=torch.int32, device=device)])
 
 
-def shard(x: torch.Tensor, dim: int, world: int, rank: int) -> torch.Tensor:
-    """The contiguous slice `rank` of `world` along `dim`: rows [rank*n, min((rank+1)*n, len)) with
-    n = ceil(len / world), zero-padded to n rows (no padding when the length divides by world)."""
-    n = -(-x.shape[dim] // world)
-    lo = min(rank * n, x.shape[dim])
-    part = x.narrow(dim, lo, min(n, x.shape[dim] - lo))
-    if part.shape[dim] == n:
-        return part.contiguous()
-    pad = list(x.shape)
-    pad[dim] = n - part.shape[dim]
-    return torch.cat([part, x.new_zeros(pad)], dim)
-
-
 def _step_calc(transformer):
     """jenga_hyi2v.py's own `step_calc` when its ra_forward has been bound to the class, else STEP_CALC"""
     ra = getattr(type(transformer), "ra_forward", None)
@@ -102,19 +57,13 @@ def parallelize_i2v(transformer, group=None, attention=None):
     """Replaces `transformer.forward` (an instance attribute, as parallelize_transformer sets it) with
     the sharded I2V forward and sets `block.jenga_sp = attention` on every double and single block.
     attention: a Ulysses object with the hybrid_seq_parallel_attn call contract; None means
-    default_attention(group).  Returns the attention object."""
+    default_attention(group, "hyvideo_i2v").  Returns the attention object."""
     if not dist.is_initialized():
-        raise RuntimeError("sequence-parallel HunyuanVideo-I2V needs an initialised process group")
-    P = dist.get_world_size(group)
-    check_degree(0, int(transformer.heads_num), P)
+        raise RuntimeError(f"sequence-parallel {MODEL} needs an initialised process group")
+    check_degree(0, int(transformer.heads_num), dist.get_world_size(group))
     blocks = list(transformer.double_blocks) + list(transformer.single_blocks)
-    for block in blocks:
-        # an unpatched forward ignores jenga_sp: every rank would attend over its own rows alone
-        if not getattr(type(block).forward, "__jenga_b200__", False):
-            raise RuntimeError(f"{type(block).__module__}.{type(block).__name__}.forward is not the fused "
-                               "jenga_b200 forward: install() (fused_blocks=True) must run before the I2V "
-                               "model module is imported")
-    sp = attention if attention is not None else default_attention(group)
+    check_fused_blocks(blocks, "I2V", "install() (fused_blocks=True)", instance_forward=False)
+    sp = attention if attention is not None else default_attention(group, "hyvideo_i2v")
     for block in blocks:
         # deliberately not `hybrid_seq_parallel_attn`: a block with that attribute keeps running the
         # reference's own (dense) SP forward
@@ -130,7 +79,7 @@ def _forward_factory(group):
                 guidance: torch.Tensor = None, return_dict: bool = True, token_per_block=128):
         """jenga_hyi2v.py:53-221 (ra_forward) on this rank's Hilbert slice; returns the full output
         on every rank"""
-        P, r = dist.get_world_size(group), dist.get_rank(group)
+        P, r = world(group)
         for name in ("hilbert_order", "linear_to_hilbert", "curve_sel", "sa_drop_rate", "p_remain_rates"):
             if getattr(self, name, None) is None:
                 raise RuntimeError(f"sequence-parallel HunyuanVideo-I2V: transformer.{name} is not set "
@@ -211,10 +160,8 @@ def _forward_factory(group):
         if self.cnt == self.num_steps:
             self.cnt = 0
         # the image rows of every rank in rank order (NCCL, once per forward), then replicated as
-        # jenga_hyvideo_multigpu.py:193-198 does
-        parts = [torch.empty_like(img) for _ in range(P)]
-        dist.all_gather(parts, img.contiguous(), group=group)
-        img = torch.cat(parts, dim=1)
+        # jenga_hyvideo_multigpu.py:193-198 does (P*n = L rows: nothing is cut)
+        img = gather_rows(img, L, P, group)
         img = img[:, self.linear_to_hilbert]                                       # :213-217
         img = self.final_layer(img, vec)
         img = self.unpatchify(img, tt, th, tw)
@@ -225,21 +172,17 @@ def _forward_factory(group):
     return forward
 
 
-def install_parallelize_transformer(inference_module) -> bool:
+def install_parallelize_transformer(inference_module) -> list[str]:
     """Swaps hyvideo_i2v.inference.parallelize_transformer for one that calls parallelize_i2v.
     Inference.from_pretrained calls it with ulysses_degree > 1, after its xfuser / NCCL process-group
     initialisation (hyvideo_i2v/inference.py:226-250, :568-569); the sharded forward reads the Jenga
     attributes jenga_hyi2v.py sets later (hilbert_order, curve_sels, sa_drop_rates, p_remain_rates)
-    when it runs.  Returns False when there is nothing to swap or it is already swapped."""
-    orig = getattr(inference_module, "parallelize_transformer", None)
-    if orig is None or getattr(orig, "__jenga_b200__", False):
-        return False
+    when it runs.  Returns what it swapped: nothing when there is nothing to swap or it is already swapped."""
+    from .blocks import _swap
 
     def parallelize_transformer(pipe):
+        """jenga_b200: Hilbert-sharded I2V forward over the Ulysses exchange"""
         parallelize_i2v(pipe.transformer)
 
-    parallelize_transformer.__jenga_b200__ = True
-    parallelize_transformer.__wrapped__ = orig
-    parallelize_transformer.__doc__ = "jenga_b200: Hilbert-sharded I2V forward over the Ulysses exchange"
-    inference_module.parallelize_transformer = parallelize_transformer
-    return True
+    swapped = _swap(inference_module, "parallelize_transformer", parallelize_transformer)
+    return [f"{inference_module.__name__}.parallelize_transformer"] if swapped else []

@@ -68,7 +68,7 @@ def install(flash_attn: bool = True, gilbert: bool = True, ulysses: bool = True,
     from . import attention as A
     from . import flash_attn_shim as F
     from . import gilbert as G
-    from . import ulysses as U
+    from .sharding import default_attention
 
     def variant(name, text_blocks, p):
         def block_sparse_attention(query, key, value, top_k, block_size_M=128, block_size_N=128,
@@ -103,28 +103,11 @@ def install(flash_attn: bool = True, gilbert: bool = True, ulysses: bool = True,
             def __init__(self, *a, **k):
                 pass
 
-            @classmethod
-            def _get(cls):
-                if cls._impl is None:
-                    import torch
-                    import torch.distributed as dist
-                    want_fused = os.environ.get("JENGA_ULYSSES", "fused") != "nccl"
-                    ok = 0
-                    if want_fused and dist.is_initialized() and dist.get_backend() == "nccl":
-                        try:
-                            import torch.distributed._symmetric_memory as symm
-                            symm.enable_symm_mem_for_group(dist.group.WORLD.group_name)
-                            ok = 1
-                        except Exception:  # noqa: BLE001
-                            ok = 0
-                        t = torch.tensor([ok], device="cuda")
-                        dist.all_reduce(t, op=dist.ReduceOp.MIN)
-                        ok = int(t.item())
-                    cls._impl = U.UlyssesFusedAttention() if ok else U.UlyssesCarvedAttention(group=None)
-                return cls._impl
-
             def forward(self, attn, query, key, value, **kw):
-                return self._get()(attn, query, key, value, **kw)
+                cls = type(self)
+                if cls._impl is None:
+                    cls._impl = default_attention(None, "hyvideo")
+                return cls._impl(attn, query, key, value, **kw)
 
             __call__ = forward
         modname = "hyvideo.modules.xdit_ring_atten"

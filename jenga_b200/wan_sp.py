@@ -55,45 +55,17 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .hyi2v_sp import check_degree, default_attention, shard
+from . import sharding
+from .sharding import LOCAL, check_fused_blocks, default_attention, gather_rows, shard, world
 
 MODEL = "Wan2.1"
-MAX_WORLD = 8        # the peer arrays of the fused exchange and of the attention epilogue
-
-
-class _Local:
-    """the group of the one-GPU forward: one rank, no process group, no exchange"""
-
-    def __repr__(self):
-        return "LOCAL"
-
-
-LOCAL = _Local()
-
-
-def _world(group) -> tuple[int, int]:
-    return (1, 0) if group is LOCAL else (dist.get_world_size(group), dist.get_rank(group))
+# the Wan degree rule, (heads, world), and the rows per rank, (L, world, rank) -> (n, real)
+_check_world = functools.partial(sharding.check_world, model=MODEL)
+shard_rows = functools.partial(sharding.shard_rows, model=MODEL)
 
 
 def _route(group) -> str:
     return "single-GPU " if group is LOCAL else "sequence-parallel "
-
-
-def _check_world(heads: int, world: int) -> None:
-    check_degree(0, heads, world, model=MODEL)
-    if world > MAX_WORLD:
-        raise ValueError(f"sequence-parallel {MODEL}: {world} ranks; the Ulysses exchange is built for at "
-                         f"most {MAX_WORLD} (one NVLink box)")
-
-
-def shard_rows(L: int, world: int, rank: int) -> tuple[int, int]:
-    """(n, real): rows per rank, n = ceil(L / world), and how many of rank `rank`'s n rows are real.
-    Raises when some rank would hold no real row."""
-    n = -(-L // world)
-    if L - (world - 1) * n <= 0:
-        raise ValueError(f"sequence-parallel {MODEL}: {L} tokens over {world} ranks leave the last rank "
-                         f"without a real row ({n} rows per rank)")
-    return n, max(0, min(n, L - rank * n))
 
 
 def _sinusoidal_embedding_1d(model):
@@ -119,31 +91,21 @@ def parallelize_wan(model, group=None, attention=None):
     with the sharded TeaCache forward and sets `block.self_attn.jenga_sp = attention` on every block.
     attention: a Ulysses object with the hybrid_seq_parallel_attn call contract and the seq_len /
     dense / first_frame_blocks keywords; None means default_attention(group, "wan").  Returns it."""
-    _check_model(model, group, "install() (fused_blocks=True)")
-    sp = attention if attention is not None else default_attention(group, variant="wan")
-    for block in model.blocks:
-        block.self_attn.jenga_sp = sp
-    model.forward = types.MethodType(_forward_factory(group), model)
-    return sp
+    return _parallelize(model, group, attention, "install() (fused_blocks=True)", _forward_factory)
 
 
-def _check_model(model, group, install_call: str) -> None:
-    """The degree, and a fused, unshadowed self-attention in every block: an unpatched one ignores
-    jenga_sp, so every rank would attend over its own rows alone"""
+def _parallelize(model, group, attention, install_call: str, forward_factory):
+    """The checks (the degree, and a fused, unshadowed self-attention in every block), then jenga_sp on
+    every block and the forward of forward_factory(group) on the model"""
     if not dist.is_initialized():
         raise RuntimeError(f"sequence-parallel {MODEL} needs an initialised process group")
     _check_world(int(model.num_heads), dist.get_world_size(group))
+    check_fused_blocks([block.self_attn for block in model.blocks], "Wan", install_call)
+    sp = attention if attention is not None else default_attention(group, "wan")
     for block in model.blocks:
-        sa = block.self_attn
-        if not getattr(type(sa).forward, "__jenga_b200__", False):
-            raise RuntimeError(f"{type(sa).__module__}.{type(sa).__name__}.forward is not the fused "
-                               f"jenga_b200 forward: {install_call} must run before the Wan model module is "
-                               "imported")
-        inst = sa.__dict__.get("forward")
-        if inst is not None and not getattr(getattr(inst, "__func__", inst), "__jenga_b200__", False):
-            raise RuntimeError(f"{type(sa).__name__} has an instance forward ({getattr(inst, '__name__', inst)}) "
-                               "that is not the jenga_b200 one: it would run instead of the sharded "
-                               "self-attention (install(wan_sp=True) swaps usp_attn_forward)")
+        block.self_attn.jenga_sp = sp
+    model.forward = types.MethodType(forward_factory(group), model)
+    return sp
 
 
 def _teacache(self, x, e, e0, run_blocks, group):
@@ -206,7 +168,7 @@ def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of,
     is that slice, or, without a curve, the raster rows.  block_kw: what the blocks get besides the
     arguments of model.py's WanAttentionBlock.forward (with a curve, also freq_remap and
     block_neighbor_list).  group LOCAL: one GPU, no exchange."""
-    P, r = _world(group)
+    P, r = world(group)
     if len(x) != 1:
         raise ValueError(f"{_route(group)}{MODEL} runs batch 1, got {len(x)} videos")
     device = self.patch_embedding.weight.device
@@ -246,7 +208,7 @@ def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of,
     x = _teacache(self, x, e, e0, lambda x: _blocks(self, x, kwargs), group)
     # head on the rank's rows (row-local, as usp_dit_forward runs it before its gather), then the
     # [1, n, out] rows of every rank in rank order
-    x = _gather_rows(self.head(x, e), L, P, group)
+    x = gather_rows(self.head(x, e), L, P, group)
     if curve is not None:
         x = x[:, curve[1]]                                                    # :655
     x = self.unpatchify(x, grid_sizes)
@@ -275,15 +237,6 @@ def _time_and_context(self, t, context, clip_fea):
     if clip_fea is not None:
         context = torch.concat([self.img_emb(clip_fea), context], dim=1)
     return e, e0, context
-
-
-def _gather_rows(x, L, P, group):
-    """the [1, n, C] rows of every rank in rank order, then the first L"""
-    if group is LOCAL:
-        return x[:, :L]
-    parts = [torch.empty_like(x) for _ in range(P)]
-    dist.all_gather(parts, x.contiguous(), group=group)
-    return torch.cat(parts, dim=1)[:, :L]
 
 
 # ------------------------------------------------------------------------------------------------
@@ -364,12 +317,7 @@ def parallelize_wan_i2v(model, group=None, attention=None):
     install(wan_sp=True) hooks into that module.  attention: a Ulysses object with the
     hybrid_seq_parallel_attn call contract and the seq_len / dense / first_frame_blocks keywords; None
     means default_attention(group, "wan").  Returns it."""
-    _check_model(model, group, "install(wan_sp=True)")
-    sp = attention if attention is not None else default_attention(group, variant="wan")
-    for block in model.blocks:
-        block.self_attn.jenga_sp = sp
-    model.forward = types.MethodType(_i2v_forward_factory(group), model)
-    return sp
+    return _parallelize(model, group, attention, "install(wan_sp=True)", _i2v_forward_factory)
 
 
 def bind_wan_i2v(model) -> None:
@@ -416,7 +364,7 @@ def _is_jenga_model(model) -> bool:
     return getattr(model, "hilbert_order", None) is not None and getattr(model, "linear_to_hilbert", None) is not None
 
 
-def install_usp(xdit_module) -> bool:
+def install_usp(xdit_module) -> list[str]:
     """Swaps usp_dit_forward / usp_attn_forward of wan.distributed.xdit_context_parallel, which
     WanT2V(use_usp=True) binds to the model and to every self-attention module (text2video.py:88-99):
 
@@ -427,13 +375,15 @@ def install_usp(xdit_module) -> bool:
       usp_attn_forward  takes either WanSelfAttention.forward signature and defers to the patched class
                         forward under jenga_sp; a module without jenga_sp runs the reference function.
 
-    Returns False when there is nothing to swap or it is already swapped."""
+    Returns what it swapped: nothing when there is nothing to swap or it is already swapped."""
+    from .blocks import _swap
     orig_dit = getattr(xdit_module, "usp_dit_forward", None)
     orig_attn = getattr(xdit_module, "usp_attn_forward", None)
-    if orig_dit is None or orig_attn is None or getattr(orig_dit, "__jenga_b200__", False):
-        return False
+    if orig_attn is None:
+        return []
 
     def usp_dit_forward(self, x, t, context, seq_len, *args, **kwargs):
+        """jenga_b200: sharded TeaCache forward over the Ulysses exchange"""
         # the sharded forwards' signatures: (x, t, context, seq_len, clip_fea=None, y=None[, sa_drop_rate=0.0])
         # first call: parallelize_wan_i2v / parallelize_wan replaces this bound method by the sharded forward
         if getattr(self, "model_type", None) == "i2v":
@@ -445,6 +395,7 @@ def install_usp(xdit_module) -> bool:
         return self.forward(x, t, context, seq_len, *args, **kwargs)
 
     def usp_attn_forward(self, x, seq_lens, grid_sizes, freqs, *args, **kwargs):
+        """jenga_b200: the patched WanSelfAttention.forward under jenga_sp"""
         # WanSelfAttention.forward(x, seq_lens, grid_sizes, freqs, sa_drop_rate, per_block_tokens,
         # p_remain_rates, freq_remap, block_neighbor_list) of model_mul.py, or (x, seq_lens, grid_sizes,
         # freqs) of model.py, under jenga_sp
@@ -452,19 +403,6 @@ def install_usp(xdit_module) -> bool:
             return orig_attn(self, x, seq_lens, grid_sizes, freqs, *args, **kwargs)
         return type(self).forward(self, x, seq_lens, grid_sizes, freqs, *args, **kwargs)
 
-    for fn, orig in ((usp_dit_forward, orig_dit), (usp_attn_forward, orig_attn)):
-        fn.__jenga_b200__ = True
-        fn.__wrapped__ = orig
-    usp_dit_forward.__doc__ = "jenga_b200: sharded TeaCache forward over the Ulysses exchange"
-    usp_attn_forward.__doc__ = "jenga_b200: the patched WanSelfAttention.forward under jenga_sp"
-    xdit_module.usp_dit_forward = usp_dit_forward
-    xdit_module.usp_attn_forward = usp_attn_forward
-    return True
-
-
-def uninstall_usp(xdit_module) -> None:
-    """Puts the reference's usp_dit_forward / usp_attn_forward back"""
-    for name in ("usp_dit_forward", "usp_attn_forward"):
-        fn = getattr(xdit_module, name, None)
-        if getattr(fn, "__jenga_b200__", False):
-            setattr(xdit_module, name, fn.__wrapped__)
+    ok = (_swap(xdit_module, "usp_dit_forward", usp_dit_forward)
+          and _swap(xdit_module, "usp_attn_forward", usp_attn_forward))
+    return [f"{xdit_module.__name__}.usp_dit_forward", f"{xdit_module.__name__}.usp_attn_forward"] if ok else []

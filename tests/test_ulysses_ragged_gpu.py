@@ -376,7 +376,7 @@ def _nccl_worker(rank, world, port, ret):
     try:
         import bench
         from jenga_b200 import ulysses
-        from jenga_b200.hyi2v_sp import default_attention
+        from jenga_b200.sharding import default_attention
         ulysses.RAGGED_HEADS = True
         variant, T, valid, amp = VARIANTS["hy_amp"]
         dev = torch.device("cuda", rank)

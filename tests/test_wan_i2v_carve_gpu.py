@@ -229,7 +229,7 @@ def _section_module(c, H, jsp=None):
 @pytest.mark.parametrize("P", range(1, 9))
 def test_sharded_carved_section_equals_single_gpu(monkeypatch, P):
     from jenga_b200 import blocks, ulysses, wan_sp
-    from jenga_b200.hyi2v_sp import shard
+    from jenga_b200.sharding import shard
     from jenga_b200.wan import rope_freqs
     H = 40
     ragged = H % P != 0

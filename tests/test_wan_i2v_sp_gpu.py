@@ -89,7 +89,7 @@ def _single(H, c):
 
 def _sharded(H, P, G, c):
     from jenga_b200 import blocks
-    from jenga_b200.hyi2v_sp import shard
+    from jenga_b200.sharding import shard
     Cc = H * D
     n = -(-c["L"] // P)
     world = _World(P, n, H)
@@ -149,7 +149,7 @@ def _freqs(mod, dim, H):
 @pytest.mark.parametrize("P", [2, 4])
 def test_unmodified_i2v_blocks_under_sp_match_the_original_forward(emulated_groups, plain_wan, P):
     from jenga_b200 import blocks
-    from jenga_b200.hyi2v_sp import shard
+    from jenga_b200.sharding import shard
     f, h, w = GRIDS["ragged"]
     L, dim, H = f * h * w, 1536, 12
     blks = [plain_wan.WanAttentionBlock("i2v_cross_attn", dim, 8960, H, (-1, -1), True, True, 1e-6).cuda()

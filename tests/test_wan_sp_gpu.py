@@ -145,7 +145,7 @@ def _single(H, c, drop):
 def _sharded(H, P, G, c, drop):
     """every emulated rank's [1, n, H*D] result and its selections, in rank order"""
     from jenga_b200 import attention as A, blocks
-    from jenga_b200.hyi2v_sp import shard
+    from jenga_b200.sharding import shard
     n = -(-c["L"] // P)
     world = _World(P, n, H)
     got, cap = {}, _Capture()
@@ -239,7 +239,7 @@ def wan_module():
 def test_unmodified_block_under_sp_matches_single_gpu(emulated_groups, wan_module, P):
     from jenga_b200 import attention as A, blocks, gilbert
     from jenga_b200.attention import bits_to_onehot
-    from jenga_b200.hyi2v_sp import shard
+    from jenga_b200.sharding import shard
     f, h, w = GRIDS["ragged"]
     L, dim, H = f * h * w, 1536, 12
     blk = _make_blocks(wan_module, 1, dim=dim, H=H)[0]
