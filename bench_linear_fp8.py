@@ -11,6 +11,22 @@ These decide dense.FP8_ROUTED.  Then the 4 double + 8 single block stack (unmodi
 through install(), random-init bf16 weights) with the switch off and on with EVERY image-row Linear
 routed (what routing them would cost), alternately, the SM clock after each leg, and the difference of
 the two outputs.  Prints one JSON line with the card name, power limit and SM clock read in the same run.
+
+--model wan-14b / wan-1.3b: the Linears of one Wan2.1 WanAttentionBlock (wan/modules/model_mul.py), fp32
+nn.Linear weights as the Wan pipelines keep them, M = 75 600 (14B, 21x45x80) or 32 760 (1.3B, 21x30x52)
+rows.  Each site is timed as the chain the switch replaces, producer included:
+  self_qkv   wan_ln_modulate + q, k, v module calls   | wan_ln_modulate_fp8 + three FP8 GEMMs
+  self_o     o module call on the attention output    | quantize_rows_fp8 + FP8 GEMM      (also cross_o)
+  cross_q    wan_residual_ln (norm3) + q module call  | wan_residual_ln_fp8 + FP8 GEMM
+  ffn.0      wan_residual_ln (norm2) + module call    | wan_residual_ln_fp8 + FP8 GEMM
+  ffn.2      gelu_tanh + module call                  | gelu_tanh_fp8 + FP8 GEMM
+The module calls run under bf16 autocast, which re-casts the fp32 weight on every call.  Also per site:
+the module calls alone, the FP8 GEMMs alone, and torch._scaled_mm with row-wise scales on the same e4m3
+operands (a yardstick of what the card reaches, never on a hot path).  A (K, N) shape is "faster" when the
+sum of its sites' FP8 chains beats the sum of their bf16 chains; those are the ("fp32", K, N) entries of
+dense.FP8_ROUTED.  Then the block stack of bench_wan_blocks.py (4 Wan-14B or 8 Wan-1.3B T2V blocks) with
+the switch off and on with every Wan shape routed, alternately: times, peak memory, the output distance
+and the SM clock around each leg.
 """
 from __future__ import annotations
 
@@ -177,8 +193,198 @@ def stack_leg(n_double, n_single, rounds):
             "on_vs_off_mean_max_over_rms": [d.mean().item(), d.max().item()], "stats_per_forward_on": per_on}
 
 
+# Wan2.1 block shapes: grid, dim, heads, ffn, sa_drop_rate, p_remain_rates, blocks (bench_wan_blocks.MODELS)
+WAN = {"wan-14b": "14b", "wan-1.3b": "1.3b"}
+
+
+def wan_sites(C, F):
+    """site: (K, N, producer, GEMMs per call) of one WanAttentionBlock's routable Linears"""
+    return {"self_qkv": (C, C, "ln_modulate", 3), "self_o": (C, C, "quantize", 1),
+            "cross_q": (C, C, "residual_norm3", 1), "cross_o": (C, C, "quantize", 1),
+            "ffn.0": (C, F, "residual_norm2", 1), "ffn.2": (F, C, "gelu", 1)}
+
+
+def wan_routed(model):
+    """every ("fp32", K, N) shape of the Wan model's routable Linears"""
+    from bench_wan_blocks import MODELS
+    _, C, _, F, *_ = MODELS[WAN[model]]
+    return frozenset(("fp32", k_, n_) for k_, n_, _, _ in wan_sites(C, F).values())
+
+
+def scaled_mm(x8, a_scale, w8, w_scale, b):
+    # row-wise _scaled_mm takes a bf16 bias only
+    return torch._scaled_mm(x8, w8.t(), scale_a=a_scale[:, None], scale_b=w_scale[None, :],
+                            bias=b.to(torch.bfloat16), out_dtype=torch.bfloat16)
+
+
+def wan_gemm_leg(model, windows, iters):
+    from bench_wan_blocks import MODELS
+    from jenga_b200 import dense as DN
+    (f, h, w_), C, _, F, *_ = MODELS[WAN[model]]
+    M = f * h * w_
+    dev = torch.device("cuda")
+    g = torch.Generator(device=dev).manual_seed(11)
+    e = 0.1 * torch.randn(6, C, generator=g, device=dev)
+    xr = torch.randn(1, M, C, generator=g, device=dev)                    # fp32 residual stream
+    y = torch.randn(1, M, C, generator=g, device=dev).bfloat16()          # attention / cross output
+    nw, nb = torch.ones(C, device=dev), torch.zeros(C, device=dev)        # norm3 (affine)
+    out, sites = {}, {}
+    for site, (K, N, prod, n) in wan_sites(C, F).items():
+        lin = torch.nn.Linear(K, N, device=dev)                           # fp32, as the Wan pipelines keep it
+        lin.requires_grad_(False)
+        with torch.no_grad():
+            lin.weight.normal_(0.0, 0.02, generator=g)
+            lin.bias.normal_(0.0, 0.02, generator=g)
+        w8, ws, b = DN.fp8_weight(lin)
+        a_in = torch.randn(1, M, K, generator=g, device=dev).bfloat16() if prod == "gelu" else None
+        if prod == "ln_modulate":
+            p16 = lambda: DN.wan_ln_modulate(xr, e[0], e[1])                                    # noqa: E731
+            p8 = lambda: DN.wan_ln_modulate_fp8(xr, e[0], e[1])                                 # noqa: E731
+        elif prod == "quantize":
+            p16 = lambda: y                                                                     # noqa: E731
+            p8 = lambda: DN.quantize_rows_fp8(y)                                                # noqa: E731
+        elif prod == "residual_norm3":
+            p16 = lambda: DN.wan_residual_ln(xr, y, e[2], weight=nw, bias=nb)[1]                # noqa: E731
+            p8 = lambda: DN.wan_residual_ln_fp8(xr, y, e[2], weight=nw, bias=nb)[1]             # noqa: E731
+        elif prod == "residual_norm2":
+            p16 = lambda: DN.wan_residual_ln(xr, y, None, shift=e[3], scale=e[4])[1]            # noqa: E731
+            p8 = lambda: DN.wan_residual_ln_fp8(xr, y, None, shift=e[3], scale=e[4])[1]         # noqa: E731
+        else:
+            p16 = lambda: DN.gelu_tanh_into(a_in, torch.empty_like(a_in))                       # noqa: E731
+            p8 = lambda: DN.gelu_tanh_fp8(a_in)                                                 # noqa: E731
+        h16, h8 = p16(), p8()
+
+        def bf16_chain():
+            hh = p16()
+            return [lin(hh) for _ in range(n)]
+
+        def fp8_chain():
+            hh = p8()
+            return [DN.linear_fp8(*hh, w8, ws, b) for _ in range(n)]
+
+        legs = {"bf16_chain": bf16_chain, "fp8_chain": fp8_chain,
+                "bf16_module_only": lambda: [lin(h16) for _ in range(n)],
+                "fp8_gemm_only": lambda: [DN.linear_fp8(*h8, w8, ws, b) for _ in range(n)]}
+        try:
+            scaled_mm(*h8, w8, ws, b)
+            legs["scaled_mm_yardstick"] = lambda: [scaled_mm(*h8, w8, ws, b) for _ in range(n)]
+            mm_err = None
+        except Exception as ex:  # noqa: BLE001
+            mm_err = f"{type(ex).__name__}: {ex}"[:200]
+        with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
+            for fn in legs.values():
+                fn()
+            t = {k: [] for k in legs}
+            for _ in range(windows):
+                for k, fn in legs.items():
+                    t[k].append(timed(fn, iters))
+            ref = lin(h16).float()
+            got = DN.linear_fp8(*h8, w8, ws, b).float()
+        err = (got - ref).abs() / ref.pow(2).mean().sqrt()
+        flop = 2.0 * M * K * N * n
+        best = {k: min(v) for k, v in t.items()}
+        sites[site] = {"M": M, "K": K, "N": N, "gemms": n, "seconds_best": best,
+                       "tflops": {k: flop / v / 1e12 for k, v in best.items() if "only" in k or "scaled" in k},
+                       "speedup_chain": best["bf16_chain"] / best["fp8_chain"],
+                       "scaled_mm_error": mm_err,
+                       "fp8_vs_bf16_mean_max_over_rms": [err.mean().item(), err.max().item()]}
+        del lin, w8, a_in, h16, h8, ref, got
+        torch.cuda.empty_cache()
+    shapes = {}
+    for site, r in sites.items():
+        s_ = shapes.setdefault(f"{r['K']}x{r['N']}", {"sites": [], "bf16_chain": 0.0, "fp8_chain": 0.0})
+        s_["sites"].append(site)
+        s_["bf16_chain"] += r["seconds_best"]["bf16_chain"]
+        s_["fp8_chain"] += r["seconds_best"]["fp8_chain"]
+    for s_ in shapes.values():
+        s_["faster"] = s_["fp8_chain"] < s_["bf16_chain"]
+    out["sites"], out["shapes"] = sites, shapes
+    return out
+
+
+def wan_stack_leg(model, rounds):
+    from oracle import ref_loader
+    from bench_wan_blocks import MODELS
+    from jenga_b200 import blocks as jb, dense as DN, gilbert
+    if not ref_loader.available():
+        return {"unavailable": "oracle/_ref/ not staged"}
+    our = ref_loader.load_blocks(product=True)[1]
+    (f, h, w_), dim, heads, ffn, drop, p_remain, n_blocks = MODELS[WAN[model]]
+    dev = torch.device("cuda")
+    g = torch.Generator(device=dev).manual_seed(2024)
+    with torch.device(dev):
+        blks = [our.WanAttentionBlock("t2v_cross_attn", dim, ffn, heads, (-1, -1), True, True, 1e-6)
+                for _ in range(n_blocks)]
+    with torch.no_grad():
+        for m in blks:
+            m.requires_grad_(False)
+            for n_, p_ in m.named_parameters():
+                if "norm" in n_ and n_.endswith("weight"):
+                    p_.fill_(1.0)
+                else:
+                    p_.copy_(torch.randn(p_.shape, generator=g, device=dev).mul_(0.02))
+    L = f * h * w_
+    _, h2l = gilbert.mapping_tensors(f, h, w_, sliced=True)
+    nbr = gilbert.block_neighbor_mapping(f, h, w_, sliced=True)
+    d = dim // heads
+    freqs = torch.cat([our.rope_params(1024, d - 4 * (d // 6)), our.rope_params(1024, 2 * (d // 6)),
+                       our.rope_params(1024, 2 * (d // 6))], dim=1).to(dev)
+    seq_lens = torch.tensor([L], dtype=torch.long)
+    grid = torch.tensor([[f, h, w_]], dtype=torch.long)
+    x0 = torch.randn(1, L, dim, generator=g, device=dev).bfloat16()
+    e0 = 0.1 * torch.randn(1, 6, dim, generator=g, device=dev)
+    ctx = torch.randn(1, 512, dim, generator=g, device=dev).bfloat16()
+    kw = dict(sa_drop_rate=drop, freq_remap=h2l.to(dev), block_neighbor_list=nbr, p_remain_rates=p_remain)
+    every = wan_routed(model)
+    saved = DN.LINEAR_FP8, DN.FP8_ROUTED
+    jb.remove_gather_hook()
+
+    def forward(on):
+        DN.LINEAR_FP8, DN.FP8_ROUTED = on, every if on else frozenset()
+        x = x0
+        for blk in blks:
+            x = blk(x, e0, seq_lens, grid, freqs, ctx, None, **kw)
+        return x
+
+    res, clocks, peak = {"off": [], "on": []}, {"off": [], "on": []}, {}
+    try:
+        with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
+            for leg in ("off", "on"):                 # warm-up; the first "on" quantises and caches the weights
+                torch.cuda.synchronize()
+                torch.cuda.reset_peak_memory_stats()
+                base = torch.cuda.memory_allocated()
+                out_ = forward(leg == "on")
+                torch.cuda.synchronize()
+                peak[leg] = {"peak_gb": torch.cuda.max_memory_allocated() / 1e9,
+                             "above_start_gb": (torch.cuda.max_memory_allocated() - base) / 1e9}
+                if leg == "off":
+                    out_off = out_
+                else:
+                    out_on = out_
+            peak["e4m3_weight_cache_gb"] = sum(
+                m.__dict__["_jenga_fp8"][1].numel() for b_ in blks for m in b_.modules()
+                if "_jenga_fp8" in m.__dict__) / 1e9
+            s0 = dict(jb.STATS)
+            forward(True)
+            per_on = {k: jb.STATS[k] - s0[k] for k in s0 if jb.STATS[k] != s0[k]}
+            for r in range(rounds):
+                for leg in (("off", "on") if r % 2 == 0 else ("on", "off")):
+                    c0 = sm_clock()
+                    res[leg].append(timed(lambda: forward(leg == "on"), 1))
+                    clocks[leg].append([c0, sm_clock()])
+    finally:
+        DN.LINEAR_FP8, DN.FP8_ROUTED = saved
+    rms = out_off.float().pow(2).mean().sqrt()
+    dd = (out_on.float() - out_off.float()).abs() / rms
+    return {"blocks": n_blocks, "tokens": L, "routed": sorted(every), "seconds": res,
+            "sm_clock_before_after_leg_mhz": clocks, "memory": peak,
+            "best": {k: min(v) for k, v in res.items()}, "speedup": min(res["off"]) / min(res["on"]),
+            "on_vs_off_mean_max_over_rms": [dd.mean().item(), dd.max().item()], "stats_per_forward_on": per_on}
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--model", choices=["hy", *WAN], default="hy")
     ap.add_argument("--windows", type=int, default=5)
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--blocks", default="4,8")
@@ -188,10 +394,16 @@ def main(argv=None):
     if not torch.cuda.is_available():
         raise SystemExit("bench_linear_fp8.py measures on a GPU; none is visible")
     line = {"card_start": card()}
-    line["gemm"] = gemm_leg(a.windows, a.iters)
-    if not a.skip_stack:
-        nd, ns = (int(v) for v in a.blocks.split(","))
-        line["stack"] = stack_leg(nd, ns, a.rounds)
+    if a.model == "hy":
+        line["gemm"] = gemm_leg(a.windows, a.iters)
+        if not a.skip_stack:
+            nd, ns = (int(v) for v in a.blocks.split(","))
+            line["stack"] = stack_leg(nd, ns, a.rounds)
+    else:
+        line["model"] = a.model
+        line["gemm"] = wan_gemm_leg(a.model, a.windows, a.iters)
+        if not a.skip_stack:
+            line["stack"] = wan_stack_leg(a.model, a.rounds)
     line["card_end"] = card()
     print(json.dumps(line))
 

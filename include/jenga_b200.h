@@ -451,7 +451,17 @@ int jenga_linear_fp8(const JengaLinearFp8Args* args, void* stream);
  *                                 form ATen's layer_norm kernel computes        (gate 1 + norm3, :334-339)
  *                    affine == 0: out = bf16( LN(r) * (1 + vec_a) + vec_b )  scale / shift
  *                                                                   (cross residual + norm2, :339-340)
- * wan_gate_residual: out = x + y * gate, fp32                                    (gate 2, :341-342) */
+ * wan_gate_residual: out = x + y * gate, fp32                                    (gate 2, :341-342)
+ * The _fp8 forms feed the opt-in FP8 Linears (jenga_linear_fp8): each is the bf16 form followed by
+ * jenga_quantize_rows_fp8 of its bf16 rows, in one pass and bit-identical to the two calls; the bf16
+ * rows are never written.  out8 e4m3 rows `out_stride` BYTES apart (multiple of 16), a_scale [rows]
+ * f32, channels % 16 == 0 (JENGA_E_UNSUPPORTED otherwise); `res` of wan_residual_ln_fp8 is written as
+ * by wan_residual_ln.
+ * wan_ln_modulate_fp8:   norm1 + modulate, the one input of the self-attention q / k / v
+ * wan_residual_ln_fp8:   gate 1 + norm3 (affine, the cross-attention q) or cross residual + norm2 +
+ *                        modulate (ffn.0)
+ * gelu_tanh_fp8:         jenga_gelu_tanh of bf16 rows (ffn.0's output), quantised (the ffn.2 input);
+ *                        x_stride in elements (multiple of 8), channels <= 16384 */
 int jenga_wan_ln_modulate(const void* x, int32_t x_dtype, int64_t x_stride, const float* scale, const float* shift,
                           void* out, int64_t out_stride, int64_t rows, int32_t channels, float eps, void* stream);
 int jenga_wan_residual_ln(const void* x, int32_t x_dtype, int64_t x_stride, const void* y, int64_t y_stride,
@@ -461,6 +471,15 @@ int jenga_wan_residual_ln(const void* x, int32_t x_dtype, int64_t x_stride, cons
 int jenga_wan_gate_residual(const void* x, int32_t x_dtype, int64_t x_stride, const void* y, int64_t y_stride,
                             const float* gate, float* out, int64_t out_stride, int64_t rows, int32_t channels,
                             void* stream);
+int jenga_wan_ln_modulate_fp8(const void* x, int32_t x_dtype, int64_t x_stride, const float* scale,
+                              const float* shift, void* out8, int64_t out_stride, float* a_scale, int64_t rows,
+                              int32_t channels, float eps, void* stream);
+int jenga_wan_residual_ln_fp8(const void* x, int32_t x_dtype, int64_t x_stride, const void* y, int64_t y_stride,
+                              const float* gate, float* res, int64_t res_stride, const float* vec_a,
+                              const float* vec_b, int32_t affine, void* out8, int64_t out_stride, float* a_scale,
+                              int64_t rows, int32_t channels, float eps, void* stream);
+int jenga_gelu_tanh_fp8(const void* x, int64_t x_stride, void* out8, int64_t out_stride, float* a_scale,
+                        int64_t rows, int32_t channels, void* stream);
 
 /* Wan2.1-I2V cross-attention in one launch (wan/modules/model_mul.py:223-249 WanI2VCrossAttention.forward,
  * the part between the norms and self.o, under bf16 autocast):

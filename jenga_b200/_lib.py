@@ -259,6 +259,16 @@ def _load() -> C.CDLL:
     lib.jenga_ln_modulate_tr_fp8.restype = C.c_int
     lib.jenga_linear_fp8.argtypes = [C.POINTER(JengaLinearFp8Args), C.c_void_p]
     lib.jenga_linear_fp8.restype = C.c_int
+    lib.jenga_wan_ln_modulate_fp8.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_void_p]
+    lib.jenga_wan_ln_modulate_fp8.restype = C.c_int
+    lib.jenga_wan_residual_ln_fp8.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                              C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_void_p]
+    lib.jenga_wan_residual_ln_fp8.restype = C.c_int
+    lib.jenga_gelu_tanh_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                        C.c_int32, C.c_void_p]
+    lib.jenga_gelu_tanh_fp8.restype = C.c_int
     lib.jenga_gilbert_xyz2d.argtypes = [C.c_int] * 6
     lib.jenga_gilbert_xyz2d.restype = C.c_int64
     if lib.jenga_abi_version() != 3:

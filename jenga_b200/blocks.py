@@ -147,17 +147,27 @@ def _gate_res(mod, x, y, gate, tr=None):
     return x + mod.apply_gate(y, gate=gate, condition_type="token_replace", tr_gate=tr[0], first_frame_mask=tr[1])
 
 
+def _fp8_routed(layer, k: int):
+    """DN.fp8_weight(layer) when the opt-in FP8 Linears (DN.LINEAR_FP8) route `layer` on inputs of k
+    channels — its K, and a shape in DN.FP8_ROUTED — else None"""
+    if not (DN.LINEAR_FP8 and DN.FP8_ROUTED and isinstance(layer, torch.nn.Module)):
+        return None
+    # the table is consulted before fp8_weight, which quantises and caches: a layer the table does not
+    # route never carries an e4m3 copy
+    w = getattr(layer, "weight", None)
+    if (not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[1] != k
+            or (DN.fp8_weight_kind(layer), k, w.shape[0]) not in DN.FP8_ROUTED):
+        return None
+    return DN.fp8_weight(layer)
+
+
 def _fp8_weight(layer, x):
-    """DN.fp8_weight(layer) when the opt-in FP8 Linears (DN.LINEAR_FP8) take `layer` on input x — a
-    bf16 CUDA tensor with 16-byte aligned rows of the layer's K, and a shape in DN.FP8_ROUTED — else None"""
+    """_fp8_routed(layer, K) on input x — a bf16 CUDA tensor with 16-byte aligned rows — else None"""
     if not (DN.LINEAR_FP8 and DN.FP8_ROUTED and isinstance(x, torch.Tensor) and x.is_cuda
             and x.dtype == torch.bfloat16 and x.dim() >= 2 and x.stride(-1) == 1 and x.stride(-2) % 8 == 0
-            and x.data_ptr() % 16 == 0 and isinstance(layer, torch.nn.Module)):
+            and x.data_ptr() % 16 == 0):
         return None
-    w = DN.fp8_weight(layer)
-    if w is None or w[0].shape[1] != x.shape[-1]:
-        return None
-    return w if (DN.fp8_weight_kind(layer), *w[0].shape[::-1]) in DN.FP8_ROUTED else None
+    return _fp8_routed(layer, x.shape[-1])
 
 
 def _linear(layer, x, x8=None):
@@ -171,8 +181,15 @@ def _linear(layer, x, x8=None):
             x8 = DN.quantize_rows_fp8(x)
         except ValueError:                   # rows that are not uniformly strided
             return layer(x)
+    return _linear8(layer, x8, x.shape[:-1])
+
+
+def _linear8(layer, x8, lead):
+    """one jenga_linear_fp8 launch of `layer` on the e4m3 rows x8 = (codes, a_scale) a producer made; the
+    caller has checked _fp8_routed.  -> bf16 [*lead, N]"""
+    w = DN.fp8_weight(layer)
     STATS["linear_fp8"] += 1
-    return DN.linear_fp8(*x8, *w).view(*x.shape[:-1], w[0].shape[0])
+    return DN.linear_fp8(*x8, *w).view(*lead, w[0].shape[0])
 
 
 def _mod_linear(mod, layer, norm, x, shift, scale, tr=None):
@@ -192,6 +209,41 @@ def _plain_mlp(mlp) -> bool:
             and "forward" not in mlp.__dict__ and not mlp._forward_hooks and not mlp._forward_pre_hooks
             and isinstance(act, torch.nn.GELU) and act.approximate == "tanh" and isinstance(norm, torch.nn.Identity)
             and all(isinstance(d, torch.nn.Dropout) and d.p == 0.0 for d in (d1, d2)))
+
+
+def _plain_ffn(ffn) -> bool:
+    """Wan's FFN as WanAttentionBlock builds it (model_mul.py:282-284): exactly
+    Sequential(Linear, GELU(approximate="tanh"), Linear), with no hooks and no forward override"""
+    if type(ffn) is not torch.nn.Sequential or len(ffn) != 3:
+        return False
+    f0, act, f2 = ffn
+    return (type(f0) is torch.nn.Linear and type(f2) is torch.nn.Linear and type(act) is torch.nn.GELU
+            and act.approximate == "tanh"
+            and all("forward" not in m.__dict__ and not m._forward_hooks and not m._forward_pre_hooks
+                    for m in (ffn, f0, act, f2)))
+
+
+def _wan_ffn(blk, x, cross, e):
+    """(r, ffn(norm2(r) * (1 + e[4]) + e[3])) with r = x + cross, the fp32 residual (model_mul.py:339-341).
+    With the FP8 Linears on, a plain FFN is opened into ffn.0 -> GELU -> ffn.2: each routed Linear takes
+    the e4m3 rows of its input from the pass that makes that input (wan_residual_ln_fp8, gelu_tanh_fp8)."""
+    norm = dict(eps=blk.norm2.eps, shift=e[3], scale=e[4])
+    if not (DN.LINEAR_FP8 and DN.FP8_ROUTED and _plain_ffn(blk.ffn)):
+        x, h = DN.wan_residual_ln(x, cross, None, **norm)
+        return x, blk.ffn(h)
+    f0, act, f2 = blk.ffn
+    lead = x.shape[:-1]
+    if _fp8_rows((f0,), x):
+        x, h8 = DN.wan_residual_ln_fp8(x, cross, None, **norm)
+        a = _linear8(f0, h8, lead)
+    else:
+        x, h = DN.wan_residual_ln(x, cross, None, **norm)
+        a = _linear(f0, h)
+    F = a.shape[-1]
+    if (a.dtype == torch.bfloat16 and a.is_contiguous() and F % 16 == 0 and F <= 16384
+            and _fp8_routed(f2, F) is not None):
+        return x, _linear8(f2, DN.gelu_tanh_fp8(a), lead)
+    return x, _linear(f2, act(a))
 
 
 def _mlp(mod, mlp, norm, x, shift, scale, tr=None):
@@ -418,7 +470,7 @@ def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=Non
 # Wan blocks
 # ------------------------------------------------------------------------------------------------
 def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates, freq_remap,
-                    block_neighbor_list, stats=("wan_self_sp", "wan_self_dense_sp")):
+                    block_neighbor_list, stats=("wan_self_sp", "wan_self_dense_sp"), x8=None):
     """WanSelfAttention.forward with the fused norm + RoPE prologue and no fall-back.
     jsp set: x is a rank's n rows of a sharded Wan forward (wan_sp.py); the prologue runs on them, then
     the Ulysses exchange and the operator over the first L (the global token count) exchanged rows.
@@ -426,13 +478,13 @@ def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tok
     top_k and first_frame_blocks follow the single-GPU rule over L (model_mul.py:161-164); sa_drop_rate
     <= 0.25 (:153, the warm-up steps) runs the dense class, the flash_attn shim's launch.  freq_remap:
     the RoPE row of each row (None: raster, one GPU only).  stats: the STATS keys of a carved and of a
-    dense call."""
+    dense call.  x8: see _wan_qkv."""
     b, n = x.shape[:2]
     if not _wan_self_fused_ok(self, x, per_block_tokens) or (jsp is not None and freq_remap is None):
         raise RuntimeError(f"{type(self).__name__}: the call is not one the fused Wan self-attention takes (a "
                            "CUDA batch-1 input, head_dim 128, 128-token blocks, WanRMSNorm q / k norms with "
                            "weights and, under jenga_sp, a freq_remap); this route has no fall-back")
-    q_lin, k_lin = self.q(x), self.k(x)
+    q_lin, k_lin, v = _wan_qkv(self, x, x8)
     if q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype != q_lin.dtype:
         raise RuntimeError(f"{type(self).__name__}: q / k Linears return {q_lin.dtype}, the prologue takes bf16 "
                            "or fp32")
@@ -441,7 +493,7 @@ def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tok
     eps = float(self.norm_q.eps)
     wq, wk = self.norm_q.weight, self.norm_k.weight
     # the bf16 v both single-GPU routes attend: flash_attention's half() and the operator's cast
-    v = self.v(x).view(b, n, self.num_heads, self.head_dim).to(torch.bfloat16).contiguous()
+    v = v.view(b, n, self.num_heads, self.head_dim).to(torch.bfloat16).contiguous()
     dense = sa_drop_rate <= 0.25
     if jsp is None and not dense:
         out = WAN.self_attention(q_lin, k_lin, v, wq, wk, self.num_heads, grid, freqs, sa_drop_rate,
@@ -460,7 +512,15 @@ def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tok
     out = out.flatten(2)
     if not torch.is_autocast_enabled():
         out = out.float()       # the query dtype the reference returns, as in _wan_self
-    return self.o(out)
+    return _linear(self.o, out)
+
+
+def _wan_qkv(self, x, x8):
+    """self.q(x), self.k(x), self.v(x); or, with x8 = (codes, a_scale) — the block's wan_ln_modulate_fp8
+    rows, passed as `jenga_x8` with x their [1, n, C] e4m3 view — three FP8 GEMMs on the one input"""
+    if x8 is None:
+        return self.q(x), self.k(x), self.v(x)
+    return tuple(_linear8(lin, x8, x.shape[:-1]) for lin in (self.q, self.k, self.v))
 
 
 def _wan_self_fused_ok(self, x, per_block_tokens=128):
@@ -473,7 +533,7 @@ def _wan_self_fused_ok(self, x, per_block_tokens=128):
 
 
 def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=None, freq_remap=None, block_neighbor_list=None,
-                  p_remain_rates=0.8):
+                  p_remain_rates=0.8, *, jenga_x8=None):
     """WanSelfAttention.forward of wan/modules/model.py (:127-156).  Called in that module's signature
     (sa_drop_rate None):
       under `jenga_sp` (the raster-sharded I2V forward, wan_sp.parallelize_wan_i2v) x holds rank r's n
@@ -483,7 +543,8 @@ def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=None, freq_
       without jenga_sp: the original forward.
     With the Jenga arguments of model_mul.py (the I2V forwards of wan_sp.py): _wan_self_fused, on one GPU
     or under jenga_sp.  A call it does not take runs the original forward on raster rows (freq_remap None)
-    and raises on curve-ordered rows, whose RoPE positions the original forward does not know."""
+    and raises on curve-ordered rows, whose RoPE positions the original forward does not know.
+    jenga_x8: the block's e4m3 q / k / v input (_wan_qkv), passed only when _wan_i2v_self_fuses says so."""
     jsp = getattr(self, "jenga_sp", None)
     if sa_drop_rate is None:
         if jsp is None:
@@ -494,31 +555,37 @@ def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=None, freq_
         rows = torch.arange(r * n, (r + 1) * n, device=x.device)
         remap = torch.where(rows < L, rows, torch.zeros_like(rows))
         return _wan_self_fused(self, jsp, x, grid_sizes, freqs, 0.0, 128, 0.0, remap, None,
-                               stats=(None, "wan_i2v_self_sp"))
-    if jsp is None and freq_remap is None and not _wan_self_fused_ok(self, x):
+                               stats=(None, "wan_i2v_self_sp"), x8=jenga_x8)
+    if not _wan_i2v_self_fuses(self, x, sa_drop_rate, freq_remap):
         STATS["fallback"] += 1
         return type(self).forward.__wrapped__(self, x, seq_lens, grid_sizes, freqs)
     stats = ("wan_i2v_self_carved_sp", "wan_i2v_self_sp") if jsp is not None else ("wan_i2v_self", "wan_i2v_self_dense")
     return _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, 128, p_remain_rates, freq_remap,
-                           block_neighbor_list, stats=stats)
+                           block_neighbor_list, stats=stats, x8=jenga_x8)
+
+
+def _wan_i2v_self_fuses(self, x, sa_drop_rate=None, freq_remap=None, **_):
+    """True when _wan_i2v_self runs _wan_self_fused (or raises) rather than the original forward"""
+    if getattr(self, "jenga_sp", None) is not None:
+        return True
+    return sa_drop_rate is not None and (freq_remap is not None or _wan_self_fused_ok(self, x))
 
 
 def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128, p_remain_rates=0.8,
-              freq_remap=None, block_neighbor_list=None):
+              freq_remap=None, block_neighbor_list=None, *, jenga_x8=None):
+    """jenga_x8: the block's e4m3 q / k / v input (_wan_qkv), passed only when _wan_self_fuses says so"""
     jsp = getattr(self, "jenga_sp", None)
     if jsp is not None:
         return _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
-                               freq_remap, block_neighbor_list)
-    b, s = x.shape[:2]
-    wq = getattr(self.norm_q, "weight", None)
-    wk = getattr(self.norm_k, "weight", None)
-    if (sa_drop_rate <= 0.25 or not x.is_cuda or b != 1 or self.head_dim != 128 or per_block_tokens != 128
-            or wq is None or wk is None or type(self.norm_q).__name__ != "WanRMSNorm"):
+                               freq_remap, block_neighbor_list, x8=jenga_x8)
+    if not _wan_self_fuses(self, x, sa_drop_rate, per_block_tokens):
         return None
-    q_lin, k_lin = self.q(x), self.k(x)
+    b, s = x.shape[:2]
+    wq, wk = self.norm_q.weight, self.norm_k.weight
+    q_lin, k_lin, v = _wan_qkv(self, x, jenga_x8)
     if q_lin.dtype not in (torch.bfloat16, torch.float32):
         return None
-    v = self.v(x).view(b, s, self.num_heads, self.head_dim)
+    v = v.view(b, s, self.num_heads, self.head_dim)
     grid = [int(g) for g in grid_sizes[0].tolist()]
     out = WAN.self_attention(q_lin, k_lin, v, wq, wk, self.num_heads, grid, freqs, sa_drop_rate,
                              p_remain_rates=p_remain_rates, freq_remap=freq_remap,
@@ -529,27 +596,46 @@ def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_
         # the reference returns the query dtype, fp32 (rope_apply -> .float(), model_mul.py:71;
         # operator :530-532); under autocast the following Linear casts back to bf16 anyway
         out = out.float()
-    return self.o(out)
+    return _linear(self.o, out)
 
 
-def _wan_cross(self, x, context, context_lens):
-    wq = getattr(self.norm_q, "weight", None)
-    wk = getattr(self.norm_k, "weight", None)
+def _wan_self_fuses(self, x, sa_drop_rate=0.0, per_block_tokens=128, **_):
+    """True when _wan_self runs a fused route (jenga_sp, or the carved call on one GPU) rather than
+    returning None for the original forward; the Linears' output dtype aside"""
+    if getattr(self, "jenga_sp", None) is not None:
+        return True
+    return (sa_drop_rate > 0.25 and x.is_cuda and x.shape[0] == 1 and self.head_dim == 128
+            and per_block_tokens == 128 and getattr(self.norm_q, "weight", None) is not None
+            and getattr(self.norm_k, "weight", None) is not None and type(self.norm_q).__name__ == "WanRMSNorm")
+
+
+def _wan_cross_fuses(self, x, context, context_lens):
+    """True when _wan_cross runs the fused T2V cross-attention (the Linears' output dtypes aside)"""
     # context_lens: the reference's varlen form (wan/modules/attention.py:69-80); teacache_forward
     # passes None (jenga_wan.py:569)
-    if (context_lens is not None or not x.is_cuda or x.dim() != 3 or x.shape[0] != 1 or context.dim() != 3
-            or context.shape[0] != 1 or self.head_dim != 128 or wq is None or wk is None
-            or type(self.norm_q).__name__ != "WanRMSNorm" or type(self.norm_k).__name__ != "WanRMSNorm"
-            or not DN._autocast_bf16()):
+    return (context_lens is None and x.is_cuda and x.dim() == 3 and x.shape[0] == 1 and context.dim() == 3
+            and context.shape[0] == 1 and self.head_dim == 128 and getattr(self.norm_q, "weight", None) is not None
+            and getattr(self.norm_k, "weight", None) is not None and type(self.norm_q).__name__ == "WanRMSNorm"
+            and type(self.norm_k).__name__ == "WanRMSNorm" and DN._autocast_bf16())
+
+
+def _wan_cross(self, x, context, context_lens, *, jenga_x8=None):
+    """jenga_x8: the block's wan_residual_ln_fp8 rows of x (x their e4m3 view) for the q Linear, passed only
+    when _wan_cross_fuses says so"""
+    if not _wan_cross_fuses(self, x, context, context_lens):
         return None
-    q_lin, k_lin, v = self.q(x), self.k(context), self.v(context)
+    q_lin = self.q(x) if jenga_x8 is None else _linear8(self.q, jenga_x8, x.shape[:-1])
+    k_lin, v = self.k(context), self.v(context)
     if (q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype not in (torch.bfloat16, torch.float32)
             or v.dtype != torch.bfloat16):
+        if jenga_x8 is not None:
+            raise RuntimeError(f"{type(self).__name__}: k / v Linears return {k_lin.dtype} / {v.dtype} under bf16 "
+                               "autocast; the e4m3 q input has no fall-back")
         return None
-    out = WAN.cross_attention(q_lin, k_lin, v.view(1, -1, self.num_heads, self.head_dim), wq, wk,
-                              self.num_heads, eps=float(self.norm_q.eps))
+    out = WAN.cross_attention(q_lin, k_lin, v.view(1, -1, self.num_heads, self.head_dim),
+                              self.norm_q.weight, self.norm_k.weight, self.num_heads, eps=float(self.norm_q.eps))
     STATS["wan_cross"] += 1
-    return self.o(out.flatten(2))
+    return _linear(self.o, out.flatten(2))
 
 
 def _wan_i2v_cross_shape_ok(ca, x, context, context_lens):
@@ -571,13 +657,16 @@ def wan_i2v_cross_eligible(ca, x, context, context_lens):
     return _wan_i2v_cross_shape_ok(ca, x, context, context_lens) and x.is_cuda and DN._autocast_bf16()
 
 
-def _wan_i2v_cross(ca, x, context, context_lens, stat="wan_i2v_cross"):
+def _wan_i2v_cross(ca, x, context, context_lens, stat="wan_i2v_cross", x8=None):
     """WanI2VCrossAttention.forward (model_mul.py:223-249) with its attention part as one
     jenga_wan_i2v_cross_attn launch; the module's own q / k / v / k_img / v_img / o Linears run around
-    it.  Anything else runs the module's own forward."""
+    it (q and o through _linear: the k / v / k_img / v_img Linears over the context rows are never
+    FP8).  Anything else runs the module's own forward.  x8: the block's wan_residual_ln_fp8 rows of x
+    (x their e4m3 view) for q, passed only when wan_i2v_cross_eligible."""
     if wan_i2v_cross_eligible(ca, x, context, context_lens):
         ctx_img, ctx = context[:, :_WAN_I2V_IMG_TOKENS], context[:, _WAN_I2V_IMG_TOKENS:]   # :230-231
-        q_lin, k_lin, v = ca.q(x), ca.k(ctx), ca.v(ctx)
+        q_lin = ca.q(x) if x8 is None else _linear8(ca.q, x8, x.shape[:-1])
+        k_lin, v = ca.k(ctx), ca.v(ctx)
         kimg_lin, vimg = ca.k_img(ctx_img), ca.v_img(ctx_img)
         lin_ok = all(t.dtype in (torch.bfloat16, torch.float32) for t in (q_lin, k_lin, kimg_lin))
         if lin_ok and v.dtype == vimg.dtype == torch.bfloat16:
@@ -586,7 +675,10 @@ def _wan_i2v_cross(ca, x, context, context_lens, stat="wan_i2v_cross"):
                                           ca.norm_q.weight, ca.norm_k.weight, ca.norm_k_img.weight, n,
                                           eps=float(ca.norm_q.eps))
             STATS[stat] += 1
-            return ca.o(out.flatten(2))
+            return _linear(ca.o, out.flatten(2))
+        if x8 is not None:
+            raise RuntimeError(f"{type(ca).__name__}: context Linears return {k_lin.dtype} / {v.dtype} under bf16 "
+                               "autocast; the e4m3 q input has no fall-back")
     STATS["fallback"] += 1
     return ca(x, context, context_lens)
 
@@ -652,18 +744,49 @@ def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_le
     if not ok:
         return None                     # no autocast, batch > 1, cross_attn_norm=False (norm3 is Identity), …
     e = e6.chunk(6, dim=1)
-    # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to
-    y = self.self_attn(DN.wan_ln_modulate(x, e[0], e[1], eps=self.norm1.eps), seq_lens, grid_sizes, freqs,
-                       **attn_kw)                                              # :331-333
-    x, h = DN.wan_residual_ln(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight,
-                              bias=self.norm3.bias)                            # :334-335, :339
+    # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to; with the
+    # FP8 Linears routing q / k / v, on the e4m3 rows of that bf16 instead (:331-333)
+    sa, ca = self.self_attn, self.cross_attn
+    if _fp8_rows((sa.q, sa.k, sa.v), x) and _fused_forward(
+            sa, ((_wan_self, _wan_self_fuses), (_wan_i2v_self, _wan_i2v_self_fuses)), x, **attn_kw):
+        x8 = DN.wan_ln_modulate_fp8(x, e[0], e[1], eps=self.norm1.eps)
+        y = sa(x8[0].view(x.shape), seq_lens, grid_sizes, freqs, jenga_x8=x8, **attn_kw)
+    else:
+        y = sa(DN.wan_ln_modulate(x, e[0], e[1], eps=self.norm1.eps), seq_lens, grid_sizes, freqs, **attn_kw)
+    # gate 1 + norm3 (:334-335, :339), e4m3 when the cross-attention's q is routed
+    x8 = None
+    if _fp8_rows((ca.q,), x) and (wan_i2v_cross_eligible(ca, x, context, context_lens) if i2v else
+                                  _fused_forward(ca, ((_wan_cross, _wan_cross_fuses),), x, context, context_lens)):
+        x, x8 = DN.wan_residual_ln_fp8(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight, bias=self.norm3.bias)
+        h = x8[0].view(x.shape)
+    else:
+        x, h = DN.wan_residual_ln(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight, bias=self.norm3.bias)
     # WanI2VCrossAttention.forward itself stays unpatched: the block routes it here
-    cross = _wan_i2v_cross(self.cross_attn, h, context, context_lens,
-                           stat="wan_i2v_cross_sp" if sharded else "wan_i2v_cross") if i2v else \
-        self.cross_attn(h, context, context_lens)
-    x, h = DN.wan_residual_ln(x, cross, None, eps=self.norm2.eps, shift=e[3], scale=e[4])   # :339-340
+    if i2v:
+        cross = _wan_i2v_cross(ca, h, context, context_lens,
+                               stat="wan_i2v_cross_sp" if sharded else "wan_i2v_cross", x8=x8)
+    else:
+        cross = ca(h, context, context_lens) if x8 is None else ca(h, context, context_lens, jenga_x8=x8)
     STATS["wan_block"] += 1
-    return DN.wan_gate_residual(x, self.ffn(h), e[5])                          # :340-342
+    x, y = _wan_ffn(self, x, cross, e)                                         # :339-342
+    return DN.wan_gate_residual(x, y, e[5])
+
+
+def _fp8_rows(layers, x) -> bool:
+    """True when the FP8 Linears route every one of `layers` on the rows of the Wan residual stream x
+    (C % 16 == 0): the block then makes their one e4m3 input with a wan_*_fp8 producer"""
+    return x.shape[-1] % 16 == 0 and all(_fp8_routed(lin, x.shape[-1]) is not None for lin in layers)
+
+
+def _fused_forward(module, forms, *args, **kwargs) -> bool:
+    """True when `module`'s forward is one jenga_b200 patched in (not an instance override) and its fused
+    body takes the call: forms are (fused body, predicate) pairs, the predicate called as
+    predicate(module, *args, **kwargs).  Only such a forward is handed e4m3 rows (`jenga_x8`)."""
+    fwd = type(module).forward
+    if "forward" in module.__dict__ or not getattr(fwd, "__jenga_b200__", False):
+        return False
+    fused = getattr(fwd, "__jenga_fused__", None)
+    return any(fused is body and takes(module, *args, **kwargs) for body, takes in forms)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -698,6 +821,7 @@ def _patched(orig, fused):
             STATS["fallback"] += 1
             out = orig(self, *args, **kwargs)
         return out
+    forward.__jenga_fused__ = fused
     return forward
 
 

@@ -230,12 +230,33 @@ def wan_ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, e
     """`norm1(x).float() * (1 + scale) + shift` (model_mul.py:331-333, WanLayerNorm :98-103) followed by
     the bf16 cast the q / k / v Linears apply under autocast.  x [1, L, C] bf16 or fp32, shift / scale
     fp32 with C values (e[0] / e[1]) -> [1, L, C] bf16."""
+    return _wan_ln_modulate(x, shift, scale, eps, fp8=False)
+
+
+def wan_ln_modulate_fp8(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6):
+    """`quantize_rows_fp8(wan_ln_modulate(x, shift, scale, eps))` in one pass, bit for bit; the bf16 rows
+    are never written.  Returns (codes float8_e4m3fn [L, C], a_scale fp32 [L])."""
+    return _wan_ln_modulate(x, shift, scale, eps, fp8=True)
+
+
+def _fp8_rows(rows: int, C: int, device):
+    return (torch.empty((rows, C), dtype=torch.float8_e4m3fn, device=device),
+            torch.empty((rows,), dtype=torch.float32, device=device))
+
+
+def _wan_ln_modulate(x, shift, scale, eps, fp8):
     _require_cuda(x)
     rows, xs = _rows2d(x)
     C = x.shape[-1]
     sc, sh = _wan_vec(scale, C, "scale"), _wan_vec(shift, C, "shift")
-    out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     with torch.cuda.device(x.device):
+        if fp8:
+            out, a_scale = _fp8_rows(rows, C, x.device)
+            check(lib.jenga_wan_ln_modulate_fp8(x.data_ptr(), _x_code(x), xs, sc.data_ptr(), sh.data_ptr(),
+                                                out.data_ptr(), C, a_scale.data_ptr(), rows, C, float(eps),
+                                                _stream_ptr(x.device)), "wan_ln_modulate_fp8")
+            return out, a_scale
+        out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
         check(lib.jenga_wan_ln_modulate(x.data_ptr(), _x_code(x), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(),
                                         C, rows, C, float(eps), _stream_ptr(x.device)), "wan_ln_modulate")
     return out
@@ -248,6 +269,18 @@ def wan_residual_ln(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor | None,
     weight / bias: `norm3(r)`, the affine WanLayerNorm (gate 1 + norm3, model_mul.py:334-339).
     shift / scale: `norm2(r).float() * (1 + scale) + shift` (cross residual + norm2, :339-340).
     x [1, L, C] bf16 or fp32, y bf16 like x -> (r fp32 [1, L, C], normed bf16 [1, L, C])."""
+    return _wan_residual_ln(x, y, gate, eps, weight, bias, shift, scale, fp8=False)
+
+
+def wan_residual_ln_fp8(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor | None, eps: float = 1e-6, *,
+                        weight: torch.Tensor | None = None, bias: torch.Tensor | None = None,
+                        shift: torch.Tensor | None = None, scale: torch.Tensor | None = None):
+    """wan_residual_ln with the normed rows quantised as quantize_rows_fp8 does, in the same pass and bit
+    for bit; r is the same fp32 residual.  -> (r fp32 [1, L, C], (codes float8_e4m3fn [L, C], a_scale [L]))."""
+    return _wan_residual_ln(x, y, gate, eps, weight, bias, shift, scale, fp8=True)
+
+
+def _wan_residual_ln(x, y, gate, eps, weight, bias, shift, scale, fp8):
     _require_cuda(x)
     rows, xs = _rows2d(x)
     ys = _wan_y(x, y)
@@ -259,8 +292,16 @@ def wan_residual_ln(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor | None,
     vb = _wan_vec(bias if affine else shift, C, "bias" if affine else "shift")
     g = _wan_vec(gate, C, "gate") if gate is not None else None
     res = torch.empty(x.shape, dtype=torch.float32, device=x.device)
-    out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     with torch.cuda.device(x.device):
+        if fp8:
+            out, a_scale = _fp8_rows(rows, C, x.device)
+            check(lib.jenga_wan_residual_ln_fp8(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys,
+                                                g.data_ptr() if g is not None else None, res.data_ptr(), C,
+                                                va.data_ptr(), vb.data_ptr(), int(affine), out.data_ptr(), C,
+                                                a_scale.data_ptr(), rows, C, float(eps), _stream_ptr(x.device)),
+                  "wan_residual_ln_fp8")
+            return res, (out, a_scale)
+        out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
         check(lib.jenga_wan_residual_ln(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys,
                                         g.data_ptr() if g is not None else None, res.data_ptr(), C, va.data_ptr(),
                                         vb.data_ptr(), int(affine), out.data_ptr(), C, rows, C, float(eps),
@@ -293,9 +334,11 @@ import os as _os
 LINEAR_FP8: bool = _os.environ.get("JENGA_LINEAR_FP8", "0") == "1"
 # (weight kind, K, N) of the block Linears the switch routes: only those where quantisation + FP8 GEMM
 # measured faster than the call it replaces (bench_linear_fp8.py; kind "bf16" against bf16 F.linear,
-# "fp8_ref" against the reference's --use-fp8 forward).  On an H100 80GB at 700 W none of the six
-# HunyuanVideo image-row shapes did (README, "Opt-in FP8 Linears"), so the switch routes nothing yet.
-FP8_ROUTED: frozenset = frozenset()
+# "fp8_ref" against the reference's --use-fp8 forward, "fp32" against Wan's producer + autocast module
+# call, weight cast included).  On an H100 80GB at 700 W none of the six HunyuanVideo image-row shapes did,
+# and of the Wan shapes only Wan-14B's ffn.2, 13 824 -> 5120, fed by gelu_tanh_fp8 (README, "Opt-in FP8
+# Linears").
+FP8_ROUTED: frozenset = frozenset({("fp32", 13824, 5120)})
 
 
 def linear_fp8_shape_ok(k: int, n: int) -> bool:
@@ -346,6 +389,22 @@ def ln_modulate_fp8(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, e
     return out, a_scale
 
 
+def gelu_tanh_fp8(x: torch.Tensor):
+    """`quantize_rows_fp8(nn.GELU(approximate="tanh")(x))` in one pass, bit for bit (gelu_tanh_into's
+    arithmetic); the bf16 rows are never written.  x [..., C] bf16 with uniformly strided rows, C <= 16384
+    (Wan's ffn.0 output) -> (codes float8_e4m3fn [rows, C], a_scale fp32 [rows])."""
+    _require_cuda(x)
+    if x.dtype != torch.bfloat16:
+        raise ValueError("x must be bf16")
+    rows, xs = _rows2d(x)
+    C = x.shape[-1]
+    out, a_scale = _fp8_rows(rows, C, x.device)
+    with torch.cuda.device(x.device):
+        check(lib.jenga_gelu_tanh_fp8(x.data_ptr(), xs, out.data_ptr(), C, a_scale.data_ptr(), rows, C,
+                                      _stream_ptr(x.device)), "gelu_tanh_fp8")
+    return out, a_scale
+
+
 def linear_fp8(x8: torch.Tensor, a_scale: torch.Tensor, w8: torch.Tensor, w_scale: torch.Tensor,
                bias: torch.Tensor | None = None) -> torch.Tensor:
     """bf16( (x8 . w8^T) * a_scale[m] * w_scale[n] + bias[n] ), fp32 accumulation.
@@ -382,24 +441,28 @@ def linear_fp8(x8: torch.Tensor, a_scale: torch.Tensor, w8: torch.Tensor, w_scal
 
 
 def fp8_weight_kind(layer: torch.nn.Module) -> str:
-    """the FP8_ROUTED kind of a layer fp8_weight takes: "fp8_ref" for a --use-fp8 layer, else "bf16"
+    """the FP8_ROUTED kind of a layer fp8_weight takes: "fp8_ref" for a --use-fp8 layer, "fp32" for an
+    fp32 weight (Wan2.1's Linears), else "bf16"; HunyuanVideo layers are never of kind "fp32"
     """
-    return "fp8_ref" if layer.weight.dtype == torch.float8_e4m3fn else "bf16"
+    dt = layer.weight.dtype
+    return "fp8_ref" if dt == torch.float8_e4m3fn else "fp32" if dt == torch.float32 else "bf16"
 
 
 def fp8_weight(layer: torch.nn.Module):
     """(w8 e4m3 [N, K], w_scale fp32, bias) of an nn.Linear, or None when the layer is not one the FP8
     path takes.  A bf16 weight is quantised once per output channel (w_scale[n] = amax / 448) and the
     result is cached on the module, keyed on the weight's data_ptr and _version (one extra byte per
-    parameter).  A reference --use-fp8 layer (e4m3 weight and `fp8_scale`, hyvideo/modules/
-    fp8_optimization.py:convert_fp8_linear) is used as it is with the per-tensor scale
-    float(fp8_scale.to(bf16)) that fp8_activation_dequant multiplies by."""
+    parameter).  An fp32 weight (Wan2.1 keeps fp32 parameters) is first rounded to bf16, the operand
+    autocast hands cuBLAS, then quantised and cached the same way.  A reference --use-fp8 layer (e4m3
+    weight and `fp8_scale`, hyvideo/modules/fp8_optimization.py:convert_fp8_linear) is used as it is with
+    the per-tensor scale float(fp8_scale.to(bf16)) that fp8_activation_dequant multiplies by."""
     w = getattr(layer, "weight", None)
     if not isinstance(w, torch.Tensor) or not w.is_cuda or w.dim() != 2 or not w.is_contiguous():
         return None
     s = getattr(layer, "fp8_scale", None)
     fp8_ref = w.dtype == torch.float8_e4m3fn and isinstance(s, torch.Tensor) and s.numel() == 1
-    plain = (type(layer) is torch.nn.Linear and w.dtype == torch.bfloat16 and "forward" not in layer.__dict__)
+    plain = (type(layer) is torch.nn.Linear and w.dtype in (torch.bfloat16, torch.float32)
+             and "forward" not in layer.__dict__)
     if not (fp8_ref or plain) or layer._forward_hooks or layer._forward_pre_hooks:
         return None
     if not linear_fp8_shape_ok(w.shape[1], w.shape[0]):
@@ -410,7 +473,7 @@ def fp8_weight(layer: torch.nn.Module):
     if fp8_ref:
         key = ("ref", w.data_ptr(), w._version, s.data_ptr(), s._version)
     else:
-        key = ("bf16", w.data_ptr(), w._version)
+        key = (fp8_weight_kind(layer), w.data_ptr(), w._version)
     hit = layer.__dict__.get("_jenga_fp8")
     if hit is not None and hit[0] == key:
         return hit[1], hit[2], b
@@ -420,6 +483,6 @@ def fp8_weight(layer: torch.nn.Module):
             w_scale = torch.tensor([float(s.to(torch.bfloat16))], dtype=torch.float32,
                                    device=w.device)
         else:
-            w8, w_scale = quantize_rows_fp8(w)
+            w8, w_scale = quantize_rows_fp8(w.to(torch.bfloat16))
     layer.__dict__["_jenga_fp8"] = (key, w8, w_scale)
     return w8, w_scale, b
