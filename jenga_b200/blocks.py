@@ -469,31 +469,50 @@ def _i2v_single(mod, self, x, vec, txt_len, cu_seqlens_q=None, cu_seqlens_kv=Non
 # ------------------------------------------------------------------------------------------------
 # Wan blocks
 # ------------------------------------------------------------------------------------------------
+def _wan_rms(norm) -> bool:
+    """the q / k norm the fused Wan prologues take: WanRMSNorm (model_mul.py:74-90) with a weight"""
+    return type(norm).__name__ == "WanRMSNorm" and getattr(norm, "weight", None) is not None
+
+
+def _wan_self_ok(self, x, per_block_tokens=128) -> bool:
+    """the WanSelfAttention call _wan_self_fused takes, the Linears' output dtypes aside"""
+    return (x.is_cuda and x.shape[0] == 1 and self.head_dim == 128 and per_block_tokens == 128
+            and _wan_rms(self.norm_q) and _wan_rms(self.norm_k))
+
+
 def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates, freq_remap,
-                    block_neighbor_list, stats=("wan_self_sp", "wan_self_dense_sp"), x8=None):
-    """WanSelfAttention.forward with the fused norm + RoPE prologue and no fall-back.
+                    block_neighbor_list, stats, x8=None, fallback=False):
+    """WanSelfAttention.forward with the fused norm + RoPE prologue: the body of every fused Wan
+    self-attention route (_wan_self, _wan_i2v_self).
     jsp set: x is a rank's n rows of a sharded Wan forward (wan_sp.py); the prologue runs on them, then
     the Ulysses exchange and the operator over the first L (the global token count) exchanged rows.
-    jsp None: x is all L rows on one GPU (the single-GPU I2V forward of wan_sp.py).
-    top_k and first_frame_blocks follow the single-GPU rule over L (model_mul.py:161-164); sa_drop_rate
-    <= 0.25 (:153, the warm-up steps) runs the dense class, the flash_attn shim's launch.  freq_remap:
-    the RoPE row of each row (None: raster, one GPU only).  stats: the STATS keys of a carved and of a
-    dense call.  x8: see _wan_qkv."""
+    jsp None: x is all L rows on one GPU; a carved call runs WAN.self_attention, a dense one the flash_attn
+    shim's launch.  top_k and first_frame_blocks follow the single-GPU rule over L (model_mul.py:161-164);
+    sa_drop_rate <= 0.25 (:153, the warm-up steps) is a dense call.  freq_remap: the RoPE row of each row
+    (None: raster, one GPU only).  stats: the STATS keys of a carved and of a dense call.  x8: see _wan_qkv.
+    A call it does not take raises, except with `fallback` (the one-GPU carved route of model_mul.py), where
+    a q Linear dtype the prologue does not take returns None for the original forward, and v goes to the
+    operator as the v Linear returns it (the operator casts it)."""
     b, n = x.shape[:2]
-    if not _wan_self_fused_ok(self, x, per_block_tokens) or (jsp is not None and freq_remap is None):
+    if not _wan_self_ok(self, x, per_block_tokens) or (jsp is not None and freq_remap is None):
         raise RuntimeError(f"{type(self).__name__}: the call is not one the fused Wan self-attention takes (a "
                            "CUDA batch-1 input, head_dim 128, 128-token blocks, WanRMSNorm q / k norms with "
                            "weights and, under jenga_sp, a freq_remap); this route has no fall-back")
     q_lin, k_lin, v = _wan_qkv(self, x, x8)
-    if q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype != q_lin.dtype:
+    if fallback:
+        if q_lin.dtype not in (torch.bfloat16, torch.float32):
+            return None
+        v = v.view(b, n, self.num_heads, self.head_dim)
+    elif q_lin.dtype not in (torch.bfloat16, torch.float32) or k_lin.dtype != q_lin.dtype:
         raise RuntimeError(f"{type(self).__name__}: q / k Linears return {q_lin.dtype}, the prologue takes bf16 "
                            "or fp32")
+    else:
+        # the bf16 v both single-GPU routes attend: flash_attention's half() and the operator's cast
+        v = v.view(b, n, self.num_heads, self.head_dim).to(torch.bfloat16).contiguous()
     grid = [int(g) for g in grid_sizes[0].tolist()]
     L = grid[0] * grid[1] * grid[2]
     eps = float(self.norm_q.eps)
     wq, wk = self.norm_q.weight, self.norm_k.weight
-    # the bf16 v both single-GPU routes attend: flash_attention's half() and the operator's cast
-    v = v.view(b, n, self.num_heads, self.head_dim).to(torch.bfloat16).contiguous()
     dense = sa_drop_rate <= 0.25
     if jsp is None and not dense:
         out = WAN.self_attention(q_lin, k_lin, v, wq, wk, self.num_heads, grid, freqs, sa_drop_rate,
@@ -511,7 +530,9 @@ def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tok
     STATS[stats[dense]] += 1
     out = out.flatten(2)
     if not torch.is_autocast_enabled():
-        out = out.float()       # the query dtype the reference returns, as in _wan_self
+        # the reference returns the query dtype, fp32 (rope_apply -> .float(), model_mul.py:71;
+        # operator :530-532); under autocast the following Linear casts back to bf16 anyway
+        out = out.float()
     return _linear(self.o, out)
 
 
@@ -523,13 +544,25 @@ def _wan_qkv(self, x, x8):
     return tuple(_linear8(lin, x8, x.shape[:-1]) for lin in (self.q, self.k, self.v))
 
 
-def _wan_self_fused_ok(self, x, per_block_tokens=128):
-    """the configuration _wan_self_fused takes, the Linears' output dtype aside"""
-    wq = getattr(self.norm_q, "weight", None)
-    wk = getattr(self.norm_k, "weight", None)
-    return (x.is_cuda and x.shape[0] == 1 and self.head_dim == 128 and per_block_tokens == 128 and wq is not None
-            and wk is not None and type(self.norm_q).__name__ == "WanRMSNorm"
-            and type(self.norm_k).__name__ == "WanRMSNorm")
+def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128, p_remain_rates=0.8,
+              freq_remap=None, block_neighbor_list=None, *, jenga_x8=None):
+    """WanSelfAttention.forward of model_mul.py (:134-180).  Under `jenga_sp` (the Hilbert-sharded Wan
+    forward of wan_sp.py) every call runs _wan_self_fused through the exchange, or raises; on one GPU the
+    carved call does, and any other call runs the original forward.
+    jenga_x8: the block's e4m3 q / k / v input (_wan_qkv), passed only when _wan_self_takes says so."""
+    if not _wan_self_takes(self, x, sa_drop_rate, per_block_tokens):
+        return None
+    jsp = getattr(self, "jenga_sp", None)
+    stats = ("wan_self_sp", "wan_self_dense_sp") if jsp is not None else ("wan_self", None)
+    return _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
+                           freq_remap, block_neighbor_list, stats, x8=jenga_x8, fallback=jsp is None)
+
+
+def _wan_self_takes(self, x, sa_drop_rate=0.0, per_block_tokens=128, **_):
+    """True when _wan_self runs _wan_self_fused rather than the original forward: under jenga_sp, or for
+    the carved call (sa_drop_rate > 0.25) on one GPU"""
+    return getattr(self, "jenga_sp", None) is not None or (
+        sa_drop_rate > 0.25 and _wan_self_ok(self, x, per_block_tokens))
 
 
 def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=None, freq_remap=None, block_neighbor_list=None,
@@ -544,85 +577,48 @@ def _wan_i2v_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=None, freq_
     With the Jenga arguments of model_mul.py (the I2V forwards of wan_sp.py): _wan_self_fused, on one GPU
     or under jenga_sp.  A call it does not take runs the original forward on raster rows (freq_remap None)
     and raises on curve-ordered rows, whose RoPE positions the original forward does not know.
-    jenga_x8: the block's e4m3 q / k / v input (_wan_qkv), passed only when _wan_i2v_self_fuses says so."""
-    jsp = getattr(self, "jenga_sp", None)
-    if sa_drop_rate is None:
-        if jsp is None:
+    jenga_x8: the block's e4m3 q / k / v input (_wan_qkv), passed only when _wan_i2v_self_takes says so."""
+    if not _wan_i2v_self_takes(self, x, sa_drop_rate, freq_remap):
+        if sa_drop_rate is None:
             return None
+        STATS["fallback"] += 1
+        return type(self).forward.__wrapped__(self, x, seq_lens, grid_sizes, freqs)
+    jsp = getattr(self, "jenga_sp", None)
+    if jsp is None:
+        stats = ("wan_i2v_self", "wan_i2v_self_dense")
+    elif sa_drop_rate is not None:
+        stats = ("wan_i2v_self_carved_sp", "wan_i2v_self_sp")
+    else:
         _, r = world(jsp.group)
         n = x.shape[1]
         L = int(torch.prod(grid_sizes[0]))
         rows = torch.arange(r * n, (r + 1) * n, device=x.device)
-        remap = torch.where(rows < L, rows, torch.zeros_like(rows))
-        return _wan_self_fused(self, jsp, x, grid_sizes, freqs, 0.0, 128, 0.0, remap, None,
-                               stats=(None, "wan_i2v_self_sp"), x8=jenga_x8)
-    if not _wan_i2v_self_fuses(self, x, sa_drop_rate, freq_remap):
-        STATS["fallback"] += 1
-        return type(self).forward.__wrapped__(self, x, seq_lens, grid_sizes, freqs)
-    stats = ("wan_i2v_self_carved_sp", "wan_i2v_self_sp") if jsp is not None else ("wan_i2v_self", "wan_i2v_self_dense")
+        freq_remap = torch.where(rows < L, rows, torch.zeros_like(rows))
+        sa_drop_rate, p_remain_rates, stats = 0.0, 0.0, (None, "wan_i2v_self_sp")
     return _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, 128, p_remain_rates, freq_remap,
-                           block_neighbor_list, stats=stats, x8=jenga_x8)
+                           block_neighbor_list, stats, x8=jenga_x8)
 
 
-def _wan_i2v_self_fuses(self, x, sa_drop_rate=None, freq_remap=None, **_):
-    """True when _wan_i2v_self runs _wan_self_fused (or raises) rather than the original forward"""
-    if getattr(self, "jenga_sp", None) is not None:
-        return True
-    return sa_drop_rate is not None and (freq_remap is not None or _wan_self_fused_ok(self, x))
+def _wan_i2v_self_takes(self, x, sa_drop_rate=None, freq_remap=None, **_):
+    """True when _wan_i2v_self runs _wan_self_fused (or raises) rather than the original forward: under
+    jenga_sp, or with the Jenga arguments on curve-ordered rows or for a call _wan_self_fused takes"""
+    return getattr(self, "jenga_sp", None) is not None or (
+        sa_drop_rate is not None and (freq_remap is not None or _wan_self_ok(self, x)))
 
 
-def _wan_self(self, x, seq_lens, grid_sizes, freqs, sa_drop_rate=0.0, per_block_tokens=128, p_remain_rates=0.8,
-              freq_remap=None, block_neighbor_list=None, *, jenga_x8=None):
-    """jenga_x8: the block's e4m3 q / k / v input (_wan_qkv), passed only when _wan_self_fuses says so"""
-    jsp = getattr(self, "jenga_sp", None)
-    if jsp is not None:
-        return _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates,
-                               freq_remap, block_neighbor_list, x8=jenga_x8)
-    if not _wan_self_fuses(self, x, sa_drop_rate, per_block_tokens):
-        return None
-    b, s = x.shape[:2]
-    wq, wk = self.norm_q.weight, self.norm_k.weight
-    q_lin, k_lin, v = _wan_qkv(self, x, jenga_x8)
-    if q_lin.dtype not in (torch.bfloat16, torch.float32):
-        return None
-    v = v.view(b, s, self.num_heads, self.head_dim)
-    grid = [int(g) for g in grid_sizes[0].tolist()]
-    out = WAN.self_attention(q_lin, k_lin, v, wq, wk, self.num_heads, grid, freqs, sa_drop_rate,
-                             p_remain_rates=p_remain_rates, freq_remap=freq_remap,
-                             block_neighbor_list=block_neighbor_list, eps=float(self.norm_q.eps))
-    STATS["wan_self"] += 1
-    out = out.flatten(2)
-    if not torch.is_autocast_enabled():
-        # the reference returns the query dtype, fp32 (rope_apply -> .float(), model_mul.py:71;
-        # operator :530-532); under autocast the following Linear casts back to bf16 anyway
-        out = out.float()
-    return _linear(self.o, out)
-
-
-def _wan_self_fuses(self, x, sa_drop_rate=0.0, per_block_tokens=128, **_):
-    """True when _wan_self runs a fused route (jenga_sp, or the carved call on one GPU) rather than
-    returning None for the original forward; the Linears' output dtype aside"""
-    if getattr(self, "jenga_sp", None) is not None:
-        return True
-    return (sa_drop_rate > 0.25 and x.is_cuda and x.shape[0] == 1 and self.head_dim == 128
-            and per_block_tokens == 128 and getattr(self.norm_q, "weight", None) is not None
-            and getattr(self.norm_k, "weight", None) is not None and type(self.norm_q).__name__ == "WanRMSNorm")
-
-
-def _wan_cross_fuses(self, x, context, context_lens):
+def _wan_cross_takes(self, x, context, context_lens):
     """True when _wan_cross runs the fused T2V cross-attention (the Linears' output dtypes aside)"""
     # context_lens: the reference's varlen form (wan/modules/attention.py:69-80); teacache_forward
     # passes None (jenga_wan.py:569)
     return (context_lens is None and x.is_cuda and x.dim() == 3 and x.shape[0] == 1 and context.dim() == 3
-            and context.shape[0] == 1 and self.head_dim == 128 and getattr(self.norm_q, "weight", None) is not None
-            and getattr(self.norm_k, "weight", None) is not None and type(self.norm_q).__name__ == "WanRMSNorm"
-            and type(self.norm_k).__name__ == "WanRMSNorm" and DN._autocast_bf16())
+            and context.shape[0] == 1 and self.head_dim == 128 and _wan_rms(self.norm_q) and _wan_rms(self.norm_k)
+            and DN._autocast_bf16())
 
 
 def _wan_cross(self, x, context, context_lens, *, jenga_x8=None):
     """jenga_x8: the block's wan_residual_ln_fp8 rows of x (x their e4m3 view) for the q Linear, passed only
-    when _wan_cross_fuses says so"""
-    if not _wan_cross_fuses(self, x, context, context_lens):
+    when _wan_cross_takes says so"""
+    if not _wan_cross_takes(self, x, context, context_lens):
         return None
     q_lin = self.q(x) if jenga_x8 is None else _linear8(self.q, jenga_x8, x.shape[:-1])
     k_lin, v = self.k(context), self.v(context)
@@ -647,7 +643,7 @@ def _wan_i2v_cross_shape_ok(ca, x, context, context_lens):
     return (context_lens is None and isinstance(x, torch.Tensor) and isinstance(context, torch.Tensor)
             and x.dim() == 3 and x.shape[0] == 1 and context.dim() == 3 and context.shape[0] == 1
             and context.shape[1] > _WAN_I2V_IMG_TOKENS and getattr(ca, "head_dim", None) == 128
-            and all(type(n).__name__ == "WanRMSNorm" and getattr(n, "weight", None) is not None for n in norms)
+            and all(_wan_rms(n) for n in norms)
             and len({float(n.eps) for n in norms}) == 1)
 
 
@@ -683,51 +679,44 @@ def _wan_i2v_cross(ca, x, context, context_lens, stat="wan_i2v_cross", x8=None):
     return ca(x, context, context_lens)
 
 
-def _wan_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=0.0, freq_remap=None,
-               block_neighbor_list=None, p_remain_rates=0.0):
-    return _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens,
-                           dict(sa_drop_rate=sa_drop_rate, freq_remap=freq_remap,
-                                block_neighbor_list=block_neighbor_list, p_remain_rates=p_remain_rates))
-
-
-def _wan_plain_block(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=None,
-                     freq_remap=None, block_neighbor_list=None, p_remain_rates=0.8):
-    """WanAttentionBlock.forward of wan/modules/model.py (:274-313): the fused body, with the
-    self-attention called in that module's signature, or, when the I2V forwards of wan_sp.py pass the
-    Jenga arguments of model_mul.py (sa_drop_rate not None), with those.  Under `self_attn.jenga_sp`
-    (parallelize_wan_i2v) x is a rank's rows and there is no fall-back: the checks run before the
-    exchange, so every rank raises alike.  On one GPU a call the fused body does not take runs the
-    original forward on raster rows and raises on curve-ordered rows (freq_remap set)."""
-    attn_kw = {} if sa_drop_rate is None else dict(sa_drop_rate=sa_drop_rate, freq_remap=freq_remap,
-                                                   block_neighbor_list=block_neighbor_list,
-                                                   p_remain_rates=p_remain_rates)
-    if getattr(self.self_attn, "jenga_sp", None) is None:
-        out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw)
-        if out is not None or sa_drop_rate is None:
-            return out
-        if freq_remap is not None:
-            raise RuntimeError(f"{type(self).__name__}: the call is not one the fused block takes (a CUDA input "
-                               "under bf16 autocast, fp32 modulation, cross_attn_norm=True); the original forward "
-                               "cannot take the curve-ordered rows of the carved I2V forward")
-        STATS["fallback"] += 1
-        return type(self).forward.__wrapped__(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens)
-    if not (type(self.cross_attn).__name__ == "WanI2VCrossAttention"
-            and _wan_i2v_cross_shape_ok(self.cross_attn, x, context, context_lens)):
+def _wan_block(plain, self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, sa_drop_rate=0.0,
+               freq_remap=None, block_neighbor_list=None, p_remain_rates=0.0):
+    """WanAttentionBlock.forward of model_mul.py (:303-346), or, `plain`, of wan/modules/model.py (:274-313),
+    whose own signature (sa_drop_rate None) hands the self-attention (x, seq_lens, grid_sizes, freqs) and
+    whose I2V forwards in wan_sp.py pass the Jenga arguments of model_mul.py.  A call the fused body does
+    not take runs the original forward, except on a plain block:
+      under `self_attn.jenga_sp` (parallelize_wan_i2v) x is a rank's rows and there is no fall-back: the
+      checks run before the exchange, so every rank raises alike;
+      with the Jenga arguments, the original forward runs on raster rows, in model.py's own signature, and
+      the block raises on curve-ordered rows (freq_remap set), whose RoPE positions it does not know."""
+    attn_kw = {} if plain and sa_drop_rate is None else dict(
+        sa_drop_rate=sa_drop_rate, freq_remap=freq_remap, block_neighbor_list=block_neighbor_list,
+        p_remain_rates=p_remain_rates)
+    sharded = plain and getattr(self.self_attn, "jenga_sp", None) is not None
+    if sharded and not (type(self.cross_attn).__name__ == "WanI2VCrossAttention"
+                        and _wan_i2v_cross_shape_ok(self.cross_attn, x, context, context_lens)):
         raise RuntimeError(f"{type(self).__name__} under jenga_sp: the cross-attention is not one the fused I2V "
                            "kernel takes (a WanI2VCrossAttention with WanRMSNorm q / k / k_img norms, head_dim "
                            f"128, batch 1, context_lens None and more than {_WAN_I2V_IMG_TOKENS} context rows); "
                            "the sharded I2V forward has no fall-back")
-    out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded=True)
-    if out is None:
+    out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded)
+    if out is None and sharded:
         raise RuntimeError(f"{type(self).__name__} under jenga_sp: the call is not one the fused block takes (a "
                            "CUDA input under bf16 autocast, fp32 modulation, cross_attn_norm=True); the sharded "
                            "I2V forward has no fall-back")
-    return out
+    if out is not None or not (plain and attn_kw):
+        return out                      # None: the original forward with the caller's arguments (_patched)
+    if freq_remap is not None:
+        raise RuntimeError(f"{type(self).__name__}: the call is not one the fused block takes (a CUDA input "
+                           "under bf16 autocast, fp32 modulation, cross_attn_norm=True); the original forward "
+                           "cannot take the curve-ordered rows of the carved I2V forward")
+    STATS["fallback"] += 1
+    return type(self).forward.__wrapped__(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens)
 
 
-def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded=False):
-    """attn_kw: the Jenga self-attention arguments of model_mul.py (empty for wan/modules/model.py called
-    in its own signature).
+def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded):
+    """The fused block forward, or None for a call it does not take.  attn_kw: the Jenga self-attention
+    arguments of model_mul.py (empty for wan/modules/model.py called in its own signature).
     sharded: the I2V rows of parallelize_wan_i2v; the cross-attention must then be the fused one."""
     i2v = type(self.cross_attn).__name__ == "WanI2VCrossAttention"
     ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
@@ -747,8 +736,7 @@ def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_le
     # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to; with the
     # FP8 Linears routing q / k / v, on the e4m3 rows of that bf16 instead (:331-333)
     sa, ca = self.self_attn, self.cross_attn
-    if _fp8_rows((sa.q, sa.k, sa.v), x) and _fused_forward(
-            sa, ((_wan_self, _wan_self_fuses), (_wan_i2v_self, _wan_i2v_self_fuses)), x, **attn_kw):
+    if _fp8_rows((sa.q, sa.k, sa.v), x) and _fused_forward(sa, x, **attn_kw):
         x8 = DN.wan_ln_modulate_fp8(x, e[0], e[1], eps=self.norm1.eps)
         y = sa(x8[0].view(x.shape), seq_lens, grid_sizes, freqs, jenga_x8=x8, **attn_kw)
     else:
@@ -756,7 +744,7 @@ def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_le
     # gate 1 + norm3 (:334-335, :339), e4m3 when the cross-attention's q is routed
     x8 = None
     if _fp8_rows((ca.q,), x) and (wan_i2v_cross_eligible(ca, x, context, context_lens) if i2v else
-                                  _fused_forward(ca, ((_wan_cross, _wan_cross_fuses),), x, context, context_lens)):
+                                  _fused_forward(ca, x, context, context_lens)):
         x, x8 = DN.wan_residual_ln_fp8(x, y, e[2], eps=self.norm3.eps, weight=self.norm3.weight, bias=self.norm3.bias)
         h = x8[0].view(x.shape)
     else:
@@ -778,15 +766,15 @@ def _fp8_rows(layers, x) -> bool:
     return x.shape[-1] % 16 == 0 and all(_fp8_routed(lin, x.shape[-1]) is not None for lin in layers)
 
 
-def _fused_forward(module, forms, *args, **kwargs) -> bool:
-    """True when `module`'s forward is one jenga_b200 patched in (not an instance override) and its fused
-    body takes the call: forms are (fused body, predicate) pairs, the predicate called as
-    predicate(module, *args, **kwargs).  Only such a forward is handed e4m3 rows (`jenga_x8`)."""
+def _fused_forward(module, *args, **kwargs) -> bool:
+    """True when `module`'s forward is one jenga_b200 patched in (not an instance override) and the
+    predicate _patched stored on it takes the call, called as takes(module, *args, **kwargs).  Only such a
+    forward is handed e4m3 rows (`jenga_x8`); one with no predicate never is."""
     fwd = type(module).forward
     if "forward" in module.__dict__ or not getattr(fwd, "__jenga_b200__", False):
         return False
-    fused = getattr(fwd, "__jenga_fused__", None)
-    return any(fused is body and takes(module, *args, **kwargs) for body, takes in forms)
+    takes = getattr(fwd, "__jenga_takes__", None)
+    return takes is not None and takes(module, *args, **kwargs)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -812,32 +800,35 @@ def _unswap(owner, *attrs: str) -> None:
             setattr(owner, attr, fn.__wrapped__)
 
 
-def _patched(orig, fused):
+def _patched(orig, fused, takes=None):
     """The patched forward: `fused` takes the reference arguments and returns None for a call it does
-    not take; that call then runs `orig` with exactly the caller's arguments."""
+    not take; that call then runs `orig` with exactly the caller's arguments.  takes(module, *args,
+    **kwargs): True when `fused` runs its fused body on the call, the Linears' output dtypes aside; it is
+    stored on the forward for _fused_forward."""
     def forward(self, *args, **kwargs):
         out = fused(self, *args, **kwargs)
         if out is None:
             STATS["fallback"] += 1
             out = orig(self, *args, **kwargs)
         return out
-    forward.__jenga_fused__ = fused
+    forward.__jenga_takes__ = takes
     return forward
 
 
 def _patch_classes(mod, fused) -> list[str]:
+    """fused: class name -> (fused body, its predicate or None), see _patched"""
     done = []
-    for cls, body in fused.items():
+    for cls, (body, takes) in fused.items():
         owner = getattr(mod, cls, None)
-        if owner is not None and _swap(owner, "forward", _patched(owner.forward, body)):
+        if owner is not None and _swap(owner, "forward", _patched(owner.forward, body, takes)):
             done.append(f"{mod.__name__}.{cls}.forward")
     return done
 
 
 def _patch_hy(double, single):
     """the patch of a HunyuanVideo block module: both stream kinds, with the module's own helpers"""
-    return lambda mod: _patch_classes(mod, dict(MMDoubleStreamBlock=functools.partial(double, mod),
-                                                MMSingleStreamBlock=functools.partial(single, mod)))
+    return lambda mod: _patch_classes(mod, dict(MMDoubleStreamBlock=(functools.partial(double, mod), None),
+                                                MMSingleStreamBlock=(functools.partial(single, mod), None)))
 
 
 def patch_plain_wan(mod) -> list[str]:
@@ -845,7 +836,10 @@ def patch_plain_wan(mod) -> list[str]:
     self-attention (x, seq_lens, grid_sizes, freqs), or the Jenga arguments the I2V forwards of wan_sp.py
     pass, and runs the fused I2V cross-attention; WanT2VCrossAttention and WanI2VCrossAttention stay as
     they are"""
-    return _patch_classes(mod, dict(WanSelfAttention=_wan_i2v_self, WanAttentionBlock=_wan_plain_block))
+    # model.py's own signature has no Jenga arguments: sa_drop_rate None stands for it
+    block = functools.partial(_wan_block, True, sa_drop_rate=None, p_remain_rates=0.8)
+    return _patch_classes(mod, dict(WanSelfAttention=(_wan_i2v_self, _wan_i2v_self_takes),
+                                    WanAttentionBlock=(block, None)))
 
 
 def _unpatch_plain_wan(mod) -> None:
@@ -889,7 +883,8 @@ _HOOKS = {
     # WanI2VCrossAttention overrides forward itself and is left as it is; the fused block forward runs
     # its fused form (_wan_i2v_cross)
     "wan.modules.model_mul": _Hook(lambda mod: _patch_classes(mod, dict(
-        WanSelfAttention=_wan_self, WanT2VCrossAttention=_wan_cross, WanAttentionBlock=_wan_block)), _FUSED),
+        WanSelfAttention=(_wan_self, _wan_self_takes), WanT2VCrossAttention=(_wan_cross, _wan_cross_takes),
+        WanAttentionBlock=(functools.partial(_wan_block, False), None))), _FUSED),
     # WanI2V(use_usp=False) gets the single-GPU I2V forward of wan_sp.py, and the plain model's blocks the
     # fused forwards, when the pipeline is built (wan.modules.model itself, which only WanI2V imports,
     # stays untouched at import without the Wan switch).  Not undone by set_wan_sp(False).
