@@ -324,7 +324,8 @@ def block_sparse_attention_variant(
     use_cu = variant != "wan" and cu_seqlens_q is not None and cu_seqlens_kv is not None
     seqlen_dev = None
     if use_cu:
-        # ref :328-329 — only element [1] is read, on the device
+        # ref :328-329 — only element [1] is read, on the device.  At B > 1 it limits every sample, as
+        # in the reference: exact when the samples share one prompt (--num-videos)
         seqlen_dev = cu_seqlens_q[1:2].to(device=query.device, dtype=torch.int32)
     if variant == "hyvideo" and S % BLOCK != 0:
         # ref :216 reshape fails on ragged S (the padded copies of :331-335 are never used)

@@ -137,7 +137,7 @@ def _ln_mod(mod, norm, x, shift, scale, tr=None):
 
 
 def _gate_res(mod, x, y, gate, tr=None):
-    """x + apply_gate(y, gate) — one fused pass for bf16 batch-1 tensors.
+    """x + apply_gate(y, gate) — one fused pass per sample for bf16 tensors.
     tr=(tr_gate, first_frame_mask): the I2V token-replace form (modulate_layers.py:84-95)."""
     if DN.gate_residual_supported(x, y, gate, tr=tr):
         STATS["gate_residual"] += 1
@@ -364,10 +364,11 @@ def _single_stream(mod, self, x, vec, txt_len, cu_seqlens_q, cu_seqlens_kv, freq
     assert cu_seqlens_q.shape[0] == 2 * x.shape[0] + 1                           # :444-446
     # `torch.cat((attn, self.mlp_act(mlp)), 2)` (:499) without the concatenation copy: the attention
     # kernel writes its rows into the first `hidden` columns of linear2's input buffer and the
-    # GELU kernel writes the rest
+    # GELU kernel writes the rest.  At B > 1 sample b's attention rows start b*S*(C + mlp) elements in
+    # (the kernel's o_stride_b); the GELU rows stay uniformly strided
     act = self.mlp_act
     fuse_cat = (isinstance(act, torch.nn.GELU) and getattr(act, "approximate", "none") == "tanh"
-                and lin1.dtype == torch.bfloat16 and x.shape[0] == 1
+                and lin1.dtype == torch.bfloat16
                 and not getattr(self, "hybrid_seq_parallel_attn", None) and getattr(self, "jenga_sp", None) is None)
     cat = attn_view = None
     if fuse_cat:

@@ -9,6 +9,11 @@ callers (jenga_b200/blocks.py) fall back to the reference's own ops for anything
 (hyvideo_i2v/modules/modulate_layers.py:51-56,84-95): `tr=(tr_shift, tr_scale, row_mask)` /
 `tr=(tr_gate, row_mask)`, where rows whose mask entry is true take the tr_ parameters.
 
+The HunyuanVideo chains take several samples per call (`--num-videos N`): x [B, L, C] with
+modulation vectors [B, C], one row per sample, or [1, C] shared by all.  Sample b runs the same
+launch as a B = 1 call, on its rows with its vector row, so its result is bit-identical to that
+call; a token-replace row mask has one entry per row of a sample and is shared by all samples.
+
 The `wan_*` functions are the chains of Wan2.1's WanAttentionBlock.forward
 (wan/modules/model_mul.py:326-346), whose residual stream is fp32 and whose modulation vectors are
 the fp32 rows of `e` [1, 6, C]."""
@@ -79,13 +84,51 @@ def _per_channel(v: torch.Tensor, C: int, what: str) -> torch.Tensor:
     return v
 
 
+def _samples(x: torch.Tensor):
+    """x [..., C] -> (samples, rows per sample, row stride, sample stride), strides in elements.  A 3-D x
+    with B > 1 is B samples, each launched on its own rows, so its batch stride may be any multiple of 8
+    (attn[:, :L] of the double-stream block); any other x is one sample of uniformly strided rows."""
+    if x.dim() == 3 and x.shape[0] > 1:
+        if x.stride(-1) != 1:
+            raise ValueError("channel dim must be contiguous")
+        return x.shape[0], x.shape[1], x.stride(1), x.stride(0)
+    rows, stride = _rows2d(x)
+    return 1, rows, stride, 0
+
+
+def _sample_vecs(x: torch.Tensor, vecs: dict, mask=None) -> dict:
+    """The shape checks of the HunyuanVideo chains, made before any device check or launch.  Each vector
+    of `vecs` (name -> tensor) holds C values, shared by every sample, or is [B, C] for x [B, L, C], one
+    row per sample; a token-replace mask is 1-D with one entry per row of a sample.
+    -> name -> [1, C] or [B, C] view."""
+    C = x.shape[-1]
+    B = x.shape[0] if x.dim() == 3 else 1
+    out = {}
+    for name, v in vecs.items():
+        if v.numel() == C:
+            out[name] = v.reshape(1, C)
+        elif B > 1 and v.dim() >= 2 and v.shape[-1] == C and v.numel() == B * C:
+            out[name] = v.reshape(B, C)
+        else:
+            raise ValueError(f"{name} must hold one value per channel ({C}), or one row of them per sample "
+                             f"([{B}, {C}]); got {tuple(v.shape)}")
+    if mask is not None and (mask.dim() != 1 or mask.numel() * B * C != x.numel()):
+        raise ValueError("row mask must hold one entry per row")
+    return out
+
+
+def _vec_ptr(v: torch.Tensor, b: int) -> int:
+    """address of sample b's row of a contiguous [1, C] / [B, C] vector"""
+    return v.data_ptr() + (b if v.shape[0] > 1 else 0) * v.stride(0) * v.element_size()
+
+
 def ln_modulate_supported(x: torch.Tensor, norm: torch.nn.Module, shift, scale, tr=None) -> bool:
     return (isinstance(norm, torch.nn.LayerNorm) and norm.weight is None and norm.bias is None
             and x.is_cuda and x.dtype == torch.bfloat16 and torch.is_autocast_enabled()
-            and torch.get_autocast_dtype("cuda") == torch.bfloat16 and x.dim() == 3 and x.shape[0] == 1
+            and torch.get_autocast_dtype("cuda") == torch.bfloat16 and x.dim() == 3
             and shift is not None and scale is not None and shift.dtype == torch.bfloat16
             and scale.dtype == torch.bfloat16 and x.shape[-1] % 8 == 0 and x.shape[-1] <= 6144
-            and x.stride(-1) == 1 and x.stride(-2) % 8 == 0
+            and x.stride(-1) == 1 and x.stride(-2) % 8 == 0 and (x.shape[0] == 1 or x.stride(0) % 8 == 0)
             and (tr is None or _tr_supported(x, tr[:2], tr[2])))
 
 
@@ -93,60 +136,87 @@ def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: 
                 tr=None) -> torch.Tensor:
     """`modulate(LayerNorm(x), shift=shift, scale=scale)` followed by the bf16 cast the next Linear
     applies under autocast (models_mul…:196-199,297-304,409; modulate_layers.py:31-49).
-    x [1, L, C] bf16, shift/scale [1, C] bf16 -> [1, L, C] bf16.
+    x [B, L, C] bf16, shift/scale [B, C] or [1, C] bf16 -> [B, L, C] bf16.
     tr=(tr_shift, tr_scale, row_mask): the token-replace form (hyvideo_i2v/…/modulate_layers.py:51-56),
     row_mask a bool [L] on x's device or on the CPU."""
-    _require_cuda(x, shift, scale)
-    rows, xs = _rows2d(x)
+    return _ln_modulate(x, shift, scale, eps, tr, fp8=False)
+
+
+def _ln_modulate(x, shift, scale, eps, tr, fp8):
+    vecs = {"shift": shift, "scale": scale}
+    if tr is not None:
+        vecs.update(tr_shift=tr[0], tr_scale=tr[1])
+    v = _sample_vecs(x, vecs, tr[2] if tr is not None else None)
+    _require_cuda(x, *vecs.values())
+    n, rows, xs, xb = _samples(x)
     C = x.shape[-1]
-    out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    sc, sh = _per_channel(scale, C, "scale"), _per_channel(shift, C, "shift")
+    v = {k: t.contiguous() for k, t in v.items()}
+    m = _row_mask(tr[2], x.device) if tr is not None else None
+    if fp8:
+        out, a_scale = _fp8_rows(n * rows, C, x.device)
+    else:
+        out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    stream = _stream_ptr(x.device)
     with torch.cuda.device(x.device):
-        if tr is None:
-            check(lib.jenga_ln_modulate(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(), C, rows, C,
-                                        float(eps), _stream_ptr(x.device)), "ln_modulate")
-            return out
-        tr_shift, tr_scale, mask = tr
-        _require_cuda(tr_shift, tr_scale)
-        tsc, tsh = _per_channel(tr_scale, C, "tr_scale"), _per_channel(tr_shift, C, "tr_shift")
-        if mask.dim() != 1 or mask.numel() != rows:
-            raise ValueError("row mask must hold one entry per row")
-        m = _row_mask(mask, x.device)
-        check(lib.jenga_ln_modulate_tr(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), tsc.data_ptr(), tsh.data_ptr(),
-                                       m.data_ptr(), out.data_ptr(), C, rows, C, float(eps), _stream_ptr(x.device)),
-              "ln_modulate_tr")
-    return out
+        for b in range(n):
+            xp = x.data_ptr() + b * xb * x.element_size()
+            op = out.data_ptr() + b * rows * C * out.element_size()
+            sc, sh = _vec_ptr(v["scale"], b), _vec_ptr(v["shift"], b)
+            if tr is not None:
+                tsc, tsh = _vec_ptr(v["tr_scale"], b), _vec_ptr(v["tr_shift"], b)
+            if fp8:
+                sp = a_scale.data_ptr() + b * rows * a_scale.element_size()
+                if tr is None:
+                    check(lib.jenga_ln_modulate_fp8(xp, xs, sc, sh, op, C, sp, rows, C, float(eps), stream),
+                          "ln_modulate_fp8")
+                else:
+                    check(lib.jenga_ln_modulate_tr_fp8(xp, xs, sc, sh, tsc, tsh, m.data_ptr(), op, C, sp, rows, C,
+                                                       float(eps), stream), "ln_modulate_tr_fp8")
+            elif tr is None:
+                check(lib.jenga_ln_modulate(xp, xs, sc, sh, op, C, rows, C, float(eps), stream), "ln_modulate")
+            else:
+                check(lib.jenga_ln_modulate_tr(xp, xs, sc, sh, tsc, tsh, m.data_ptr(), op, C, rows, C, float(eps),
+                                               stream), "ln_modulate_tr")
+    return (out, a_scale) if fp8 else out
 
 
 def gate_residual_supported(x, y, gate, tr=None) -> bool:
     return (x.is_cuda and x.dtype == y.dtype == torch.bfloat16 and gate is not None and gate.dtype == torch.bfloat16
-            and x.shape == y.shape and x.dim() == 3 and x.shape[0] == 1 and x.shape[-1] % 8 == 0
+            and x.shape == y.shape and x.dim() == 3 and x.shape[-1] % 8 == 0
             and x.stride(-1) == 1 and y.stride(-1) == 1 and x.stride(-2) % 8 == 0 and y.stride(-2) % 8 == 0
+            and (x.shape[0] == 1 or (x.stride(0) % 8 == 0 and y.stride(0) % 8 == 0))
             and (tr is None or _tr_supported(x, tr[:1], tr[1])))
 
 
 def gate_residual(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor, tr=None) -> torch.Tensor:
     """`x + apply_gate(y, gate=gate)` (models_mul…:295-315,:500; modulate_layers.py:52-68).
+    x, y [B, L, C] bf16, gate [B, C] or [1, C] bf16 -> [B, L, C] bf16.
     tr=(tr_gate, row_mask): the token-replace form (hyvideo_i2v/…/modulate_layers.py:84-95)."""
-    _require_cuda(x, y, gate)
-    rows, xs = _rows2d(x)
-    _, ys = _rows2d(y)
+    vecs = {"gate": gate}
+    if tr is not None:
+        vecs["tr_gate"] = tr[0]
+    v = _sample_vecs(x, vecs, tr[1] if tr is not None else None)
+    if y.shape != x.shape:
+        raise ValueError("y must be shaped like x")
+    _require_cuda(x, y, *vecs.values())
+    n, rows, xs, xb = _samples(x)
+    _, _, ys, yb = _samples(y)
     C = x.shape[-1]
-    g = _per_channel(gate, C, "gate")
+    v = {k: t.contiguous() for k, t in v.items()}
+    m = _row_mask(tr[1], x.device) if tr is not None else None
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    stream = _stream_ptr(x.device)
     with torch.cuda.device(x.device):
-        if tr is None:
-            check(lib.jenga_gate_residual(x.data_ptr(), xs, y.data_ptr(), ys, g.data_ptr(), out.data_ptr(), C, rows,
-                                          C, _stream_ptr(x.device)), "gate_residual")
-            return out
-        tr_gate, mask = tr
-        _require_cuda(tr_gate)
-        tg = _per_channel(tr_gate, C, "tr_gate")
-        if mask.dim() != 1 or mask.numel() != rows:
-            raise ValueError("row mask must hold one entry per row")
-        m = _row_mask(mask, x.device)
-        check(lib.jenga_gate_residual_tr(x.data_ptr(), xs, y.data_ptr(), ys, g.data_ptr(), tg.data_ptr(), m.data_ptr(),
-                                         out.data_ptr(), C, rows, C, _stream_ptr(x.device)), "gate_residual_tr")
+        for b in range(n):
+            xp = x.data_ptr() + b * xb * x.element_size()
+            yp = y.data_ptr() + b * yb * y.element_size()
+            op = out.data_ptr() + b * rows * C * out.element_size()
+            g = _vec_ptr(v["gate"], b)
+            if tr is None:
+                check(lib.jenga_gate_residual(xp, xs, yp, ys, g, op, C, rows, C, stream), "gate_residual")
+            else:
+                check(lib.jenga_gate_residual_tr(xp, xs, yp, ys, g, _vec_ptr(v["tr_gate"], b), m.data_ptr(), op, C,
+                                                 rows, C, stream), "gate_residual_tr")
     return out
 
 
@@ -347,46 +417,31 @@ def linear_fp8_shape_ok(k: int, n: int) -> bool:
 
 
 def quantize_rows_fp8(x: torch.Tensor):
-    """x [..., K] bf16 (uniformly strided rows) -> (codes float8_e4m3fn [rows, K], scale fp32 [rows]):
-    scale = amax(row) / 448 (1 for a zero row), codes = e4m3_rn_satfinite(x / scale)."""
+    """x [..., K] bf16 (uniformly strided rows, or [B, L, K] with any batch stride) -> (codes
+    float8_e4m3fn [rows, K], scale fp32 [rows]): scale = amax(row) / 448 (1 for a zero row),
+    codes = e4m3_rn_satfinite(x / scale)."""
     _require_cuda(x)
     if x.dtype != torch.bfloat16:
         raise ValueError("x must be bf16")
-    rows, xs = _rows2d(x)
+    n, rows, xs, xb = _samples(x)
+    if n > 1 and xb % 8:
+        raise ValueError("batch stride must be a multiple of 8 elements")
     K = x.shape[-1]
-    out = torch.empty((rows, K), dtype=torch.float8_e4m3fn, device=x.device)
-    scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
+    out = torch.empty((n * rows, K), dtype=torch.float8_e4m3fn, device=x.device)
+    scale = torch.empty((n * rows,), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        check(lib.jenga_quantize_rows_fp8(x.data_ptr(), xs, rows, K, out.data_ptr(), K, scale.data_ptr(),
-                                          _stream_ptr(x.device)), "quantize_rows_fp8")
+        for b in range(n):
+            check(lib.jenga_quantize_rows_fp8(x.data_ptr() + b * xb * x.element_size(), xs, rows, K,
+                                              out.data_ptr() + b * rows * K, K,
+                                              scale.data_ptr() + b * rows * scale.element_size(),
+                                              _stream_ptr(x.device)), "quantize_rows_fp8")
     return out, scale
 
 
 def ln_modulate_fp8(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6, tr=None):
     """`quantize_rows_fp8(ln_modulate(x, shift, scale, eps, tr))` in one pass, bit for bit; the bf16 rows
-    are never written.  Returns (codes float8_e4m3fn [L, C], a_scale fp32 [L])."""
-    _require_cuda(x, shift, scale)
-    rows, xs = _rows2d(x)
-    C = x.shape[-1]
-    out = torch.empty((rows, C), dtype=torch.float8_e4m3fn, device=x.device)
-    a_scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
-    sc, sh = _per_channel(scale, C, "scale"), _per_channel(shift, C, "shift")
-    with torch.cuda.device(x.device):
-        if tr is None:
-            check(lib.jenga_ln_modulate_fp8(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(), C,
-                                            a_scale.data_ptr(), rows, C, float(eps), _stream_ptr(x.device)),
-                  "ln_modulate_fp8")
-            return out, a_scale
-        tr_shift, tr_scale, mask = tr
-        _require_cuda(tr_shift, tr_scale)
-        tsc, tsh = _per_channel(tr_scale, C, "tr_scale"), _per_channel(tr_shift, C, "tr_shift")
-        if mask.dim() != 1 or mask.numel() != rows:
-            raise ValueError("row mask must hold one entry per row")
-        m = _row_mask(mask, x.device)
-        check(lib.jenga_ln_modulate_tr_fp8(x.data_ptr(), xs, sc.data_ptr(), sh.data_ptr(), tsc.data_ptr(),
-                                           tsh.data_ptr(), m.data_ptr(), out.data_ptr(), C, a_scale.data_ptr(), rows,
-                                           C, float(eps), _stream_ptr(x.device)), "ln_modulate_tr_fp8")
-    return out, a_scale
+    are never written.  Returns (codes float8_e4m3fn [B*L, C], a_scale fp32 [B*L]), sample after sample."""
+    return _ln_modulate(x, shift, scale, eps, tr, fp8=True)
 
 
 def gelu_tanh_fp8(x: torch.Tensor):

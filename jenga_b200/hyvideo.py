@@ -130,6 +130,8 @@ def carved_attention_from_pools(q, k, v, pools, *, top_k: int, text_blocks: int 
     # pooled tensors cover all nb blocks; only the first n_img rows / columns are ranked
     bits = select_blocks(qp[:, :, :n_img].contiguous() if qp.shape[2] != n_img else qp, kp, n_img=n_img, nb=nb,
                          top_k=top_k, p_threshold=p_remain_rates, text_blocks=text_blocks, nbr_bits=nbr)
+    # sample 0's valid length, cu_seqlens_q[1], limits every sample's rows, as in the operator
+    # (attention_block_triton_diffres.py:328-329): exact for --num-videos, whose samples share one prompt
     seq = cu_seqlens_q[1:2].to(device=q.device, dtype=torch.int32) if cu_seqlens_q is not None else None
     if out is None:
         out = torch.empty_like(q)
