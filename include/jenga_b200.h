@@ -128,9 +128,11 @@ typedef struct JengaAttnArgs {
    * the same data movement with two all-to-alls after the kernel).  q/k/v hold this rank's
    * `heads` heads over the FULL sequence (image rows of all ranks in rank order, then the dense
    * text rows).  out_peers_host[r] (HOST array of sp_world device pointers, peer-mapped) is the
-   * base of rank r's result buffer [sp_rows + dense rows, sp_heads_total, D]; each output row is
-   * stored directly into its owner's buffer (image row t -> rank t / sp_rows; dense rows ->
-   * every rank, sp_world == 1 included), at heads [sp_rank*heads, (sp_rank+1)*heads).  Every
+   * base of rank r's result buffer [batch, sp_rows + T, sp_heads_total, D], T = q_rows -
+   * sp_world*sp_rows (the dense text rows; 0 when q_rows is shorter); each output row is stored
+   * directly into its owner's buffer (sample b's image row t -> rank t / sp_rows; its dense rows ->
+   * every rank, sp_world == 1 included), in sample b's slab, at heads [sp_rank*heads,
+   * (sp_rank+1)*heads).  Every
    * entry must be non-NULL and 16-byte aligned.  `out` is ignored and may be NULL.  The caller
    * synchronises the ranks before reading (jenga_b200.ulysses.UlyssesFusedAttention). */
   int32_t sp_world, sp_rank, sp_heads_total;
@@ -248,6 +250,21 @@ int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* args, void* stream);
  * [off[rank] + s).  With off[p] = p*heads/world the bytes written equal jenga_ulysses_scatter's. */
 int jenga_ulysses_scatter_ragged(const JengaUlyssesScatterArgs* args, const int32_t* head_offsets_host,
                                  void* stream);
+
+/* Batched form of both exchanges, one launch for `batch` samples: sample b reads x[w] + b*x_stride_b
+ * and joint[w] + b*joint_stride_b (element strides, multiples of 8), and every rank's receive buffer
+ * is [3, batch, world*n_loc + n_text, slots, head_dim]: sample b of q/k/v w starts at slab w*batch + b.
+ * head_offsets_host == NULL is the divisible split (jenga_ulysses_scatter's rules, slots =
+ * heads/world), otherwise the ragged one (jenga_ulysses_scatter_ragged's).  batch is 1..65535.  At
+ * batch 1 the bytes written equal those of the unbatched entry point, which is this call at batch 1. */
+typedef struct JengaUlyssesScatterBatchArgs {
+  JengaUlyssesScatterArgs base;
+  int32_t batch;
+  int64_t x_stride_b, joint_stride_b;
+} JengaUlyssesScatterBatchArgs;
+
+int jenga_ulysses_scatter_batched(const JengaUlyssesScatterBatchArgs* args, const int32_t* head_offsets_host,
+                                  void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Host <-> device staging for callers whose q/k/v live in (pinned) host memory: a strided 2-D

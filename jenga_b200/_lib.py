@@ -66,6 +66,11 @@ class JengaUlyssesScatterArgs(C.Structure):
     ]
 
 
+class JengaUlyssesScatterBatchArgs(C.Structure):
+    _fields_ = [("base", JengaUlyssesScatterArgs), ("batch", C.c_int32),
+                ("x_stride_b", C.c_int64), ("joint_stride_b", C.c_int64)]
+
+
 class JengaSelectArgs(C.Structure):
     _fields_ = [
         ("q_pool", C.c_void_p), ("k_pool", C.c_void_p), ("dtype", C.c_int32),
@@ -181,6 +186,8 @@ def _load() -> C.CDLL:
     lib.jenga_ulysses_scatter.restype = C.c_int
     lib.jenga_ulysses_scatter_ragged.argtypes = [C.POINTER(JengaUlyssesScatterArgs), C.c_void_p, C.c_void_p]
     lib.jenga_ulysses_scatter_ragged.restype = C.c_int
+    lib.jenga_ulysses_scatter_batched.argtypes = [C.POINTER(JengaUlyssesScatterBatchArgs), C.c_void_p, C.c_void_p]
+    lib.jenga_ulysses_scatter_batched.restype = C.c_int
     lib.jenga_block_neighbors_from_mapping_host.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int,
                                                             C.c_void_p, C.c_void_p]
     lib.jenga_block_neighbors_from_mapping_host.restype = C.c_int

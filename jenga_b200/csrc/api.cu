@@ -96,11 +96,13 @@ onehot_to_bits_kernel(const uint8_t* __restrict__ onehot, uint32_t* __restrict__
 // Ulysses inbound exchange: one pass over the local q,k,v, 16-byte stores into peer memory.
 // A call moves the local heads [hg0, hg0+hg) of EVERY destination rank's head group (hg == h_loc
 // moves everything); the head-group form lets the exchange of group g+1 run on a second stream
-// under the attention of group g.
+// under the attention of group g.  blockIdx.z is the sample: sample b reads x[w] + b*x_stride_bv and
+// lands in slab (w*batch + b) of the [3, batch, N+T, slots, D] buffers (batch 1: slab w).
 struct ScatterParams {
   const uint4* x[3];
   const uint4* joint[3];
   long long x_stride_v, joint_stride_v;  // uint4 units between tokens
+  long long x_stride_bv, joint_stride_bv;  // uint4 units between samples
   int world, rank, heads, vec_per_head;  // vec_per_head = head_dim*2/16
   int hg0, hg;                           // local head range of this call
   long long n_loc, n_text;
@@ -109,6 +111,9 @@ struct ScatterParams {
 __global__ void __launch_bounds__(256)
 ulysses_scatter_kernel(const ScatterParams p) {
   const int w = blockIdx.y;  // 0:q 1:k 2:v
+  const uint4* x = p.x[w] + blockIdx.z * p.x_stride_bv;
+  const uint4* joint = p.joint[w] + blockIdx.z * p.joint_stride_bv;
+  const long long slab = static_cast<long long>(w) * gridDim.z + blockIdx.z;   // [3, batch] slab of the buffers
   const int h_loc = p.heads / p.world;
   const int vec_per_tok = p.world * p.hg * p.vec_per_head;     // vectors this call moves per image token
   const long long n_total = static_cast<long long>(p.world) * p.n_loc + p.n_text;
@@ -125,9 +130,9 @@ ulysses_scatter_kernel(const ScatterParams p) {
       const int hl = p.hg0 + r / p.vec_per_head;               // local head at the destination
       const int v_in_head = r - (r / p.vec_per_head) * p.vec_per_head;
       const int head = dst_rank * h_loc + hl;                    // global head = column of x
-      const uint4 v = __ldg(p.x[w] + tok * p.x_stride_v + head * p.vec_per_head + v_in_head);
+      const uint4 v = __ldg(x + tok * p.x_stride_v + head * p.vec_per_head + v_in_head);
       uint4* dst = reinterpret_cast<uint4*>(p.peer[dst_rank]) +
-                   ((static_cast<long long>(w) * n_total + p.rank * p.n_loc + tok) * h_loc + hl) * p.vec_per_head +
+                   ((slab * n_total + p.rank * p.n_loc + tok) * h_loc + hl) * p.vec_per_head +
                    v_in_head;
       *dst = v;
     } else {
@@ -136,9 +141,9 @@ ulysses_scatter_kernel(const ScatterParams p) {
       const int r = static_cast<int>(k - tok * txt_per_tok);
       const int hl = p.hg0 + r / p.vec_per_head;
       const int v_in_head = r - (r / p.vec_per_head) * p.vec_per_head;
-      const uint4 v = __ldg(p.joint[w] + tok * p.joint_stride_v + (p.rank * h_loc + hl) * p.vec_per_head + v_in_head);
+      const uint4 v = __ldg(joint + tok * p.joint_stride_v + (p.rank * h_loc + hl) * p.vec_per_head + v_in_head);
       uint4* dst = reinterpret_cast<uint4*>(p.peer[p.rank]) +
-                   ((static_cast<long long>(w) * n_total + p.world * p.n_loc + tok) * h_loc + hl) * p.vec_per_head +
+                   ((slab * n_total + p.world * p.n_loc + tok) * h_loc + hl) * p.vec_per_head +
                    v_in_head;
       *dst = v;
     }
@@ -152,6 +157,7 @@ struct ScatterRaggedParams {
   const uint4* x[3];
   const uint4* joint[3];
   long long x_stride_v, joint_stride_v;
+  long long x_stride_bv, joint_stride_bv;
   int world, rank, slots, vec_per_head;
   int hg0;
   int off[9], cnt[8], cstart[9];   // cstart[world] = heads moved per image token
@@ -161,6 +167,9 @@ struct ScatterRaggedParams {
 __global__ void __launch_bounds__(256)
 ulysses_scatter_ragged_kernel(const ScatterRaggedParams p) {
   const int w = blockIdx.y;  // 0:q 1:k 2:v
+  const uint4* x = p.x[w] + blockIdx.z * p.x_stride_bv;
+  const uint4* joint = p.joint[w] + blockIdx.z * p.joint_stride_bv;
+  const long long slab = static_cast<long long>(w) * gridDim.z + blockIdx.z;   // [3, batch] slab of the buffers
   const int vec_per_tok = p.cstart[p.world] * p.vec_per_head;
   const long long n_total = static_cast<long long>(p.world) * p.n_loc + p.n_text;
   const long long img_vecs = p.n_loc * vec_per_tok;
@@ -177,9 +186,9 @@ ulysses_scatter_ragged_kernel(const ScatterRaggedParams p) {
       while (j >= p.cstart[dst_rank + 1]) ++dst_rank;
       const int slot = p.hg0 + (j - p.cstart[dst_rank]);
       const int head = p.off[dst_rank] + slot;                   // global head = column of x
-      const uint4 v = __ldg(p.x[w] + tok * p.x_stride_v + head * p.vec_per_head + v_in_head);
+      const uint4 v = __ldg(x + tok * p.x_stride_v + head * p.vec_per_head + v_in_head);
       uint4* dst = reinterpret_cast<uint4*>(p.peer[dst_rank]) +
-                   ((static_cast<long long>(w) * n_total + p.rank * p.n_loc + tok) * p.slots + slot) * p.vec_per_head +
+                   ((slab * n_total + p.rank * p.n_loc + tok) * p.slots + slot) * p.vec_per_head +
                    v_in_head;
       *dst = v;
     } else {
@@ -188,9 +197,9 @@ ulysses_scatter_ragged_kernel(const ScatterRaggedParams p) {
       const int r = static_cast<int>(k - tok * txt_per_tok);
       const int slot = p.hg0 + r / p.vec_per_head;
       const int v_in_head = r - (r / p.vec_per_head) * p.vec_per_head;
-      const uint4 v = __ldg(p.joint[w] + tok * p.joint_stride_v + (p.off[p.rank] + slot) * p.vec_per_head + v_in_head);
+      const uint4 v = __ldg(joint + tok * p.joint_stride_v + (p.off[p.rank] + slot) * p.vec_per_head + v_in_head);
       uint4* dst = reinterpret_cast<uint4*>(p.peer[p.rank]) +
-                   ((static_cast<long long>(w) * n_total + p.world * p.n_loc + tok) * p.slots + slot) * p.vec_per_head +
+                   ((slab * n_total + p.world * p.n_loc + tok) * p.slots + slot) * p.vec_per_head +
                    v_in_head;
       *dst = v;
     }
@@ -298,7 +307,9 @@ extern "C" int jenga_copy2d_async(void* dst, int64_t dst_pitch, const void* src,
   return ce == cudaSuccess ? JENGA_OK : set_cuda_error(ce, "cudaMemcpy2DAsync");
 }
 
-extern "C" int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* a, void* stream) {
+// The exchange of `batch` samples, the batch strides in elements (checked by the caller).
+static int ulysses_scatter_impl(const JengaUlyssesScatterArgs* a, int batch, int64_t x_stride_b,
+                                int64_t joint_stride_b, cudaStream_t stream) {
   if (!a || !a->x[0] || !a->x[1] || !a->x[2] || !a->peer_qkv_host)
     return set_error(JENGA_E_INVALID, "ulysses_scatter: null pointer");
   if (a->world <= 0 || a->world > 8 || a->rank < 0 || a->rank >= a->world || a->heads % a->world ||
@@ -316,6 +327,8 @@ extern "C" int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* a, void* str
   }
   p.x_stride_v = a->x_stride_s / 8;
   p.joint_stride_v = a->joint_stride_s / 8;
+  p.x_stride_bv = x_stride_b / 8;
+  p.joint_stride_bv = joint_stride_b / 8;
   p.world = a->world; p.rank = a->rank; p.heads = a->heads; p.vec_per_head = a->head_dim / 8;
   const int h_loc = a->heads / a->world;
   p.hg0 = a->head_count > 0 ? a->head_begin : 0;
@@ -326,13 +339,14 @@ extern "C" int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* a, void* str
   const long long total = (a->n_loc * a->world + a->n_text) * p.hg * p.vec_per_head;
   long long blocks = (total + 255) / 256;
   if (blocks > static_cast<long long>(kNumSMs) * 16) blocks = static_cast<long long>(kNumSMs) * 16;
-  dim3 grid(static_cast<unsigned>(blocks), 3);
-  ulysses_scatter_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  dim3 grid(static_cast<unsigned>(blocks), 3, static_cast<unsigned>(batch));
+  ulysses_scatter_kernel<<<grid, 256, 0, stream>>>(p);
   cudaError_t ce = cudaGetLastError();
   return ce == cudaSuccess ? JENGA_OK : set_cuda_error(ce, "ulysses_scatter launch");
 }
 
-extern "C" int jenga_ulysses_scatter_ragged(const JengaUlyssesScatterArgs* a, const int32_t* off, void* stream) {
+static int ulysses_scatter_ragged_impl(const JengaUlyssesScatterArgs* a, const int32_t* off, int batch,
+                                       int64_t x_stride_b, int64_t joint_stride_b, cudaStream_t stream) {
   if (!a || !off || !a->x[0] || !a->x[1] || !a->x[2] || !a->peer_qkv_host)
     return set_error(JENGA_E_INVALID, "ulysses_scatter_ragged: null pointer");
   if (a->world <= 0 || a->world > 8 || a->rank < 0 || a->rank >= a->world || a->heads <= 0 ||
@@ -361,6 +375,8 @@ extern "C" int jenga_ulysses_scatter_ragged(const JengaUlyssesScatterArgs* a, co
   }
   p.x_stride_v = a->x_stride_s / 8;
   p.joint_stride_v = a->joint_stride_s / 8;
+  p.x_stride_bv = x_stride_b / 8;
+  p.joint_stride_bv = joint_stride_b / 8;
   p.world = a->world; p.rank = a->rank; p.slots = slots; p.vec_per_head = a->head_dim / 8;
   p.hg0 = a->head_count > 0 ? a->head_begin : 0;
   const int hg = a->head_count > 0 ? a->head_count : slots;
@@ -380,10 +396,31 @@ extern "C" int jenga_ulysses_scatter_ragged(const JengaUlyssesScatterArgs* a, co
   if (total == 0) return JENGA_OK;
   long long blocks = (total + 255) / 256;
   if (blocks > static_cast<long long>(kNumSMs) * 16) blocks = static_cast<long long>(kNumSMs) * 16;
-  dim3 grid(static_cast<unsigned>(blocks), 3);
-  ulysses_scatter_ragged_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  dim3 grid(static_cast<unsigned>(blocks), 3, static_cast<unsigned>(batch));
+  ulysses_scatter_ragged_kernel<<<grid, 256, 0, stream>>>(p);
   cudaError_t ce = cudaGetLastError();
   return ce == cudaSuccess ? JENGA_OK : set_cuda_error(ce, "ulysses_scatter_ragged launch");
+}
+
+extern "C" int jenga_ulysses_scatter(const JengaUlyssesScatterArgs* a, void* stream) {
+  return ulysses_scatter_impl(a, 1, 0, 0, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int jenga_ulysses_scatter_ragged(const JengaUlyssesScatterArgs* a, const int32_t* off, void* stream) {
+  return ulysses_scatter_ragged_impl(a, off, 1, 0, 0, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int jenga_ulysses_scatter_batched(const JengaUlyssesScatterBatchArgs* a, const int32_t* off,
+                                             void* stream) {
+  if (!a) return set_error(JENGA_E_INVALID, "ulysses_scatter_batched: null pointer");
+  if (a->batch < 1 || a->batch > 65535)
+    return set_error(JENGA_E_INVALID, "ulysses_scatter_batched: batch %d must be 1..65535", a->batch);
+  if (a->x_stride_b % 8 || a->joint_stride_b % 8)
+    return set_error(JENGA_E_INVALID, "ulysses_scatter_batched: batch strides (%lld, %lld) must be multiples of 8",
+                     static_cast<long long>(a->x_stride_b), static_cast<long long>(a->joint_stride_b));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return off ? ulysses_scatter_ragged_impl(&a->base, off, a->batch, a->x_stride_b, a->joint_stride_b, st)
+             : ulysses_scatter_impl(&a->base, a->batch, a->x_stride_b, a->joint_stride_b, st);
 }
 
 extern "C" int64_t jenga_select_blocks_workspace_bytes(int32_t batch_heads, int32_t nq, int32_t n_img) {

@@ -224,17 +224,19 @@ carved_attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q,
     if (p.sp_world > 0) {
       // Fused Ulysses exchange (ref xdit_ring_atten.py:206-219 does this with two all-to-alls
       // after the kernel): image row t belongs to rank t / sp_rows; text rows go to every rank.
+      // Every owner's buffer is [batch, sp_rows + T, sp_heads_total, D]: sample b's rows sit in slab b.
       const long long n_img = p.sp_rows * p.sp_world;
+      const long long slab_rows = p.sp_rows + (p.q_rows > n_img ? p.q_rows - n_img : 0);
       const int gh = p.sp_head_base + h;
       if (q_row < n_img) {
         const int owner = static_cast<int>(q_row / p.sp_rows);
         obase = reinterpret_cast<uint16_t*>(p.peer_out[owner]);
-        o_off = ((q_row - owner * p.sp_rows) * p.sp_heads_total + gh) * kHeadDim;
+        o_off = ((b * slab_rows + q_row - owner * p.sp_rows) * p.sp_heads_total + gh) * kHeadDim;
       } else {
         // every rank's buffer; with one rank that is peer_out[0] through the single-store path
         obase = reinterpret_cast<uint16_t*>(p.peer_out[0]);
         n_dst = p.sp_world;
-        o_off = ((p.sp_rows + (q_row - n_img)) * p.sp_heads_total + gh) * kHeadDim;
+        o_off = ((b * slab_rows + p.sp_rows + (q_row - n_img)) * p.sp_heads_total + gh) * kHeadDim;
       }
     }
 #pragma unroll
@@ -393,7 +395,7 @@ int carved_attn_fwd_impl(const JengaAttnArgs* a, cudaStream_t stream, const Jeng
   }
   if (a->sp_world != 0 &&
       (a->sp_world < 0 || a->sp_world > 8 || a->sp_rank < 0 || a->sp_rank >= a->sp_world || !a->out_peers_host ||
-       a->sp_rows <= 0 || a->batch != 1 || a->out_dtype != a->dtype))
+       a->sp_rows <= 0 || a->out_dtype != a->dtype))
     return set_error(JENGA_E_INVALID, "bad Ulysses epilogue arguments");
   const int sp_head_base = a->sp_head_base_valid ? a->sp_head_base : a->sp_rank * a->heads;
   if (a->sp_world != 0 &&

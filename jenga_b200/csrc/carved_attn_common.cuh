@@ -27,7 +27,7 @@ struct KernelParams {
   long long o_stride_b, o_stride_s, o_stride_h;  // elements
   int out_f32;                // 1: write fp32 (values still rounded through the MMA dtype)
   // Ulysses fused epilogue (sp_world > 0): O rows are stored straight into the token owner's
-  // buffer over NVLink instead of `out`.  peer_out[r] = base of rank r's [sp_rows + dense rows,
+  // buffer over NVLink instead of `out`.  peer_out[r] = base of rank r's [batch, sp_rows + dense rows,
   // sp_heads_total, D] buffer; this rank's heads are [sp_rank*heads, (sp_rank+1)*heads).
   int sp_world, sp_rank, sp_heads_total;
   int sp_head_base;           // global head index of local head 0 (default sp_rank*heads)

@@ -36,14 +36,15 @@ check_degree = functools.partial(sharding.check_degree, model=MODEL)
 
 
 def get_cu_seqlens(text_mask: torch.Tensor, img_len: int, device) -> torch.Tensor:
-    """hyvideo_i2v/modules/attenion.py:34-57 for batch 1, on `device`: [0, valid text + img_len,
-    text + img_len].  Under SP img_len is the rank's image length (what my_parallel_attention
-    expects: it rebuilds the global table from it)."""
-    if text_mask.shape[0] != 1:
-        raise ValueError("sequence-parallel HunyuanVideo-I2V runs batch 1")
+    """hyvideo_i2v/modules/attenion.py:34-57 on `device`, without a host round trip: the 2B+1 entries
+    [0, valid_0 + img_len, max_len, max_len + valid_1 + img_len, 2 max_len, ...] with
+    max_len = text + img_len.  Under SP img_len is the rank's image length (what my_parallel_attention
+    expects: it rebuilds the global table from entry [1], which limits every sample)."""
+    max_len = text_mask.shape[1] + img_len
     s = text_mask.sum(dim=1).to(device=device, dtype=torch.int32) + img_len
-    return torch.cat([torch.zeros(1, dtype=torch.int32, device=device), s,
-                      torch.full((1,), text_mask.shape[1] + img_len, dtype=torch.int32, device=device)])
+    ends = torch.arange(1, len(s) + 1, dtype=torch.int32, device=device) * max_len
+    return torch.cat([torch.zeros(1, dtype=torch.int32, device=device),
+                      torch.stack([ends - max_len + s, ends], dim=1).reshape(-1)])
 
 
 def _step_calc(transformer):
@@ -84,8 +85,6 @@ def _forward_factory(group):
             if getattr(self, name, None) is None:
                 raise RuntimeError(f"sequence-parallel HunyuanVideo-I2V: transformer.{name} is not set "
                                    "(jenga_hyi2v.py sets the Jenga attributes before sampling)")
-        if x.shape[0] != 1:
-            raise ValueError("sequence-parallel HunyuanVideo-I2V runs batch 1")
         out = {}
         img, txt = x, text_states
         _, _, ot, oh, ow = x.shape
@@ -117,6 +116,7 @@ def _forward_factory(group):
         order = self.hilbert_order
         img = img[:, order]
         freqs_cos, freqs_sin = freqs_cos[order], freqs_sin[order]
+        # one first-frame mask, shared by every sample (as on the single-GPU path)
         first_frame_mask = torch.zeros_like(img[0, :, 0]).bool()                   # :124-126
         first_frame_mask[:th * tw] = 1
         first_frame_mask = first_frame_mask[order]

@@ -52,7 +52,7 @@ def shard_rows(L: int, world: int, rank: int, model: str) -> tuple[int, int]:
 
 
 def gather_rows(x: torch.Tensor, L: int, P: int, group) -> torch.Tensor:
-    """the [1, n, C] rows of every rank in rank order, then the first L"""
+    """the [B, n, C] rows of every rank in rank order along dim 1, then the first L"""
     if group is LOCAL:
         return x[:, :L]
     parts = [torch.empty_like(x) for _ in range(P)]

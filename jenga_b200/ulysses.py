@@ -254,14 +254,14 @@ class UlyssesFusedAttention:
     """Same contract as UlyssesCarvedAttention, with the exchange fused into the kernels over
     NVLink peer memory (torch symmetric memory provides the mapped pointers):
 
-      in : jenga_ulysses_scatter stores this rank's Q/K/V image rows into every rank's
-           [3, N+T, H/P, D] buffer with 16-byte peer stores — replaces three all-to-alls and their
+      in : jenga_ulysses_scatter_batched stores this rank's Q/K/V image rows into every rank's
+           [3, B, N+T, H/P, D] buffer with 16-byte peer stores — replaces three all-to-alls and their
            .contiguous() staging copies; text rows are a local head-slice copy.  The rank's H/P
            heads are processed as `groups` head sub-groups: the exchange of sub-group g+1 runs on
            a second stream UNDER the attention of sub-group g, so only the first sub-group's
            exchange is exposed.
       out: the attention kernel's epilogue stores each finished O row straight into the token
-           owner's [n_loc+T, H, D] buffer (text rows into every rank's) — replaces the
+           owner's [B, n_loc+T, H, D] buffer (text rows into every rank's) — replaces the
            all-to-all, the all-gather and the permute copies.  The result buffer is double
            buffered across calls (no copy out): the tensor returned by call i stays valid until
            call i+2 is issued on the same stream.
@@ -269,6 +269,13 @@ class UlyssesFusedAttention:
     after its exchange, one per call after the attention.  The operator's opt-in switches
     (attention.QK_INT8, attention.PV_FP8) apply: a sub-group's q, k, v are quantised on the main
     stream once its exchange is complete, and the next call's exchange waits for the main stream.
+
+    A batch of B samples runs as one exchange and one attention launch per sub-group: q/k/v are
+    [B, n, H, D] views with contiguous heads, one row stride and one batch stride (a multiple of 8
+    elements), the joint tensors likewise.  As in the reference wrapper and the single-GPU operator,
+    cu_seqlens_q[1] limits the text rows of every sample (exact when the samples share one prompt,
+    as --num-videos runs them).  Batch 1 uses the buffers [3, N+T, slots, D] and [n_loc+T, H, D];
+    B > 1 has its own, keyed by B.
 
     Ragged head split (ragged(H, P)): the qkv buffer has slots = ⌈H/P⌉ head slots on every rank (symmetric
     memory needs one shape), filled by jenga_ulysses_scatter_ragged; G comes from the slot count, so every
@@ -288,10 +295,13 @@ class UlyssesFusedAttention:
         self._side = None
         self._call = 0
 
-    def _buffers(self, N, T, h, D, n_loc, H, dtype, dev):
+    def _buffers(self, N, T, h, D, n_loc, H, dtype, dev, batch=1):
+        """(qkv, its handle, its peer array, two (result, handle, peer array)): qkv [3, N+T, h, D] and
+        results [n_loc+T, H, D] at batch 1, [3, batch, N+T, h, D] and [batch, n_loc+T, H, D] above"""
         import ctypes as C
         import torch.distributed._symmetric_memory as symm
-        key = (N, T, h, D, n_loc, H, dtype, str(dev))
+        key = (N, T, h, D, n_loc, H, dtype, str(dev), batch)
+        lead = (batch,) if batch > 1 else ()
         hit = self._bufs.get(key)
         if hit is not None:
             return hit
@@ -300,12 +310,12 @@ class UlyssesFusedAttention:
             symm.enable_symm_mem_for_group(self.group.group_name)
         except Exception:
             pass
-        qkv = symm.empty((3, N + T, h, D), dtype=dtype, device=dev)
+        qkv = symm.empty((3, *lead, N + T, h, D), dtype=dtype, device=dev)
         h_qkv = symm.rendezvous(qkv, self.group.group_name)
         p_qkv = (C.c_uint64 * P)(*[int(x) for x in h_qkv.buffer_ptrs])
         outs = []
         for _ in range(2):
-            out = symm.empty((n_loc + T, H, D), dtype=dtype, device=dev)
+            out = symm.empty((*lead, n_loc + T, H, D), dtype=dtype, device=dev)
             h_out = symm.rendezvous(out, self.group.group_name)
             outs.append((out, h_out, (C.c_uint64 * P)(*[int(x) for x in h_out.buffer_ptrs])))
         self._bufs[key] = (qkv, h_qkv, p_qkv, outs)
@@ -314,7 +324,7 @@ class UlyssesFusedAttention:
     @staticmethod
     def _n_groups(h: int, want: int | None, q_blocks: int | None = None) -> int:
         """Head sub-groups per rank.  Each sub-group is its own attention launch of
-        (h/G) * q_blocks CTAs, one per SM at a time on the 132 SMs of an H100: a launch of only a few
+        (h/G) * q_blocks CTAs (q_blocks: the query blocks of all samples of the launch), one per SM at a time on the 132 SMs of an H100: a launch of only a few
         waves pays its nearly empty last wave (902 CTAs = 6.8 waves run as 7), which costs more than
         the exposed exchange saves — so sub-groups are used only while every launch stays >= 12
         waves."""
@@ -338,8 +348,6 @@ class UlyssesFusedAttention:
         from .attention import _stream_ptr, block_sparse_attention_variant
         P, r = _group_size_rank(self.group)
         B, n, H, D = query.shape
-        if B != 1:
-            raise ValueError("the fused Ulysses path is built for batch 1 (what the pipelines run)")
         hooks = _hooks or {}
         off, h, b, slots = _layout(H, P, r)
         joint = joint_tensor_query is not None
@@ -351,34 +359,33 @@ class UlyssesFusedAttention:
         N = P * n
         L = _valid_rows(seq_len, N, n, T, dense, first_frame_blocks)
         dev, dt = query.device, query.dtype
-        qkv, h_qkv, p_qkv, outs = self._buffers(N, T, slots, D, n, H, dt, dev)
+        # batch 1 asks for the buffers with the eight arguments it always passed
+        bufs = self._buffers(N, T, slots, D, n, H, dt, dev, *((B,) if B > 1 else ()))
+        qkv, h_qkv, p_qkv, outs = bufs
         out, h_out, p_out = outs[self._call & 1]
         self._call += 1
-        # this rank's pad rows (global rows >= L): no rank stores them, so they are zeroed whenever the
-        # buffer is first used at this L
+        qkv, out = qkv.view(3, B, N + T, slots, D), out.view(B, n + T, H, D)
+        # this rank's pad rows (global rows >= L) of every sample: no rank stores them, so they are
+        # zeroed whenever the buffer is first used at this L
         pad0 = min(n, max(0, L - r * n))
         if self._pad_len.get(out.data_ptr(), N) != L and pad0 < n:
-            out[pad0:n].zero_()
+            out[:, pad0:n].zero_()
         self._pad_len[out.data_ptr()] = L
         # the same G on every rank, from the slot count: every rank issues every scatter and barrier
-        G = self._n_groups(slots, self.groups, (L + T + BLOCK - 1) // BLOCK)
+        G = self._n_groups(slots, self.groups, B * ((L + T + BLOCK - 1) // BLOCK))
         hg = slots // G
-        xs = [t[0] for t in (query, key, value)]
-        for t in xs:
-            if t.stride(2) != 1 or t.stride(1) != D or t.stride(0) != xs[0].stride(0):
-                raise ValueError("q/k/v must be [1, n, H, D] views with contiguous heads and one row stride")
-        a = _lib.JengaUlyssesScatterArgs()
-        a.x = (C.c_void_p * 3)(*[t.data_ptr() for t in xs])
-        a.x_stride_s = xs[0].stride(0)
+        a = _lib.JengaUlyssesScatterBatchArgs()
+        a.batch = B
+        a.x_stride_b = _batch_strides((query, key, value), "q/k/v", B, D)
+        a.base.x = (C.c_void_p * 3)(*[t.data_ptr() for t in (query, key, value)])
+        a.base.x_stride_s = query.stride(1)
         if joint:
-            js = [t[0] for t in (joint_tensor_query, joint_tensor_key, joint_tensor_value)]
-            for t in js:
-                if t.stride(2) != 1 or t.stride(1) != D:
-                    raise ValueError("joint tensors must be [1, T, H, D] views with contiguous heads")
-            a.joint = (C.c_void_p * 3)(*[t.data_ptr() for t in js])
-            a.joint_stride_s = js[0].stride(0)
-        a.world, a.rank, a.heads, a.head_dim, a.n_loc, a.n_text = P, r, H, D, n, T
-        a.peer_qkv_host = C.addressof(p_qkv)
+            js = (joint_tensor_query, joint_tensor_key, joint_tensor_value)
+            a.joint_stride_b = _batch_strides(js, "joint tensors", B, D)
+            a.base.joint = (C.c_void_p * 3)(*[t.data_ptr() for t in js])
+            a.base.joint_stride_s = js[0].stride(1)
+        a.base.world, a.base.rank, a.base.heads, a.base.head_dim, a.base.n_loc, a.base.n_text = P, r, H, D, n, T
+        a.base.peer_qkv_host = C.addressof(p_qkv)
         c_off = None if off is None else (C.c_int32 * (P + 1))(*off)
         main = torch.cuda.current_stream(dev)
         if self._side is None:
@@ -391,12 +398,8 @@ class UlyssesFusedAttention:
             for g in range(G):
                 if "pre_scatter" in hooks:
                     hooks["pre_scatter"](g, side)
-                a.head_begin, a.head_count = g * hg, hg
-                if c_off is None:
-                    check(lib.jenga_ulysses_scatter(C.byref(a), _stream_ptr(dev)), "ulysses_scatter")
-                else:
-                    check(lib.jenga_ulysses_scatter_ragged(C.byref(a), c_off, _stream_ptr(dev)),
-                          "ulysses_scatter_ragged")
+                a.base.head_begin, a.base.head_count = g * hg, hg
+                check(lib.jenga_ulysses_scatter_batched(C.byref(a), c_off, _stream_ptr(dev)), "ulysses_scatter_batched")
                 if "post_scatter" in hooks:
                     hooks["post_scatter"](g, side)
                 h_qkv.barrier(channel=0)
@@ -416,7 +419,7 @@ class UlyssesFusedAttention:
             sl = slice(g * hg, min((g + 1) * hg, h))
             if sl.start < sl.stop:      # a short ragged group may own no head of this slot range
                 sp = dict(world=P, rank=r, heads_total=H, rows=n, peers=p_out, head_base=b + g * hg)
-                q, k, v = (x[None, :L + T, sl] for x in qkv)       # all N + T rows without seq_len
+                q, k, v = (x[:, :L + T, sl] for x in qkv)       # all N + T rows without seq_len
                 if dense:
                     # flash_attn_shim._dense's launch, with the peer-store epilogue instead of `out`
                     v8, qk8 = A.quantize_operands(q, k, v, A.PV_FP8, A.QK_INT8)
@@ -434,7 +437,7 @@ class UlyssesFusedAttention:
                 hooks["post_attention"](g, main, out, hg)
         if "post_attention" not in hooks:
             h_out.barrier(channel=0)
-        return out[None]
+        return out
 
     def plan(self, heads_per_rank: int, tokens: int | None = None) -> tuple[int, int]:
         """(groups, heads per group) this object will use for `heads_per_rank` heads over `tokens`
@@ -542,6 +545,20 @@ class HostPipelinedUlysses:
         if wait:
             main.wait_stream(self.s_out)
         return hout
+
+
+def _batch_strides(ts, what, B, D) -> int:
+    """The one batch stride of the [B, rows, H, D] views `ts` (contiguous heads, one row stride);
+    ValueError for any other layout"""
+    sb, ss = ts[0].stride(0), ts[0].stride(1)
+    for t in ts:
+        if t.dim() != 4 or t.shape[0] != B or t.stride(3) != 1 or t.stride(2) != D or t.stride(1) != ss or \
+                (B > 1 and t.stride(0) != sb):
+            raise ValueError(f"{what} must be [B, rows, H, D] views with contiguous heads, one row stride and "
+                             "one batch stride")
+    if B > 1 and sb % 8:
+        raise ValueError(f"{what}: the batch stride {sb} is not a multiple of 8 elements")
+    return sb if B > 1 else 0
 
 
 def my_parallel_attention(hybrid_seq_parallel_attn, q, k, v, img_q_len, img_kv_len, cu_seqlens_q,
