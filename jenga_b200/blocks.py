@@ -22,10 +22,10 @@ followed by select_blocks + the carved-attention launch.  Everything around the 
 section (modulation, linear layers, gates, MLP) is executed by the block's own sub-modules and
 the reference module's own helper functions (`modulate`, `apply_gate`), so those numerics are the
 reference's by construction.  Whenever a call is not the carved configuration (sa_drop_rate == 0,
-no RMS qk-norm, unusual dtype, batch > 1 for Wan, the reference's own sequence parallel for I2V, …) the
-ORIGINAL forward runs, with the caller's own arguments (`_patched`).  An I2V block with `jenga_sp` set
-(the Hilbert-sharded forward of hyi2v_sp.py) routes its attention section through that Ulysses object
-and has no such fall-back; so does a WanSelfAttention with `jenga_sp` set (the Hilbert-sharded Wan
+no RMS qk-norm, unusual dtype, Wan samples on several latent grids, the reference's own sequence
+parallel for I2V, …) the ORIGINAL forward runs, with the caller's own arguments (`_patched`).  An I2V
+block with `jenga_sp` set (the Hilbert-sharded forward of hyi2v_sp.py) routes its attention section
+through that Ulysses object and has no such fall-back; so does a WanSelfAttention with `jenga_sp` set (the Hilbert-sharded Wan
 forward of wan_sp.py), whose carved and dense calls both go through the exchange; and so does a
 plain-module WanSelfAttention under `jenga_sp` (the raster-sharded I2V forward of wan_sp.py), whose
 block then runs the fused I2V cross-attention on the rank's rows or raises.
@@ -476,9 +476,25 @@ def _wan_rms(norm) -> bool:
 
 
 def _wan_self_ok(self, x, per_block_tokens=128) -> bool:
-    """the WanSelfAttention call _wan_self_fused takes, the Linears' output dtypes aside"""
-    return (x.is_cuda and x.shape[0] == 1 and self.head_dim == 128 and per_block_tokens == 128
+    """the WanSelfAttention call _wan_self_fused takes, the Linears' output dtypes and the grid aside:
+    any batch (every sample on one latent grid, _one_grid)"""
+    return (x.is_cuda and self.head_dim == 128 and per_block_tokens == 128
             and _wan_rms(self.norm_q) and _wan_rms(self.norm_k))
+
+
+def _one_grid(grid_sizes) -> bool:
+    """every sample of the call on one latent grid: the fused self-attention reads grid_sizes[0] for all of
+    them, as teacache_forward gathers every sample with the one curve (jenga_wan.py:559)"""
+    return (isinstance(grid_sizes, torch.Tensor) and grid_sizes.dim() == 2 and grid_sizes.shape[0] >= 1
+            and bool((grid_sizes == grid_sizes[:1]).all()))
+
+
+def _check_one_grid(grid_sizes, what: str) -> None:
+    """_one_grid, or the ValueError of a route without a fall-back"""
+    if not _one_grid(grid_sizes):
+        rows = grid_sizes.tolist() if isinstance(grid_sizes, torch.Tensor) else grid_sizes
+        raise ValueError(f"{what}: the samples of one call must share one latent grid (one curve and one RoPE "
+                         f"grid for all); got grid_sizes {rows}")
 
 
 def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tokens, p_remain_rates, freq_remap,
@@ -491,14 +507,19 @@ def _wan_self_fused(self, jsp, x, grid_sizes, freqs, sa_drop_rate, per_block_tok
     shim's launch.  top_k and first_frame_blocks follow the single-GPU rule over L (model_mul.py:161-164);
     sa_drop_rate <= 0.25 (:153, the warm-up steps) is a dense call.  freq_remap: the RoPE row of each row
     (None: raster, one GPU only).  stats: the STATS keys of a carved and of a dense call.  x8: see _wan_qkv.
+    x may hold several samples [B, n, C] on one latent grid (grid_sizes rows all equal): the prologue and
+    the attention take the batch, and freq_remap is shared by every sample.
     A call it does not take raises, except with `fallback` (the one-GPU carved route of model_mul.py), where
-    a q Linear dtype the prologue does not take returns None for the original forward, and v goes to the
-    operator as the v Linear returns it (the operator casts it)."""
+    samples on different grids and a q Linear dtype the prologue does not take return None for the
+    original forward, and v goes to the operator as the v Linear returns it (the operator casts it)."""
     b, n = x.shape[:2]
     if not _wan_self_ok(self, x, per_block_tokens) or (jsp is not None and freq_remap is None):
         raise RuntimeError(f"{type(self).__name__}: the call is not one the fused Wan self-attention takes (a "
-                           "CUDA batch-1 input, head_dim 128, 128-token blocks, WanRMSNorm q / k norms with "
+                           "CUDA input, head_dim 128, 128-token blocks, WanRMSNorm q / k norms with "
                            "weights and, under jenga_sp, a freq_remap); this route has no fall-back")
+    if fallback and not _one_grid(grid_sizes):
+        return None
+    _check_one_grid(grid_sizes, type(self).__name__)
     q_lin, k_lin, v = _wan_qkv(self, x, x8)
     if fallback:
         if q_lin.dtype not in (torch.bfloat16, torch.float32):
@@ -608,12 +629,13 @@ def _wan_i2v_self_takes(self, x, sa_drop_rate=None, freq_remap=None, **_):
 
 
 def _wan_cross_takes(self, x, context, context_lens):
-    """True when _wan_cross runs the fused T2V cross-attention (the Linears' output dtypes aside)"""
+    """True when _wan_cross runs the fused T2V cross-attention (the Linears' output dtypes aside): x
+    [B, L, C] and context [B, Lc, C] of one batch, each sample attending its own context rows"""
     # context_lens: the reference's varlen form (wan/modules/attention.py:69-80); teacache_forward
     # passes None (jenga_wan.py:569)
-    return (context_lens is None and x.is_cuda and x.dim() == 3 and x.shape[0] == 1 and context.dim() == 3
-            and context.shape[0] == 1 and self.head_dim == 128 and _wan_rms(self.norm_q) and _wan_rms(self.norm_k)
-            and DN._autocast_bf16())
+    return (context_lens is None and x.is_cuda and x.dim() == 3 and context.dim() == 3
+            and context.shape[0] == x.shape[0] and DN.distinct_samples(x, context) and self.head_dim == 128
+            and _wan_rms(self.norm_q) and _wan_rms(self.norm_k) and DN._autocast_bf16())
 
 
 def _wan_cross(self, x, context, context_lens, *, jenga_x8=None):
@@ -629,20 +651,21 @@ def _wan_cross(self, x, context, context_lens, *, jenga_x8=None):
             raise RuntimeError(f"{type(self).__name__}: k / v Linears return {k_lin.dtype} / {v.dtype} under bf16 "
                                "autocast; the e4m3 q input has no fall-back")
         return None
-    out = WAN.cross_attention(q_lin, k_lin, v.view(1, -1, self.num_heads, self.head_dim),
+    out = WAN.cross_attention(q_lin, k_lin, v.view(x.shape[0], -1, self.num_heads, self.head_dim),
                               self.norm_q.weight, self.norm_k.weight, self.num_heads, eps=float(self.norm_q.eps))
     STATS["wan_cross"] += 1
     return _linear(self.o, out.flatten(2))
 
 
 def _wan_i2v_cross_shape_ok(ca, x, context, context_lens):
-    """the I2V cross-attention configuration the fused kernel takes, device and autocast aside: one
-    sample, every context row valid (teacache_forward passes context_lens=None, jenga_wan.py:569),
-    head_dim 128, WanRMSNorm q / k / k_img norms with weights and one eps, and text rows after the
-    image rows"""
+    """the I2V cross-attention configuration the fused kernel takes, device and autocast aside: a context
+    of x's batch, each sample attending its own context rows, every one valid (teacache_forward passes
+    context_lens=None, jenga_wan.py:569), head_dim 128, WanRMSNorm q / k / k_img norms with weights and one
+    eps, and text rows after the image rows"""
     norms = [getattr(ca, n, None) for n in ("norm_q", "norm_k", "norm_k_img")]
     return (context_lens is None and isinstance(x, torch.Tensor) and isinstance(context, torch.Tensor)
-            and x.dim() == 3 and x.shape[0] == 1 and context.dim() == 3 and context.shape[0] == 1
+            and x.dim() == 3 and context.dim() == 3 and context.shape[0] == x.shape[0]
+            and DN.distinct_samples(x, context)
             and context.shape[1] > _WAN_I2V_IMG_TOKENS and getattr(ca, "head_dim", None) == 128
             and all(_wan_rms(n) for n in norms)
             and len({float(n.eps) for n in norms}) == 1)
@@ -667,8 +690,8 @@ def _wan_i2v_cross(ca, x, context, context_lens, stat="wan_i2v_cross", x8=None):
         kimg_lin, vimg = ca.k_img(ctx_img), ca.v_img(ctx_img)
         lin_ok = all(t.dtype in (torch.bfloat16, torch.float32) for t in (q_lin, k_lin, kimg_lin))
         if lin_ok and v.dtype == vimg.dtype == torch.bfloat16:
-            n = ca.num_heads
-            out = WAN.i2v_cross_attention(q_lin, k_lin, v.view(1, -1, n, 128), kimg_lin, vimg.view(1, -1, n, 128),
+            b, n = x.shape[0], ca.num_heads
+            out = WAN.i2v_cross_attention(q_lin, k_lin, v.view(b, -1, n, 128), kimg_lin, vimg.view(b, -1, n, 128),
                                           ca.norm_q.weight, ca.norm_k.weight, ca.norm_k_img.weight, n,
                                           eps=float(ca.norm_q.eps))
             STATS[stat] += 1
@@ -689,17 +712,22 @@ def _wan_block(plain, self, x, e, seq_lens, grid_sizes, freqs, context, context_
       under `self_attn.jenga_sp` (parallelize_wan_i2v) x is a rank's rows and there is no fall-back: the
       checks run before the exchange, so every rank raises alike;
       with the Jenga arguments, the original forward runs on raster rows, in model.py's own signature, and
-      the block raises on curve-ordered rows (freq_remap set), whose RoPE positions it does not know."""
+      the block raises on curve-ordered rows (freq_remap set), whose RoPE positions it does not know.
+    x may hold several samples [B, L, C] with `e` [B, 6, C] (or [1, 6, C], shared) and a context of the same
+    batch; all of them on one latent grid.  Samples on different grids run the original forward, or raise
+    ValueError where there is none (the sharded rows, the curve-ordered rows)."""
     attn_kw = {} if plain and sa_drop_rate is None else dict(
         sa_drop_rate=sa_drop_rate, freq_remap=freq_remap, block_neighbor_list=block_neighbor_list,
         p_remain_rates=p_remain_rates)
     sharded = plain and getattr(self.self_attn, "jenga_sp", None) is not None
+    if sharded or (plain and freq_remap is not None):
+        _check_one_grid(grid_sizes, type(self).__name__)
     if sharded and not (type(self.cross_attn).__name__ == "WanI2VCrossAttention"
                         and _wan_i2v_cross_shape_ok(self.cross_attn, x, context, context_lens)):
         raise RuntimeError(f"{type(self).__name__} under jenga_sp: the cross-attention is not one the fused I2V "
                            "kernel takes (a WanI2VCrossAttention with WanRMSNorm q / k / k_img norms, head_dim "
-                           f"128, batch 1, context_lens None and more than {_WAN_I2V_IMG_TOKENS} context rows); "
-                           "the sharded I2V forward has no fall-back")
+                           f"128, a context of x's batch, context_lens None and more than {_WAN_I2V_IMG_TOKENS} "
+                           "context rows); the sharded I2V forward has no fall-back")
     out = _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens, attn_kw, sharded)
     if out is None and sharded:
         raise RuntimeError(f"{type(self).__name__} under jenga_sp: the call is not one the fused block takes (a "
@@ -721,7 +749,7 @@ def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_le
     sharded: the I2V rows of parallelize_wan_i2v; the cross-attention must then be the fused one."""
     i2v = type(self.cross_attn).__name__ == "WanI2VCrossAttention"
     ok = (isinstance(e, torch.Tensor) and e.dtype == torch.float32 and x.is_cuda and x.dim() == 3
-          and (i2v or type(self.cross_attn).__name__ == "WanT2VCrossAttention")
+          and _one_grid(grid_sizes) and (i2v or type(self.cross_attn).__name__ == "WanT2VCrossAttention")
           and self.modulation.dtype == torch.float32
           and (not sharded or wan_i2v_cross_eligible(self.cross_attn, x, context, context_lens)))
     if ok:
@@ -732,7 +760,7 @@ def _wan_block_body(self, x, e, seq_lens, grid_sizes, freqs, context, context_le
               and DN.wan_residual_ln_supported(x, self.norm2, e6, affine=False)
               and DN.wan_gate_residual_supported(x, e6))
     if not ok:
-        return None                     # no autocast, batch > 1, cross_attn_norm=False (norm3 is Identity), …
+        return None                     # no autocast, several grids, cross_attn_norm=False (norm3 is Identity), …
     e = e6.chunk(6, dim=1)
     # self-attention on the bf16 its q / k / v Linears would cast the fp32 modulate output to; with the
     # FP8 Linears routing q / k / v, on the e4m3 rows of that bf16 instead (:331-333)

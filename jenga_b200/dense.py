@@ -16,7 +16,9 @@ call; a token-replace row mask has one entry per row of a sample and is shared b
 
 The `wan_*` functions are the chains of Wan2.1's WanAttentionBlock.forward
 (wan/modules/model_mul.py:326-346), whose residual stream is fp32 and whose modulation vectors are
-the fp32 rows of `e` [1, 6, C]."""
+the fp32 rows of `e` [B, 6, C] (one row per sample, as `t` [B] makes them) or [1, 6, C] (shared by
+every sample).  They take several samples the same way: sample b runs the batch-1 launch on its rows
+with its vector row, so its result is bit-identical to that call."""
 from __future__ import annotations
 
 import weakref
@@ -75,13 +77,6 @@ def _row_mask(mask: torch.Tensor, device: torch.device) -> torch.Tensor:
         _MASK_CACHE.clear()
     _MASK_CACHE[key] = (weakref.ref(mask), dev)
     return dev
-
-
-def _per_channel(v: torch.Tensor, C: int, what: str) -> torch.Tensor:
-    v = v.reshape(-1).contiguous()
-    if v.numel() != C:
-        raise ValueError(f"{what} must hold one value per channel (batch 1)")
-    return v
 
 
 def _samples(x: torch.Tensor):
@@ -241,13 +236,21 @@ def _autocast_bf16() -> bool:
     return torch.is_autocast_enabled() and torch.get_autocast_dtype("cuda") == torch.bfloat16
 
 
+def distinct_samples(*ts: torch.Tensor) -> bool:
+    """each tensor holds one sample, or a batch of samples of their own (batch stride non-zero): an
+    expanded batch (stride 0) is one sample seen B times, which the fused Wan path does not take"""
+    return all(t.shape[0] == 1 or t.stride(0) != 0 for t in ts)
+
+
 def _wan_rows_ok(x: torch.Tensor, e: torch.Tensor) -> bool:
-    """x [1, L, C] bf16 or fp32 on a GPU with 8-aligned rows, e the fp32 [1, 6, C] modulation sum"""
+    """x [B, L, C] bf16 or fp32 on a GPU with 8-aligned rows and distinct, 8-aligned sample starts, e the
+    fp32 modulation sum [B, 6, C] (one row per sample) or [1, 6, C] (shared by every sample)"""
     return (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype in (torch.bfloat16, torch.float32)
-            and x.dim() == 3 and x.shape[0] == 1 and x.shape[-1] % 8 == 0 and x.shape[-1] <= 6144
+            and x.dim() == 3 and x.shape[-1] % 8 == 0 and x.shape[-1] <= 6144
             and x.stride(-1) == 1 and x.stride(-2) % 8 == 0
-            and isinstance(e, torch.Tensor) and e.is_cuda and e.dtype == torch.float32
-            and tuple(e.shape) == (1, 6, x.shape[-1]) and _autocast_bf16())
+            and (x.shape[0] == 1 or (x.stride(0) % 8 == 0 and distinct_samples(x)))
+            and isinstance(e, torch.Tensor) and e.is_cuda and e.dtype == torch.float32 and e.dim() == 3
+            and tuple(e.shape[1:]) == (6, x.shape[-1]) and e.shape[0] in (1, x.shape[0]) and _autocast_bf16())
 
 
 def _wan_layer_norm(norm, affine: bool) -> bool:
@@ -275,18 +278,35 @@ def wan_gate_residual_supported(x: torch.Tensor, e: torch.Tensor) -> bool:
     return _wan_rows_ok(x, e)
 
 
-def _wan_vec(v: torch.Tensor, C: int, what: str) -> torch.Tensor:
+def _wan_vecs(x: torch.Tensor, vecs: dict) -> dict:
+    """_sample_vecs for the Wan chains, whose optional vectors may be None: each one holds C values,
+    shared by every sample, or one row of C values per sample of x [B, L, C] (a [B, 1, C] view of
+    `e6.chunk(6, dim=1)`, batch stride 6*C).  -> name -> [1, C] or [B, C] view, or None."""
+    out = _sample_vecs(x, {k: v for k, v in vecs.items() if v is not None})
+    return {k: out.get(k) for k in vecs}
+
+
+def _wan_vec(v: torch.Tensor | None, what: str) -> torch.Tensor | None:
+    """a [1, C] / [B, C] view of _wan_vecs on the GPU, fp32, with contiguous channels"""
+    if v is None:
+        return None
     _require_cuda(v)
     if v.dtype != torch.float32:
         raise ValueError(f"{what} must be fp32")
-    return _per_channel(v, C, what)
+    return v if v.stride(-1) == 1 else v.contiguous()
 
 
-def _wan_y(x: torch.Tensor, y: torch.Tensor):
-    _require_cuda(y)
-    if y.dtype != torch.bfloat16 or y.shape != x.shape:
+def _wan_samples(x: torch.Tensor, y: torch.Tensor | None = None):
+    """(samples, rows per sample, x row stride, x batch stride, y row stride, y batch stride) of the Wan
+    residual stream x — [B, L, C], B samples launched one by one at 8-element aligned starts, or at B = 1
+    uniformly strided rows — and of y, bf16 shaped like x (None: y strides 0)"""
+    if y is not None and (y.dtype != torch.bfloat16 or y.shape != x.shape):
         raise ValueError("y must be a bf16 tensor shaped like x")
-    return _rows2d(y)[1]
+    n, rows, xs, xb = _samples(x)
+    ys, yb = _samples(y)[2:] if y is not None else (0, 0)
+    if n > 1 and (xb % 8 or yb % 8):
+        raise ValueError("the batch stride of x and y must be a multiple of 8 elements")
+    return n, rows, xs, xb, ys, yb
 
 
 def _x_code(x: torch.Tensor) -> int:
@@ -296,16 +316,22 @@ def _x_code(x: torch.Tensor) -> int:
     return codes[x.dtype]
 
 
+def _at(t: torch.Tensor, elems: int) -> int:
+    """address `elems` elements past t's start"""
+    return t.data_ptr() + elems * t.element_size()
+
+
 def wan_ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6) -> torch.Tensor:
     """`norm1(x).float() * (1 + scale) + shift` (model_mul.py:331-333, WanLayerNorm :98-103) followed by
-    the bf16 cast the q / k / v Linears apply under autocast.  x [1, L, C] bf16 or fp32, shift / scale
-    fp32 with C values (e[0] / e[1]) -> [1, L, C] bf16."""
+    the bf16 cast the q / k / v Linears apply under autocast.  x [B, L, C] bf16 or fp32, shift / scale
+    fp32 with C values (e[0] / e[1] of a [1, 6, C] e) or one row of them per sample (of a [B, 6, C] e)
+    -> [B, L, C] bf16.  Sample b runs the batch-1 launch on its rows with its vector row."""
     return _wan_ln_modulate(x, shift, scale, eps, fp8=False)
 
 
 def wan_ln_modulate_fp8(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, eps: float = 1e-6):
     """`quantize_rows_fp8(wan_ln_modulate(x, shift, scale, eps))` in one pass, bit for bit; the bf16 rows
-    are never written.  Returns (codes float8_e4m3fn [L, C], a_scale fp32 [L])."""
+    are never written.  Returns (codes float8_e4m3fn [B*L, C], a_scale fp32 [B*L]), sample after sample."""
     return _wan_ln_modulate(x, shift, scale, eps, fp8=True)
 
 
@@ -315,21 +341,26 @@ def _fp8_rows(rows: int, C: int, device):
 
 
 def _wan_ln_modulate(x, shift, scale, eps, fp8):
+    v = _wan_vecs(x, {"scale": scale, "shift": shift})
+    n, rows, xs, xb, _, _ = _wan_samples(x)
     _require_cuda(x)
-    rows, xs = _rows2d(x)
     C = x.shape[-1]
-    sc, sh = _wan_vec(scale, C, "scale"), _wan_vec(shift, C, "shift")
-    with torch.cuda.device(x.device):
-        if fp8:
-            out, a_scale = _fp8_rows(rows, C, x.device)
-            check(lib.jenga_wan_ln_modulate_fp8(x.data_ptr(), _x_code(x), xs, sc.data_ptr(), sh.data_ptr(),
-                                                out.data_ptr(), C, a_scale.data_ptr(), rows, C, float(eps),
-                                                _stream_ptr(x.device)), "wan_ln_modulate_fp8")
-            return out, a_scale
+    sc, sh = _wan_vec(v["scale"], "scale"), _wan_vec(v["shift"], "shift")
+    if fp8:
+        out, a_scale = _fp8_rows(n * rows, C, x.device)
+    else:
         out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-        check(lib.jenga_wan_ln_modulate(x.data_ptr(), _x_code(x), xs, sc.data_ptr(), sh.data_ptr(), out.data_ptr(),
-                                        C, rows, C, float(eps), _stream_ptr(x.device)), "wan_ln_modulate")
-    return out
+    with torch.cuda.device(x.device):
+        for b in range(n):
+            xp, op = _at(x, b * xb), _at(out, b * rows * C)
+            if fp8:
+                check(lib.jenga_wan_ln_modulate_fp8(xp, _x_code(x), xs, _vec_ptr(sc, b), _vec_ptr(sh, b), op, C,
+                                                    _at(a_scale, b * rows), rows, C, float(eps),
+                                                    _stream_ptr(x.device)), "wan_ln_modulate_fp8")
+            else:
+                check(lib.jenga_wan_ln_modulate(xp, _x_code(x), xs, _vec_ptr(sc, b), _vec_ptr(sh, b), op, C, rows,
+                                                C, float(eps), _stream_ptr(x.device)), "wan_ln_modulate")
+    return (out, a_scale) if fp8 else out
 
 
 def wan_residual_ln(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor | None, eps: float = 1e-6, *,
@@ -338,7 +369,8 @@ def wan_residual_ln(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor | None,
     """r = x + y * gate (gate None: x + y), then the next LayerNorm of r as the following Linear sees it.
     weight / bias: `norm3(r)`, the affine WanLayerNorm (gate 1 + norm3, model_mul.py:334-339).
     shift / scale: `norm2(r).float() * (1 + scale) + shift` (cross residual + norm2, :339-340).
-    x [1, L, C] bf16 or fp32, y bf16 like x -> (r fp32 [1, L, C], normed bf16 [1, L, C])."""
+    x [B, L, C] bf16 or fp32, y bf16 like x -> (r fp32 [B, L, C], normed bf16 [B, L, C]).  gate, shift
+    and scale hold C values or one row of them per sample (wan_ln_modulate); weight and bias C values."""
     return _wan_residual_ln(x, y, gate, eps, weight, bias, shift, scale, fp8=False)
 
 
@@ -346,51 +378,59 @@ def wan_residual_ln_fp8(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor | N
                         weight: torch.Tensor | None = None, bias: torch.Tensor | None = None,
                         shift: torch.Tensor | None = None, scale: torch.Tensor | None = None):
     """wan_residual_ln with the normed rows quantised as quantize_rows_fp8 does, in the same pass and bit
-    for bit; r is the same fp32 residual.  -> (r fp32 [1, L, C], (codes float8_e4m3fn [L, C], a_scale [L]))."""
+    for bit; r is the same fp32 residual.  -> (r fp32 [B, L, C], (codes float8_e4m3fn [B*L, C],
+    a_scale [B*L])), sample after sample."""
     return _wan_residual_ln(x, y, gate, eps, weight, bias, shift, scale, fp8=True)
 
 
 def _wan_residual_ln(x, y, gate, eps, weight, bias, shift, scale, fp8):
-    _require_cuda(x)
-    rows, xs = _rows2d(x)
-    ys = _wan_y(x, y)
-    C = x.shape[-1]
     affine = weight is not None
     if affine == (scale is not None) or (bias is None) != (weight is None) or (shift is None) != (scale is None):
         raise ValueError("pass either weight and bias or shift and scale")
-    va = _wan_vec(weight if affine else scale, C, "weight" if affine else "scale")
-    vb = _wan_vec(bias if affine else shift, C, "bias" if affine else "shift")
-    g = _wan_vec(gate, C, "gate") if gate is not None else None
+    C = x.shape[-1]
+    v = _wan_vecs(x, {"gate": gate, "scale": scale, "shift": shift})
+    if affine:                                  # norm3's parameters: one row for every sample
+        v.update(_wan_vecs(x[:1], {"weight": weight, "bias": bias}))
+    n, rows, xs, xb, ys, yb = _wan_samples(x, y)
+    _require_cuda(x, y)
+    va = _wan_vec(v["weight"] if affine else v["scale"], "weight" if affine else "scale")
+    vb = _wan_vec(v["bias"] if affine else v["shift"], "bias" if affine else "shift")
+    g = _wan_vec(v["gate"], "gate")
     res = torch.empty(x.shape, dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        if fp8:
-            out, a_scale = _fp8_rows(rows, C, x.device)
-            check(lib.jenga_wan_residual_ln_fp8(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys,
-                                                g.data_ptr() if g is not None else None, res.data_ptr(), C,
-                                                va.data_ptr(), vb.data_ptr(), int(affine), out.data_ptr(), C,
-                                                a_scale.data_ptr(), rows, C, float(eps), _stream_ptr(x.device)),
-                  "wan_residual_ln_fp8")
-            return res, (out, a_scale)
+    if fp8:
+        out, a_scale = _fp8_rows(n * rows, C, x.device)
+    else:
         out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-        check(lib.jenga_wan_residual_ln(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys,
-                                        g.data_ptr() if g is not None else None, res.data_ptr(), C, va.data_ptr(),
-                                        vb.data_ptr(), int(affine), out.data_ptr(), C, rows, C, float(eps),
-                                        _stream_ptr(x.device)), "wan_residual_ln")
-    return res, out
+    with torch.cuda.device(x.device):
+        for b in range(n):
+            xp, yp, rp, op = _at(x, b * xb), _at(y, b * yb), _at(res, b * rows * C), _at(out, b * rows * C)
+            gp = _vec_ptr(g, b) if g is not None else None
+            if fp8:
+                check(lib.jenga_wan_residual_ln_fp8(xp, _x_code(x), xs, yp, ys, gp, rp, C, _vec_ptr(va, b),
+                                                    _vec_ptr(vb, b), int(affine), op, C, _at(a_scale, b * rows),
+                                                    rows, C, float(eps), _stream_ptr(x.device)),
+                      "wan_residual_ln_fp8")
+            else:
+                check(lib.jenga_wan_residual_ln(xp, _x_code(x), xs, yp, ys, gp, rp, C, _vec_ptr(va, b),
+                                                _vec_ptr(vb, b), int(affine), op, C, rows, C, float(eps),
+                                                _stream_ptr(x.device)), "wan_residual_ln")
+    return (res, (out, a_scale)) if fp8 else (res, out)
 
 
 def wan_gate_residual(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
-    """`x + y * gate` under autocast(float32) (gate 2, model_mul.py:341-342): x [1, L, C] bf16 or fp32,
-    y bf16 like x, gate fp32 with C values (e[5]) -> fp32 [1, L, C]."""
-    _require_cuda(x)
-    rows, xs = _rows2d(x)
-    ys = _wan_y(x, y)
+    """`x + y * gate` under autocast(float32) (gate 2, model_mul.py:341-342): x [B, L, C] bf16 or fp32,
+    y bf16 like x, gate fp32 with C values (e[5]) or one row of them per sample -> fp32 [B, L, C]."""
+    v = _wan_vecs(x, {"gate": gate})
+    n, rows, xs, xb, ys, yb = _wan_samples(x, y)
+    _require_cuda(x, y)
     C = x.shape[-1]
-    g = _wan_vec(gate, C, "gate")
+    g = _wan_vec(v["gate"], "gate")
     out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        check(lib.jenga_wan_gate_residual(x.data_ptr(), _x_code(x), xs, y.data_ptr(), ys, g.data_ptr(), out.data_ptr(),
-                                          C, rows, C, _stream_ptr(x.device)), "wan_gate_residual")
+        for b in range(n):
+            check(lib.jenga_wan_gate_residual(_at(x, b * xb), _x_code(x), xs, _at(y, b * yb), ys, _vec_ptr(g, b),
+                                              _at(out, b * rows * C), C, rows, C, _stream_ptr(x.device)),
+                  "wan_gate_residual")
     return out
 
 

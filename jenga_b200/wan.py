@@ -105,9 +105,10 @@ def self_attention(q_lin, k_lin, v, norm_q_w, norm_k_w, heads, grid_size, freqs,
 
 
 def cross_attention(q_lin, k_lin, v, norm_q_w, norm_k_w, heads, eps=1e-6):
-    """WanT2VCrossAttention.forward's attention part (model_mul.py:195-200) for one sample with every
-    context row valid (context_lens=None): q_lin [1, L, C] = self.q(x), k_lin [1, Lc, C] = self.k(context),
-    v [1, Lc, H, 128] = self.v(context) bf16.  Returns [1, L, H, 128] bf16.
+    """WanT2VCrossAttention.forward's attention part (model_mul.py:195-200) with every context row valid
+    (context_lens=None): q_lin [B, L, C] = self.q(x), k_lin [B, Lc, C] = self.k(context),
+    v [B, Lc, H, 128] = self.v(context) bf16, sample b attending its own Lc context rows.
+    Returns [B, L, H, 128] bf16.
 
     q and k go through the norm-only prologue, `bf16(bf16(norm(x)) * w)` — what flash_attention's
     half() makes of norm_q(self.q(x)) (wan/modules/attention.py:59-83) — and the dense class of the
@@ -116,8 +117,10 @@ def cross_attention(q_lin, k_lin, v, norm_q_w, norm_k_w, heads, eps=1e-6):
     autocast: the bf16 result here is what self.o sees.  No segment table, no host sync."""
     q = norm_rope(q_lin, norm_q_w, heads, None, None, eps=eps)
     k = norm_rope(k_lin, norm_k_w, heads, None, None, eps=eps)
+    if k.shape[0] != q.shape[0]:
+        raise ValueError("q_lin and k_lin must hold one batch")
     if v.dtype != torch.bfloat16 or v.shape != k.shape or v.stride(3) != 1:
-        raise ValueError("v must be bf16 [1, Lc, heads, 128] with contiguous channels")
+        raise ValueError("v must be bf16 [B, Lc, heads, 128] with contiguous channels")
     _, L, _, D = q.shape
     Lc = k.shape[1]
     out = torch.empty_like(q)
@@ -157,10 +160,11 @@ def i2v_cross_attn(q, k_img, v_img, k_txt, v_txt, sm_scale=None, out=None):
 
 
 def i2v_cross_attention(q_lin, k_lin, v, kimg_lin, vimg, wq, wk, wk_img, heads, eps=1e-6):
-    """WanI2VCrossAttention.forward's attention part (model_mul.py:230-247) for one sample with every
-    context row valid: q_lin [1, L, C] = self.q(x); k_lin [1, Lt, C] = self.k(context[:, 257:]) and
-    v [1, Lt, H, 128] = self.v(…) bf16; kimg_lin [1, Li, C] = self.k_img(context[:, :257]) and
-    vimg [1, Li, H, 128] = self.v_img(…) bf16.  Returns [1, L, H, 128] bf16: what self.o receives.
+    """WanI2VCrossAttention.forward's attention part (model_mul.py:230-247) with every context row valid:
+    q_lin [B, L, C] = self.q(x); k_lin [B, Lt, C] = self.k(context[:, 257:]) and v [B, Lt, H, 128] =
+    self.v(…) bf16; kimg_lin [B, Li, C] = self.k_img(context[:, :257]) and vimg [B, Li, H, 128] =
+    self.v_img(…) bf16; sample b attends its own context rows.  Returns [B, L, H, 128] bf16: what self.o
+    receives.
 
     q, k and k_img go through the norm-only prologue, as in cross_attention; one launch then computes
     both attentions and their sum, `x + img_x` in fp32 (:247) of the two fp32-typed flash_attention
@@ -169,5 +173,5 @@ def i2v_cross_attention(q_lin, k_lin, v, kimg_lin, vimg, wq, wk, wk_img, heads, 
     k = norm_rope(k_lin, wk, heads, None, None, eps=eps)
     ki = norm_rope(kimg_lin, wk_img, heads, None, None, eps=eps)
     if v.dtype != torch.bfloat16 or v.shape != k.shape or vimg.dtype != torch.bfloat16 or vimg.shape != ki.shape:
-        raise ValueError("v / vimg must be bf16 [1, Lt / Li, heads, 128] like the projected keys")
+        raise ValueError("v / vimg must be bf16 [B, Lt / Li, heads, 128] like the projected keys")
     return i2v_cross_attn(q, ki, vimg, k, v)

@@ -12,8 +12,13 @@ Hilbert order:
   zero-padded to n rows; `freq_remap` is the same slice of hilbert_order -> TeaCache decision (rank
   0's rel-L1 value, broadcast) -> blocks, whose self-attention (blocks._wan_self) routes through
   `block.self_attn.jenga_sp`, a Ulysses object, over the first L exchanged rows -> head on the rank's
-  rows -> one all_gather of the [1, n, out_dim] rows in rank order -> [:L], inverse Hilbert scatter,
+  rows -> one all_gather of the [B, n, out_dim] rows in rank order -> [:L], inverse Hilbert scatter,
   unpatchify.
+
+Every forward here takes several videos per call (x a list of B videos of one latent grid, each with its
+own text context, t [B] or [1]): the samples are stacked into [B, L, C] as teacache_forward stacks them,
+every sample takes the same rank rows, and on a computed step each sample gets what it would get alone.
+The TeaCache decision stays one per call, taken over the whole batch as in the reference.
 
 The result is the single-GPU Jenga Wan forward's: the same selection over the global L, the same
 dense warm-up steps, the same TeaCache decisions.  Only the Linears run on a rank's rows.
@@ -167,10 +172,15 @@ def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of,
     block_neighbor_list) or None: rank r takes the curve's rows [r*n, min((r+1)*n, L)) and `freq_remap`
     is that slice, or, without a curve, the raster rows.  block_kw: what the blocks get besides the
     arguments of model.py's WanAttentionBlock.forward (with a curve, also freq_remap and
-    block_neighbor_list).  group LOCAL: one GPU, no exchange."""
+    block_neighbor_list).  group LOCAL: one GPU, no exchange.
+
+    x is a list of B videos, stacked into [B, L, C] rows as teacache_forward stacks them (jenga_wan.py:
+    550-559); every sample takes the same rows (one curve, one latent grid), each attends its own text
+    (and CLIP) context, and t holds one timestep per video or one for all.  The TeaCache decision is one
+    per call, over the whole batch, as in the reference.  _check_batch raises on anything else before any
+    launch or collective."""
     P, r = world(group)
-    if len(x) != 1:
-        raise ValueError(f"{_route(group)}{MODEL} runs batch 1, got {len(x)} videos")
+    _check_batch(self, group, x, t, context, clip_fea, y)
     device = self.patch_embedding.weight.device
     if self.freqs.device != device:
         self.freqs = self.freqs.to(device)
@@ -182,7 +192,7 @@ def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of,
     x = [u.flatten(2).transpose(1, 2) for u in x]
     seq_lens = torch.tensor([u.size(1) for u in x], dtype=torch.long)
     assert seq_lens.max() <= seq_len
-    x = x[0]
+    x = x[0] if len(x) == 1 else torch.cat(x)                                # [B, L, C]
     # rows past L (the reference's zero pad to seq_len, which the Hilbert gather drops again,
     # jenga_wan.py:554-559) are neither attended nor returned
     L = int(seq_lens[0])
@@ -198,7 +208,7 @@ def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of,
                              f"of {L} tokens (curve and grid out of step)")
         n, real = shard_rows(L, P, r)
         rows = shard(order.to(torch.long), 0, P, r)          # pad entries point at row 0 (any valid row)
-        x = x[:, rows.to(x.device)]
+        x = x[:, rows.to(x.device)]                          # the same rows of every sample
         if real < n:
             x[:, real:] = 0
         kwargs.update(freq_remap=rows.to(device), block_neighbor_list=curve[2])
@@ -207,7 +217,7 @@ def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of,
                   context_lens=None)
     x = _teacache(self, x, e, e0, lambda x: _blocks(self, x, kwargs), group)
     # head on the rank's rows (row-local, as usp_dit_forward runs it before its gather), then the
-    # [1, n, out] rows of every rank in rank order
+    # [B, n, out] rows of every rank in rank order
     x = gather_rows(self.head(x, e), L, P, group)
     if curve is not None:
         x = x[:, curve[1]]                                                    # :655
@@ -217,6 +227,30 @@ def _sharded_forward(self, group, x, t, context, seq_len, clip_fea, y, curve_of,
         if self.cnt >= self.num_steps:
             self.cnt = 0
     return [u.float() for u in x]
+
+
+def _check_batch(self, group, x, t, context, clip_fea, y) -> None:
+    """The batch rules of _sharded_forward, checked on shapes alone: one text context per video (and one
+    CLIP feature row and one y per video for I2V), t with one timestep per video or one for all, and every
+    video of one latent grid"""
+    what = f"{_route(group)}{MODEL}"
+    B = len(x)
+    if B < 1:
+        raise ValueError(f"{what}: no videos")
+    if len(context) != B:
+        raise ValueError(f"{what} with {len(context)} text context(s) runs batch {len(context)}, got {B} videos; "
+                         "each video needs its own context")
+    if not isinstance(t, torch.Tensor) or t.numel() not in (1, B):
+        raise ValueError(f"{what}: t must hold one timestep per video ({B}) or one for all")
+    if clip_fea is not None and clip_fea.shape[0] != B:
+        raise ValueError(f"{what}: clip_fea holds {clip_fea.shape[0]} samples for {B} videos")
+    if y is not None and len(y) != B:
+        raise ValueError(f"{what}: y holds {len(y)} conditions for {B} videos")
+    # the patch embedding is a Conv3d whose stride is its kernel: a grid is each dim // patch size
+    grids = {tuple(d // p for d, p in zip(u.shape[1:], self.patch_size)) for u in x}
+    if len(grids) != 1:
+        raise ValueError(f"{what}: the videos of one call must share one latent grid (one curve and one RoPE grid "
+                         f"for all); got grids {sorted(grids)}")
 
 
 def _blocks(self, x, kwargs):
