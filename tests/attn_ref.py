@@ -12,6 +12,11 @@ Two legs:
   round16(fp32(num) * fp32(1 / l)) with num and l formed exactly here.
 - fp64_rows / elem_bound: realistic inputs against fp64, with a per-element bound derived from the
   kernel's rounding points.
+
+The dense launches outside the carved path (the FlashAttention shims, the Wan T2V cross-attention and
+the two-segment Wan I2V kernel, jenga_b200/csrc/wan_cross_attn.cu) reuse both legs: dense_expected
+and segments_expected state a dense-only launch and a varlen call, i2v_expected / i2v_bound the I2V
+sum, and fp8_case / fp8_expected the FP8 P.V epilogue on V values whose e4m3 codes are exact.
 """
 from __future__ import annotations
 
@@ -287,3 +292,132 @@ def elem_bound(ref: dict, dtype: torch.dtype):
     e_lse = (1 + 2.0 ** -10) * (rel_l / (1 - rel_l) + math.log(2.0) * 2.0 ** -22 * 32
                                 + 3 * U32 * (lse.abs() + 32 * math.log(2.0)))
     return E, e_lse
+
+
+# ------------------------------------------------------------------------------------------------
+# Dense launches: varlen segments, the Wan I2V cross-attention, FP8 P.V
+# ------------------------------------------------------------------------------------------------
+LSE_RTOL = 2.0 ** -20                # Leg A LSE ln(keys): one fp32 log2f and one product with ln 2
+
+
+def dense_expected(v: torch.Tensor, q_rows: int, *, kv_limit: int | None = None,
+                   out_dtype: torch.dtype | None = None) -> torch.Tensor:
+    """Leg A output [B, q_rows, H, D] of one dense-only launch (nq_sparse = 0) over v's Sk keys with the
+    column limit kv_limit (default Sk, what the shims and cross-attentions pass): every query block
+    walks all ceil(Sk / 128) key tiles, and only the limit keeps the zero-filled keys of the last one
+    out of l."""
+    Sk = v.shape[1]
+    return flat_expected(v, None, nq_sparse=0, nq_dense=(q_rows + BLOCK - 1) // BLOCK, q_rows=q_rows,
+                         kv_limit_dense=Sk if kv_limit is None else kv_limit, out_dtype=out_dtype)
+
+
+def segments_expected(v: torch.Tensor, cu_q, cu_k, q_total: int, one=dense_expected) -> torch.Tensor:
+    """Expected output [q_total, H, D] of flash_attn_varlen_func on packed v [(total keys), H, D]:
+    segment i's rows cu_q[i]:cu_q[i+1] hold one(v[cu_k[i]:cu_k[i+1]][None], rows)[0], the expectation
+    of one dense launch over that segment's keys alone; segments with no keys (and rows no segment
+    covers) are zeros."""
+    out = torch.zeros(q_total, *v.shape[1:], dtype=v.dtype, device=v.device)
+    for i in range(len(cu_q) - 1):
+        q0, q1, k0, k1 = int(cu_q[i]), int(cu_q[i + 1]), int(cu_k[i]), int(cu_k[i + 1])
+        if q1 > q0 and k1 > k0:
+            out[q0:q1] = one(v[k0:k1][None], q1 - q0)[0]
+    return out
+
+
+def i2v_expected(v_img: torch.Tensor, v_txt: torch.Tensor, q_rows: int) -> torch.Tensor:
+    """Leg A output of wan.i2v_cross_attn: round16(f32(A_img) + f32(A_txt)), each A the dense expectation
+    of its own segment's keys (each segment's column limit is its own row count)."""
+    a_img = dense_expected(v_img, q_rows).float()
+    a_txt = dense_expected(v_txt, q_rows).float()
+    return (a_img + a_txt).to(v_img.dtype)
+
+
+def i2v_bound(ref_img: dict, ref_txt: dict):
+    """(O* [R, D], E [R, D]) for wan.i2v_cross_attn on the rows of fp64_rows over the image keys (ref_img)
+    and over the text keys (ref_txt), both dense with kv_limit_dense = the segment's row count.
+
+    The kernel runs each segment through the dense consumer loop and rounds each result to bf16 as the
+    dense epilogue does, so |A_seg - O*_seg| <= E_seg = elem_bound(ref_seg) (round16 included).  Then
+    s = f32(A_img) + f32(A_txt) is one fp32 add (relative u32) and out = round16(s) one more rounding
+    (relative u16).  With S* = O*_img + O*_txt, |A_img + A_txt - S*| <= E_img + E_txt and
+    |A_img + A_txt| <= |S*| + E_img + E_txt, so
+      |out - S*| <= E_img + E_txt + (u16 + 2 u32) (|S*| + E_img + E_txt),
+    the second term covering (1 + u32)(1 + u16) - 1 < u16 + 2 u32 of the two roundings."""
+    E_i, _ = elem_bound(ref_img, torch.bfloat16)
+    E_t, _ = elem_bound(ref_txt, torch.bfloat16)
+    o = ref_img["o"] + ref_txt["o"]
+    return o, E_i + E_t + (2.0 ** -8 + 2 * U32) * (o.abs() + E_i + E_t)
+
+
+E4M3_MAX = 448.0
+FP8_CERT_BITS = 12                   # the FP8 wgmma's accumulator is narrower than fp32 (linear_fp8.cu)
+
+
+def fp8_case(B: int, S: int, H: int, *, seed: int, device, amax=None, nnz: int = 16):
+    """q = 0, k ~ N(0, 1), and a sparse v for the FP8 P.V leg: in every (sample, head, channel) nnz keys
+    drawn at random hold +-2^e, e in 0..log2(amax[b]), the rest 0, and one key of every (sample, head)
+    holds +-amax[b] (default 8 in every sample), so the head's amax is amax[b] and fp8.cu's
+    e4m3(v * 448 / amax) is exact.  [B, S, H, D] bf16."""
+    amax = [V_MAX] * B if amax is None else list(amax)
+    g = torch.Generator(device=device).manual_seed(seed)
+    q = torch.zeros(B, S, H, D, dtype=torch.bfloat16, device=device)
+    k = torch.randn(B, S, H, D, generator=g, device=device).to(torch.bfloat16)
+    v = torch.zeros(B, S, H, D, dtype=torch.float32, device=device)
+    for b in range(B):
+        e_max = int(math.log2(amax[b]))
+        assert 2 ** e_max == amax[b]
+        idx = torch.randint(0, S, (nnz, H, D), generator=g, device=device)
+        mag = 2.0 ** torch.randint(0, e_max + 1, (nnz, H, D), generator=g, device=device)
+        sign = torch.randint(0, 2, (nnz, H, D), generator=g, device=device) * 2 - 1
+        v[b].scatter_(0, idx, mag * sign)
+        at = torch.randint(0, S, (H,), generator=g, device=device)
+        v[b, at, torch.arange(H, device=device), 0] = float(amax[b])
+    return q, k, v.to(torch.bfloat16)
+
+
+def fp8_codes(v: torch.Tensor):
+    """(codes [B, S, H, D] fp32, amax [B, H] fp32) of fp8.cu: amax = max |v| of the (sample, head),
+    codes the e4m3 values of satfinite(v * fp32(448 / amax)) (scale 1 where amax is 0)."""
+    from test_producers_cpu import e4m3_satfinite
+    amax = v.float().abs().amax(dim=(1, 3))                                     # [B, H]
+    inv = torch.where(amax > 0, torch.tensor(E4M3_MAX, device=v.device) / amax, torch.ones_like(amax))
+    codes = e4m3_satfinite(v.float() * inv[:, None, :, None]).view(torch.float8_e4m3fn).float()
+    return codes, amax
+
+
+def fp8_cert_ratio(codes: torch.Tensor, kv_limit: int | None = None) -> float:
+    """Largest |partial sum| of a flat FP8 row over its granularity: with every p = 1 (exact in e4m3) a
+    partial sum of channel d is at most sum |code| over the keys, and every code is a multiple of the
+    lowest power of two among the channel's codes (the codes here are integers)."""
+    c = codes[:, :kv_limit].double()
+    ci = c.abs().long()
+    low = torch.where(ci > 0, ci & -ci, torch.full_like(ci, 1 << 40)).amin(1).double().clamp_max(2.0 ** 40)
+    tot = c.abs().sum(1)
+    return float(torch.where(tot > 0, tot / low, torch.zeros_like(tot)).max())
+
+
+def fp8_certified(codes: torch.Tensor, kv_limit: int | None = None) -> bool:
+    """True when every partial sum stays within 2^12 units of its granularity: deliberately
+    conservative, since Hopper's FP8 wgmma accumulates in fewer bits than fp32."""
+    return fp8_cert_ratio(codes, kv_limit) <= 2.0 ** FP8_CERT_BITS
+
+
+def fp8_expected(v: torch.Tensor, q_rows: int, *, kv_limit: int | None = None) -> torch.Tensor:
+    """Leg A output [B, q_rows, H, D] of one dense-only FP8 P.V launch on v quantised by fp8.cu (one
+    amax per (sample, head) of this launch's v), q = 0: num8 = sum of the codes below the column limit
+    (exact when fp8_certified), l the number of those keys, and the epilogue of carved_attn.cu
+    restated in its order:
+      inv_l = fp32(1 / l);  inv_l = fp32(inv_l * fp32(amax * fp32(1 / 448)));  out = round16(fp32(num8) * inv_l)."""
+    B, Sk, H, _ = v.shape
+    kvl = Sk if kv_limit is None else kv_limit
+    codes, amax = fp8_codes(v)
+    assert fp8_certified(codes, kvl), "FP8 partial sums past the certificate"
+    num8 = codes[:, :kvl].double().sum(1)                                       # [B, H, D]
+    n32 = num8.float()
+    assert torch.equal(n32.double(), num8)
+    l = min(kvl, (Sk + BLOCK - 1) // BLOCK * BLOCK)                             # keys that score p = 1
+    inv_l = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(float(l), dtype=torch.float32)
+    unscale = amax * torch.tensor(1.0 / E4M3_MAX, dtype=torch.float32).item()  # fp32(amax * fp32(1/448))
+    inv = (inv_l.to(v.device) * unscale).float()                                # [B, H]
+    o = (n32 * inv[..., None]).to(v.dtype)                                      # [B, H, D]
+    return o[:, None].expand(B, q_rows, H, D).contiguous()
